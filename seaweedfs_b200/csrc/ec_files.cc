@@ -11,7 +11,6 @@
 // column-wise), so buffer_size is only validated the way the reference does.
 #include <errno.h>
 #include <fcntl.h>
-#include <libgen.h>
 #include <linux/falloc.h>
 #include <sys/stat.h>
 #include <sys/vfs.h>
@@ -30,7 +29,7 @@
 
 #include "engine.h"
 #include "io_pool.h"
-#include "mini_json.h"
+#include "volume_format.h"
 
 namespace swec {
 namespace {
@@ -42,12 +41,6 @@ size_t env_sz(const char* name, size_t dflt) {
 }
 
 int io_fail(const std::string& what) { return fail(SWEC_ERR_IO, what + ": " + strerror(errno)); }
-
-std::string shard_ext(int idx) {  // ToExt, ec_encoder.go:106-108
-    char b[16];
-    snprintf(b, sizeof b, ".ec%02d", idx);
-    return b;
-}
 
 // Reserving extents pays on disk filesystems (once instead of 14 files growing 8 MiB at a time) and costs on tmpfs,
 // where it zero-fills every page that the writers overwrite a moment later.  The reservation must NOT change the
@@ -508,35 +501,6 @@ class FilePipeline {
 
 }  // namespace
 
-// .vif is protobuf-JSON (weed/storage/volume_info/volume_info.go:73-95); we only need
-// ecShardConfig.{dataShards,parityShards} (weed/pb/volume_server.proto:561-577).
-bool read_vif_ratio(const std::string& path, int* ds, int* ps) {
-    FILE* f = fopen(path.c_str(), "rb");
-    if (!f) return false;
-    std::string txt;
-    char buf[4096];
-    size_t n;
-    while ((n = fread(buf, 1, sizeof buf, f)) > 0) txt.append(buf, n);
-    fclose(f);
-    int64_t a = 0, b = 0;
-    if (!mini_json::nested_int(txt, "ecShardConfig", "ec_shard_config", "dataShards", "data_shards", &a) ||
-        !mini_json::nested_int(txt, "ecShardConfig", "ec_shard_config", "parityShards", "parity_shards", &b))
-        return false;
-    if (a < 0 || b < 0 || a > 255 || b > 255) return false;
-    *ds = int(a);
-    *ps = int(b);
-    return true;
-}
-
-namespace {
-
-bool file_exists(const std::string& p) {
-    struct stat st;
-    return stat(p.c_str(), &st) == 0 && !S_ISDIR(st.st_mode);
-}
-
-}  // namespace
-
 void file_pipeline_trim() {  // swec_shutdown(): release parked staging rings
     std::vector<SlotSet> sets;
     {
@@ -611,9 +575,10 @@ int swec_generate_ec_files(const char* base, int64_t buffer_size, int64_t large,
     // The final shard size is known up front: reserve its extents (visible length unchanged) — one I/O thread per
     // file — so the writers fill pages/extents that already exist instead of
     // growing 14 files 8 MiB at a time under the filesystem's allocation lock (best effort).
+    const StripeGeometry g(st.st_size, k, large, small);
     if (worth_preallocating(outs[0])) {
         const double tp = PipeStats::now();
-        const int64_t shard_size = swec_expected_shard_size(st.st_size, k, large, small);
+        const int64_t shard_size = g.shard_size();
         if (shard_size > 0)
             pipe.parallel_for(total, [&](int i) -> int {
                 reserve_extents(outs[size_t(i)], shard_size);
@@ -622,8 +587,7 @@ int swec_generate_ec_files(const char* base, int64_t buffer_size, int64_t large,
         pipe.stats.prealloc += PipeStats::now() - tp;
     }
 
-    int64_t remaining = st.st_size, processed = 0, shard_off = 0;
-    const int64_t large_row = large * k, small_row = small * k;
+    int64_t processed = 0, shard_off = 0;
     auto encode_row = [&](int64_t block) -> int {  // encodeData on one row of k blocks, chunk by chunk
         for (int64_t o = 0; o < block; o += int64_t(chunk)) {
             Item it;
@@ -633,37 +597,32 @@ int swec_generate_ec_files(const char* base, int64_t buffer_size, int64_t large,
             const int r = pipe.submit(std::move(it));
             if (r) return r;
         }
+        processed += block * k;
         shard_off += block;
         return SWEC_OK;
     };
-    while (rc == SWEC_OK && remaining >= large_row) {  // ec_encoder.go:304-311
-        rc = encode_row(large);
-        remaining -= large_row;
-        processed += large_row;
-    }
-    while (rc == SWEC_OK && remaining > 0 && small > int64_t(chunk)) {  // small blocks bigger than a slot: row by row
+    for (int64_t r = 0; rc == SWEC_OK && r < g.large_rows; r++) rc = encode_row(large);  // ec_encoder.go:304-311
+    // the small rows (ec_encoder.go:312-319); the tail row is read as a whole row, zero past EOF (ec_encoder.go:258-262)
+    int64_t rows_left = g.small_rows + (g.tail > 0 ? 1 : 0);
+    for (; rc == SWEC_OK && rows_left > 0 && small > int64_t(chunk); rows_left--)  // small blocks bigger than a slot: row by row
         rc = encode_row(small);
-        remaining -= small_row;
-        processed += small_row;
-    }
-    // Small rows (ec_encoder.go:312-319) are tiny (10 x 1 MiB): many of them share one slot.  Row j of the
+    // Small rows are tiny (10 x 1 MiB): many of them share one slot.  Row j of the
     // batch is one contiguous k*small run of the .dat whose k blocks scatter to offset j*small of the k input
     // streams, so every shard still receives ONE contiguous write per item.  A default 30,000 MiB volume is
     // 2 large rows + 952 small ones — a third of its bytes take this path.
     const int64_t rows_per_item = std::max<int64_t>(1, int64_t(chunk) / small);
-    while (rc == SWEC_OK && remaining > 0) {
-        const int64_t rows_left = (remaining + small_row - 1) / small_row;
+    while (rc == SWEC_OK && rows_left > 0) {
         const int64_t n = std::min(rows_per_item, rows_left);
         Item it;
         it.len = size_t(n * small);
         for (int64_t j = 0; j < n; j++)
             for (int i = 0; i < k; i++)
-                it.reads.push_back({i, dat, processed + j * small_row + int64_t(i) * small, size_t(j * small), size_t(small), dat_d});
+                it.reads.push_back({i, dat, processed + j * g.small_row() + int64_t(i) * small, size_t(j * small), size_t(small), dat_d});
         for (int i = 0; i < total; i++) it.writes.push_back({i, outs[size_t(i)], shard_off, outs_d[size_t(i)]});
         rc = pipe.submit(std::move(it));
         shard_off += n * small;
-        remaining -= n * small_row;
-        processed += n * small_row;
+        processed += n * g.small_row();
+        rows_left -= n;
     }
     const int rc2 = pipe.finish();
     if (rc == SWEC_OK) rc = rc2;
@@ -680,8 +639,8 @@ int swec_generate_ec_files(const char* base, int64_t buffer_size, int64_t large,
 }
 
 int swec_write_ec_files(const char* base, int device) {
-    // WriteEcFilesWithContext: 256 KiB buffers, 1 GiB / 1 MiB blocks, 10+4 (ec_encoder.go:61-69)
-    return swec_generate_ec_files(base, 256 * 1024, int64_t(1) << 30, int64_t(1) << 20, 10, 4, device);
+    return swec_generate_ec_files(base, kBufferSize, kLargeBlockSize, kSmallBlockSize, kDefaultDataShards,
+                                  kDefaultParityShards, device);
 }
 
 int swec_rebuild_ec_files(const char* base, const char* const* dirs, int ndirs, int k, int m, int device,
@@ -689,25 +648,14 @@ int swec_rebuild_ec_files(const char* base, const char* const* dirs, int ndirs, 
     if (!base || !rebuilt || !n_rebuilt || (ndirs > 0 && !dirs)) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
     *n_rebuilt = 0;
     const std::string b(base);
-    if (k == 0) {  // RebuildEcFiles: ratio from .vif when valid, else default (ec_encoder.go:76-95)
-        int ds = 0, ps = 0;
-        if (read_vif_ratio(b + ".vif", &ds, &ps) && ds > 0 && ps > 0 && ds + ps <= SWEC_MAX_SHARDS) {
-            k = ds;
-            m = ps;
-        } else {
-            k = 10;
-            m = 4;
-        }
-    }
+    if (k == 0) ec_ratio(b, &k, &m);  // RebuildEcFiles (ec_encoder.go:76-95)
     swec_encoder* enc = nullptr;
     int rc = swec_encoder_new(k, m, device, &enc);
     if (rc) return rc;
     std::unique_ptr<swec_encoder, void (*)(swec_encoder*)> guard(enc, swec_encoder_free);
     const int total = k + m;
 
-    // pass 1: which shards exist (base dir first, then additionalDirs) — ec_encoder.go:131-169
-    std::string base_copy(b);
-    const std::string base_name = basename(&base_copy[0]);
+    // pass 1: which shards exist
     FdSet fds;
     const long direct = g_opt_file_direct_io.load();
     std::vector<int> in(static_cast<size_t>(total), -1), in_d(static_cast<size_t>(total), -1), out_d(static_cast<size_t>(total), -1);
@@ -715,17 +663,7 @@ int swec_rebuild_ec_files(const char* base, const char* const* dirs, int ndirs, 
     int npresent = 0;
     std::vector<uint32_t> missing;
     for (int i = 0; i < total; i++) {
-        std::string path = b + shard_ext(i);
-        if (!file_exists(path)) {
-            path.clear();
-            for (int d = 0; d < ndirs; d++) {
-                const std::string cand = std::string(dirs[d]) + "/" + base_name + shard_ext(i);
-                if (file_exists(cand)) {
-                    path = cand;
-                    break;
-                }
-            }
-        }
+        const std::string path = find_shard_file(b, dirs, ndirs, i);
         if (path.empty()) {
             missing.push_back(uint32_t(i));
             continue;
@@ -782,8 +720,9 @@ int swec_rebuild_ec_files(const char* base, const char* const* dirs, int ndirs, 
         else if (size != st.st_size)
             return fail(SWEC_ERR_SHARD_SIZE, "ec shard size expected " + std::to_string(size) + " actual " + std::to_string(st.st_size));
     }
-    const int64_t mib = int64_t(1) << 20;
-    // quirk kept: a length above 1 MiB that is not a multiple of 1 MiB errors on the last read
+    // quirk kept: the reference reads in small-block buffers, and a length above 1 MiB that is not a multiple of
+    // 1 MiB errors on the last read
+    const int64_t mib = kSmallBlockSize;
     const bool ragged = size > mib && size % mib != 0;
     const int64_t todo = ragged ? size / mib * mib : size;
 
@@ -825,30 +764,17 @@ int swec_verify_ec_files(const char* base, const char* const* dirs, int ndirs, i
     if (!base || !ok || (ndirs > 0 && !dirs)) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
     *ok = 0;
     const std::string b(base);
-    if (k == 0) {
-        int ds = 0, ps = 0;
-        if (read_vif_ratio(b + ".vif", &ds, &ps) && ds > 0 && ps > 0 && ds + ps <= SWEC_MAX_SHARDS) { k = ds; m = ps; }
-        else { k = 10; m = 4; }
-    }
+    if (k == 0) ec_ratio(b, &k, &m);
     swec_encoder* enc = nullptr;
     int rc = swec_encoder_new(k, m, device, &enc);
     if (rc) return rc;
     std::unique_ptr<swec_encoder, void (*)(swec_encoder*)> guard(enc, swec_encoder_free);
     const int total = k + m;
-    std::string base_copy(b);
-    const std::string base_name = basename(&base_copy[0]);
     FdSet fds;
     std::vector<int> in(static_cast<size_t>(total), -1);
     int64_t size = -1;
     for (int i = 0; i < total; i++) {  // verify needs every shard (verify_ec_shards, ec_encoder.rs:177-278)
-        std::string path = b + shard_ext(i);
-        if (!file_exists(path)) {
-            path.clear();
-            for (int d = 0; d < ndirs; d++) {
-                const std::string cand = std::string(dirs[d]) + "/" + base_name + shard_ext(i);
-                if (file_exists(cand)) { path = cand; break; }
-            }
-        }
+        const std::string path = find_shard_file(b, dirs, ndirs, i);
         if (path.empty()) return fail(SWEC_ERR_TOO_FEW_SHARDS, "verify needs all shards; missing " + shard_ext(i));
         const int fd = open(path.c_str(), O_RDONLY);
         if (fd < 0) return io_fail("open " + path);
@@ -912,24 +838,20 @@ int swec_write_dat_file(const char* base, int64_t dat_size, const char* const* s
     std::vector<Piece> pieces;
     const int64_t max_piece = int64_t(8) << 20;
     std::vector<int64_t> pos(static_cast<size_t>(k), 0);
-    int64_t out = 0, remaining = dat_size;
+    int64_t out = 0;
     auto plan = [&](int shard, int64_t n) {  // io.CopyN(datFile, inputFiles[shard], n)
         for (int64_t o = 0; o < n; o += max_piece)
             pieces.push_back({shard, pos[size_t(shard)] + o, out + o, std::min(max_piece, n - o)});
         pos[size_t(shard)] += n;
         out += n;
     };
-    while (remaining >= int64_t(k) * large)
-        for (int s = 0; s < k; s++) {
-            plan(s, large);
-            remaining -= large;
-        }
-    while (remaining > 0)
-        for (int s = 0; s < k; s++) {
-            const int64_t n = std::min(remaining, small);
-            plan(s, n);
-            remaining -= n;
-        }
+    const StripeGeometry g(dat_size, k, large, small);
+    for (int64_t r = 0; r < g.large_rows; r++)
+        for (int s = 0; s < k; s++) plan(s, large);
+    for (int64_t r = 0; r < g.small_rows; r++)
+        for (int s = 0; s < k; s++) plan(s, small);
+    for (int s = 0; s < k; s++)  // the last row: min(remaining, small) each; shards past the end get nothing
+        if (const int64_t n = g.tail_bytes(s)) plan(s, n);
     // a shard shorter than the plan needs is the reference's "copy … block" error: check before writing anything
     for (int s2 = 0; s2 < k; s2++) {
         struct stat st;
@@ -980,52 +902,6 @@ int swec_write_dat_file(const char* base, int64_t dat_size, const char* const* s
     const int rc = pool.parallel_for(int(pieces.size()), copy_piece);
     if (rc) return fail(rc, err_text);
     return SWEC_OK;
-}
-
-// ---- layout arithmetic -----------------------------------------------------------------------
-
-int swec_locate_data(int64_t large, int64_t small, int64_t shard_dat_size, int64_t offset, int64_t size, int k,
-                     swec_interval* out, int cap) {
-    if (large <= 0 || small <= 0 || k <= 0 || !out) return fail(SWEC_ERR_INVALID_ARG, "bad argument");
-    const int64_t nlarge_rows = shard_dat_size / large;  // ec_locate.go:67
-    const int64_t large_area = nlarge_rows * large * k;
-    bool is_large = offset < large_area;
-    const int64_t rel = is_large ? offset : offset - large_area;
-    const int64_t blk = is_large ? large : small;
-    int64_t block_index = rel / blk, inner = rel % blk;
-    int n = 0;
-    while (size > 0) {
-        const int64_t room = (is_large ? large : small) - inner;
-        if (room > 0) {
-            if (n >= cap) return fail(SWEC_ERR_INVALID_ARG, "interval buffer too small");
-            swec_interval& iv = out[n++];
-            iv.block_index = int32_t(block_index);
-            iv.is_large_block = is_large ? 1 : 0;
-            iv.inner_block_offset = inner;
-            iv.large_block_rows_count = int32_t(nlarge_rows);
-            iv.reserved = 0;
-            iv.size = std::min(size, room);
-            size -= iv.size;
-            if (size == 0) break;
-        }
-        // moveToNextBlock (ec_locate.go:55-63): the block after the last large one is small block 0
-        block_index++;
-        if (is_large && block_index == nlarge_rows * k) {
-            is_large = false;
-            block_index = 0;
-        }
-        inner = 0;
-    }
-    return n;
-}
-
-void swec_interval_to_shard(const swec_interval* iv, int64_t large, int64_t small, int k, int* shard_id,
-                            int64_t* shard_offset) {
-    const int64_t row = iv->block_index / k;  // ec_locate.go:87-98
-    int64_t off = iv->inner_block_offset;
-    off += iv->is_large_block ? row * large : int64_t(iv->large_block_rows_count) * large + row * small;
-    if (shard_id) *shard_id = iv->block_index % k;
-    if (shard_offset) *shard_offset = off;
 }
 
 }  // extern "C"

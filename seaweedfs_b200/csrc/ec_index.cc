@@ -22,38 +22,12 @@
 #include <vector>
 
 #include "engine.h"
+#include "volume_format.h"
 
 namespace swec {
 namespace {
 
-constexpr int kEntry = 16;             // NeedleMapEntrySize
-constexpr int32_t kTombstone = -1;     // TombstoneFileSize
 constexpr int64_t kSuperBlockSize = 8; // super_block.SuperBlockSize
-
-uint64_t be64(const uint8_t* p) {
-    uint64_t v = 0;
-    for (int i = 0; i < 8; i++) v = (v << 8) | p[i];
-    return v;
-}
-uint32_t be32(const uint8_t* p) { return (uint32_t(p[0]) << 24) | (uint32_t(p[1]) << 16) | (uint32_t(p[2]) << 8) | p[3]; }
-void put_be64(uint8_t* p, uint64_t v) {
-    for (int i = 7; i >= 0; i--) { p[i] = uint8_t(v); v >>= 8; }
-}
-void put_be32(uint8_t* p, uint32_t v) {
-    for (int i = 3; i >= 0; i--) { p[i] = uint8_t(v); v >>= 8; }
-}
-bool size_deleted(int32_t s) { return s < 0 || s == kTombstone; }  // Size.IsDeleted, needle_types.go:25-27
-
-bool read_all(const std::string& path, std::vector<uint8_t>* out) {
-    FILE* f = fopen(path.c_str(), "rb");
-    if (!f) return false;
-    uint8_t buf[1 << 16];
-    size_t n;
-    out->clear();
-    while ((n = fread(buf, 1, sizeof buf, f)) > 0) out->insert(out->end(), buf, buf + n);
-    fclose(f);
-    return true;
-}
 
 // Replaces `path` atomically: the bytes go to <path>.tmp.<pid>, which is renamed over the target.  A mounted
 // EcVolume maps .ecx MAP_SHARED (ec_volume.cc) and binary-searches the mapping; rewriting the same inode in place
@@ -94,13 +68,6 @@ bool exists(const std::string& p) {
 
 int io_err(const std::string& what) { return fail(SWEC_ERR_IO, what + ": " + strerror(errno)); }
 
-// GetActualSize (needle/needle_read.go:292-294, needle_read_tail.go:36-50): header 16 + body + checksum 4
-// (+ 8-byte timestamp in version 3) + padding to 8, where the padding is 1..8 bytes, never 0.
-int64_t actual_size(int32_t size, int version) {
-    const int64_t fixed = 16 + int64_t(size) + 4 + (version == 3 ? 8 : 0);
-    return fixed + (8 - fixed % 8);
-}
-
 }  // namespace
 }  // namespace swec
 
@@ -111,31 +78,31 @@ extern "C" {
 int swec_write_sorted_file_from_idx(const char* base, const char* ext) {
     if (!base || !ext) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
     std::vector<uint8_t> idx;
-    if (!read_all(std::string(base) + ".idx", &idx)) return io_err(std::string("cannot read Volume Index ") + base + ".idx");
+    if (!read_file(std::string(base) + ".idx", &idx)) return io_err(std::string("cannot read Volume Index ") + base + ".idx");
     // readNeedleMap replays the .idx into a map: a live entry (non-zero offset, size not deleted) sets the key, anything
     // else removes it — so the LAST entry of a key alone decides whether and how the key appears.  Sorting the entries
     // by (key, position) and keeping each key's last one gives the same file without a 30-million-node tree for a
     // full 30 GB volume of small needles.
     struct E { uint64_t key; uint32_t pos, offset, size; };
-    const size_t n = idx.size() / kEntry;
+    const size_t n = idx.size() / kIndexEntrySize;
     if (n > 0xFFFFFFFFull) return fail(SWEC_ERR_INVALID_ARG, "index too large");
     std::vector<E> es(n);
     for (size_t i = 0; i < n; i++) {
-        const uint8_t* p = &idx[i * kEntry];
+        const uint8_t* p = &idx[i * kIndexEntrySize];
         es[i] = {be64(p), uint32_t(i), be32(p + 8), be32(p + 12)};
     }
     std::sort(es.begin(), es.end(), [](const E& a, const E& b) { return a.key != b.key ? a.key < b.key : a.pos < b.pos; });
     std::vector<uint8_t> out;
-    out.reserve(n * kEntry);
+    out.reserve(n * kIndexEntrySize);
     for (size_t i = 0; i < n; i++) {
         if (i + 1 < n && es[i + 1].key == es[i].key) continue;  // not the key's last word
         const E& e = es[i];
         if (e.offset == 0 || size_deleted(int32_t(e.size))) continue;  // the key ends deleted
-        uint8_t rec[kEntry];
+        uint8_t rec[kIndexEntrySize];
         put_be64(rec, e.key);
         put_be32(rec + 8, e.offset);
         put_be32(rec + 12, e.size);
-        out.insert(out.end(), rec, rec + kEntry);  // ascending keys: AscendingVisit
+        out.insert(out.end(), rec, rec + kIndexEntrySize);  // ascending keys: AscendingVisit
     }
     if (!write_all(std::string(base) + ext, out)) return io_err("failed to open ecx file");
     return SWEC_OK;
@@ -148,38 +115,29 @@ int swec_rebuild_ecx_file(const char* base) {
     const int ecx = open((b + ".ecx").c_str(), O_RDWR);
     if (ecx < 0) return io_err("rebuild: failed to open ecx file");
     std::vector<uint8_t> index, ecj;
-    if (!read_all(b + ".ecx", &index)) {
+    if (!read_file(b + ".ecx", &index)) {
         close(ecx);
         return io_err("rebuild: failed to read ecx file");
     }
-    const int64_t entries = int64_t(index.size()) / kEntry;
-    if (!read_all(b + ".ecj", &ecj)) {
+    const int64_t entries = int64_t(index.size()) / kIndexEntrySize;
+    if (!read_file(b + ".ecj", &ecj)) {
         close(ecx);
         return io_err("rebuild: failed to open ecj file");
     }
     // SearchNeedleFromSortedIndex + MarkNeedleDeleted for every journalled id: the search runs on the copy in
     // memory (a 30 GB volume of small needles has a 480 MB index and 25 probes per id), the tombstone is written
     // in place on disk, exactly the four size bytes the reference rewrites
-    for (size_t off = 0; off + 8 <= ecj.size(); off += 8) {
-        const uint64_t id = be64(&ecj[off]);
-        int64_t lo = 0, hi = entries;
-        while (lo < hi) {
-            const int64_t mid = (lo + hi) / 2;
-            const uint64_t key = be64(&index[size_t(mid) * kEntry]);
-            if (key == id) {
-                uint8_t t[4];
-                put_be32(t, uint32_t(kTombstone));
-                if (memcmp(&index[size_t(mid) * kEntry + 12], t, 4) != 0) {
-                    memcpy(&index[size_t(mid) * kEntry + 12], t, 4);
-                    if (pwrite(ecx, t, 4, off_t(mid * kEntry + 12)) != 4) {
-                        close(ecx);
-                        return io_err("sorted needle write error");
-                    }
-                }
-                break;
+    for (const uint64_t id : ecj_ids(ecj)) {
+        const int64_t at = search_sorted_index(index.data(), entries, id);
+        if (at < 0) continue;
+        uint8_t t[4];
+        put_be32(t, uint32_t(kTombstone));
+        if (memcmp(&index[size_t(at) * kIndexEntrySize + 12], t, 4) != 0) {
+            memcpy(&index[size_t(at) * kIndexEntrySize + 12], t, 4);
+            if (pwrite(ecx, t, 4, off_t(at * kIndexEntrySize + 12)) != 4) {
+                close(ecx);
+                return io_err("sorted needle write error");
             }
-            if (key < id) lo = mid + 1;
-            else hi = mid;
         }
     }
     close(ecx);
@@ -191,14 +149,14 @@ int swec_write_idx_file_from_ec_index(const char* base) {
     if (!base) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
     const std::string b(base);
     std::vector<uint8_t> data;
-    if (!read_all(b + ".ecx", &data)) return io_err("cannot open ec index " + b + ".ecx");
+    if (!read_file(b + ".ecx", &data)) return io_err("cannot open ec index " + b + ".ecx");
     std::vector<uint8_t> ecj;
-    if (exists(b + ".ecj") && !read_all(b + ".ecj", &ecj)) return io_err("cannot open ec index " + b + ".ecj");
-    for (size_t off = 0; off + 8 <= ecj.size(); off += 8) {  // one tombstone entry per journalled id
-        uint8_t e[kEntry] = {0};
-        memcpy(e, &ecj[off], 8);
+    if (exists(b + ".ecj") && !read_file(b + ".ecj", &ecj)) return io_err("cannot open ec index " + b + ".ecj");
+    for (const uint64_t id : ecj_ids(ecj)) {  // one tombstone entry per journalled id
+        uint8_t e[kIndexEntrySize] = {0};
+        put_be64(e, id);
         put_be32(e + 12, uint32_t(kTombstone));
-        data.insert(data.end(), e, e + kEntry);
+        data.insert(data.end(), e, e + kIndexEntrySize);
     }
     if (!write_all(b + ".idx", data)) return io_err("cannot open " + b + ".idx");
     return SWEC_OK;
@@ -207,10 +165,10 @@ int swec_write_idx_file_from_ec_index(const char* base) {
 int swec_has_live_needles(const char* index_base, int* has_live) {
     if (!index_base || !has_live) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
     std::vector<uint8_t> ecx;
-    if (!read_all(std::string(index_base) + ".ecx", &ecx)) return io_err(std::string("cannot open ec index ") + index_base + ".ecx");
+    if (!read_file(std::string(index_base) + ".ecx", &ecx)) return io_err(std::string("cannot open ec index ") + index_base + ".ecx");
     *has_live = 0;
-    for (size_t off = 0; off + kEntry <= ecx.size(); off += kEntry)
-        if (!size_deleted(int32_t(be32(&ecx[off + 12])))) {
+    for (size_t off = 0; off + kIndexEntrySize <= ecx.size(); off += kIndexEntrySize)
+        if (!size_deleted(index_entry(&ecx[off]).size)) {
             *has_live = 1;
             break;
         }
@@ -224,11 +182,13 @@ int swec_check_index_file(const char* path, int needle_version, int64_t* entries
                           int* n_errors) {
     if (!path || !entries || !n_errors) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
     std::vector<uint8_t> raw;
-    if (!read_all(path, &raw)) return io_err(std::string("cannot read index ") + path);
+    if (!read_file(path, &raw)) return io_err(std::string("cannot read index ") + path);
     struct E { int index; uint64_t id; int64_t offset; int32_t size; };
     std::vector<E> es;
-    for (size_t off = 0; off + kEntry <= raw.size(); off += kEntry)  // WalkIndexFile ignores a trailing partial entry
-        es.push_back({int(es.size()), be64(&raw[off]), int64_t(be32(&raw[off + 8])) * 8, int32_t(be32(&raw[off + 12]))});
+    for (size_t off = 0; off + kIndexEntrySize <= raw.size(); off += kIndexEntrySize) {  // WalkIndexFile ignores a trailing partial entry
+        const IndexEntry x = index_entry(&raw[off]);
+        es.push_back({int(es.size()), x.key, x.offset, x.size});
+    }
     std::stable_sort(es.begin(), es.end(), [](const E& a, const E& b) { return a.offset != b.offset ? a.offset < b.offset : a.size < b.size; });
     // needle.GetActualSize with the reference's types: PaddingLength is computed in Size (int32) arithmetic and wraps
     // like Go does; NeedleBodyLength adds in int64 (needle_read_tail.go:36-49)
@@ -255,8 +215,8 @@ int swec_check_index_file(const char* path, int needle_version, int64_t* entries
                 std::to_string(last_end) + "]");
     }
     const int64_t n = int64_t(es.size());
-    if (n * kEntry != int64_t(raw.size()))
-        add("expected an index file of size " + std::to_string(raw.size()) + ", got " + std::to_string(n * kEntry));
+    if (n * kIndexEntrySize != int64_t(raw.size()))
+        add("expected an index file of size " + std::to_string(raw.size()) + ", got " + std::to_string(n * kIndexEntrySize));
     *entries = n;
     *n_errors = count;
     if (errors && errors_cap) {
@@ -278,12 +238,12 @@ int swec_find_dat_file_size(const char* data_base, const char* index_base, int64
     if (got != ssize_t(sizeof sb)) return fail(SWEC_ERR_IO, "cannot read the superblock from .ec00");
     const int version = sb[0];
     std::vector<uint8_t> ecx;
-    if (!read_all(std::string(index_base) + ".ecx", &ecx)) return io_err(std::string("cannot open ec index ") + index_base + ".ecx");
+    if (!read_file(std::string(index_base) + ".ecx", &ecx)) return io_err(std::string("cannot open ec index ") + index_base + ".ecx");
     int64_t size = kSuperBlockSize;
-    for (size_t off = 0; off + kEntry <= ecx.size(); off += kEntry) {
-        const int32_t sz = int32_t(be32(&ecx[off + 12]));
-        if (size_deleted(sz)) continue;
-        const int64_t stop = int64_t(be32(&ecx[off + 8])) * 8 + actual_size(sz, version);
+    for (size_t off = 0; off + kIndexEntrySize <= ecx.size(); off += kIndexEntrySize) {
+        const IndexEntry e = index_entry(&ecx[off]);
+        if (size_deleted(e.size)) continue;
+        const int64_t stop = e.offset + needle_actual_size(e.size, version);
         if (stop > size) size = stop;
     }
     *dat_size = size;

@@ -13,7 +13,6 @@
 // swec_rebuild_ec_files; the index and .vif work is host-only.
 #include <errno.h>
 #include <fcntl.h>
-#include <libgen.h>
 #include <sys/mman.h>
 #include <sys/stat.h>
 #include <unistd.h>
@@ -31,21 +30,11 @@
 
 #include "engine.h"
 #include "mini_json.h"
+#include "volume_format.h"
 
 namespace swec {
 
 namespace {
-
-std::string ext_of(int idx) {  // ToExt, ec_encoder.go:106-108
-    char b[16];
-    snprintf(b, sizeof b, ".ec%02d", idx);
-    return b;
-}
-
-bool is_file(const std::string& p) {
-    struct stat st;
-    return stat(p.c_str(), &st) == 0 && !S_ISDIR(st.st_mode);
-}
 
 // SaveVolumeInfo (weed/storage/volume_info/volume_info.go:73-95): protojson with EmitUnpopulated and
 // a two-space indent.  protojson renders 64-bit integers as strings and deliberately does not promise
@@ -88,48 +77,11 @@ int save_volume_info(const std::string& path, uint32_t version, int64_t dat_size
     return SWEC_OK;
 }
 
-// the EC ratio a handler works with: an existing valid .vif wins, else 10+4
-// (volume_grpc_erasure_coding.go:61-77, ec_encoder.go:76-95, ec_volume.go:114-154)
-void ratio_from_vif(const std::string& data_base, int* k, int* m) {
-    int ds = 0, ps = 0;
-    if (read_vif_ratio(data_base + ".vif", &ds, &ps) && ds > 0 && ps > 0 && ds + ps <= SWEC_MAX_SHARDS) {
-        *k = ds;
-        *m = ps;
-    } else {
-        *k = 10;
-        *m = 4;
-    }
-}
-
 // A numeric field of a protobuf-JSON .vif (64-bit integers are rendered as strings); false when absent.
 bool vif_number(const std::string& txt, const char* key, int64_t* out) {
     const std::string k(key);
     const char* alt = k == "datFileSize" ? "dat_file_size" : k == "expireAtSec" ? "expire_at_sec" : nullptr;
     return mini_json::top_int(txt, key, alt, out);
-}
-
-bool slurp(const std::string& path, std::string* out) {
-    FILE* f = fopen(path.c_str(), "rb");
-    if (!f) return false;
-    char buf[1 << 16];
-    size_t n;
-    out->clear();
-    while ((n = fread(buf, 1, sizeof buf, f)) > 0) out->append(buf, n);
-    fclose(f);
-    return true;
-}
-
-uint64_t be64(const uint8_t* p) {
-    uint64_t v = 0;
-    for (int i = 0; i < 8; i++) v = (v << 8) | p[i];
-    return v;
-}
-uint32_t be32(const uint8_t* p) { return (uint32_t(p[0]) << 24) | (uint32_t(p[1]) << 16) | (uint32_t(p[2]) << 8) | p[3]; }
-
-// GetActualSize (needle/needle_read.go:292-294, needle_read_tail.go:36-49)
-int64_t needle_actual_size(int64_t size, int version) {
-    const int64_t fixed = 16 + size + 4 + (version == 3 ? 8 : 0);
-    return fixed + (8 - fixed % 8);
 }
 
 }  // namespace
@@ -144,7 +96,7 @@ int swec_ec_shards_generate(const char* data_base, const char* index_base, uint3
     if (!data_base) return fail(SWEC_ERR_INVALID_ARG, "data_base_file_name is NULL");
     const std::string db(data_base), ib(index_base && *index_base ? index_base : data_base);
     int k, m;
-    ratio_from_vif(db, &k, &m);
+    ec_ratio(db, &k, &m);
 
     struct Cleanup {  // the handler's deferred cleanup: shards and .ecx go away unless we reach the end
         const std::string &db, &ib;
@@ -153,7 +105,7 @@ int swec_ec_shards_generate(const char* data_base, const char* index_base, uint3
         ~Cleanup() {
             if (!armed) return;
             const std::string keep = last_error();  // unlink() must not disturb the reported detail
-            for (int i = 0; i < total; i++) unlink((db + ext_of(i)).c_str());
+            for (int i = 0; i < total; i++) unlink((db + shard_ext(i)).c_str());
             unlink((ib + ".ecx").c_str());
             set_last_error(keep);
         }
@@ -176,8 +128,7 @@ int swec_ec_shards_generate(const char* data_base, const char* index_base, uint3
         close(fd);
         needle_version = b0;
     }
-    // WriteEcFilesWithContext: 256 KiB buffers, 1 GiB / 1 MiB blocks (ec_encoder.go:67-69)
-    rc = swec_generate_ec_files(db.c_str(), 256 * 1024, int64_t(1) << 30, int64_t(1) << 20, k, m, device);
+    rc = swec_generate_ec_files(db.c_str(), kBufferSize, kLargeBlockSize, kSmallBlockSize, k, m, device);
     if (rc) return rc;
     rc = save_volume_info(db + ".vif", needle_version, int64_t(st.st_size), expire_at_sec, k, m);
     if (rc) return rc;
@@ -203,23 +154,11 @@ int swec_ec_shards_to_volume(const char* data_base, const char* index_base, cons
     if (!data_base || (n_additional_dirs > 0 && !additional_dirs)) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
     const std::string db(data_base);
     int k, m;
-    ratio_from_vif(db, &k, &m);  // NewEcVolume loads the ratio from .vif (ec_volume.go:114-154)
+    ec_ratio(db, &k, &m);  // NewEcVolume loads the ratio from .vif (ec_volume.go:114-154)
     // CollectEcShards: every data shard must be found locally (:601-606)
-    std::string base_copy(db);
-    const std::string base_name = basename(&base_copy[0]);
     std::vector<std::string> names;
     for (int i = 0; i < k; i++) {
-        std::string path = db + ext_of(i);
-        if (!is_file(path)) {
-            path.clear();
-            for (int d = 0; d < n_additional_dirs; d++) {
-                const std::string cand = std::string(additional_dirs[d]) + "/" + base_name + ext_of(i);
-                if (is_file(cand)) {
-                    path = cand;
-                    break;
-                }
-            }
-        }
+        const std::string path = find_shard_file(db, additional_dirs, n_additional_dirs, i);
         if (path.empty()) return fail(SWEC_ERR_TOO_FEW_SHARDS, "ec volume missing shard " + std::to_string(i));
         names.push_back(path);
     }
@@ -236,7 +175,7 @@ int swec_ec_shards_to_volume(const char* data_base, const char* index_base, cons
     if ((rc = swec_find_dat_file_size(ec00_base.c_str(), ib.c_str(), &size))) return rc;
     std::vector<const char*> cnames;
     for (const auto& s : names) cnames.push_back(s.c_str());
-    if ((rc = swec_write_dat_file(db.c_str(), size, cnames.data(), k, int64_t(1) << 30, int64_t(1) << 20))) return rc;
+    if ((rc = swec_write_dat_file(db.c_str(), size, cnames.data(), k, kLargeBlockSize, kSmallBlockSize))) return rc;
     if ((rc = swec_write_idx_file_from_ec_index(ib.c_str()))) return rc;
     if (dat_file_size) *dat_file_size = size;
     return SWEC_OK;
@@ -248,7 +187,7 @@ int swec_ec_shards_to_volume(const char* data_base, const char* index_base, cons
 
 struct swec_ec_volume {
     std::mutex mu;
-    int k = 10, m = 4, version = 3, device = 0;
+    int k = swec::kDefaultDataShards, m = swec::kDefaultParityShards, version = 3, device = 0;
     int64_t shard_dat_size = 0;
     std::string index_base;
     std::vector<int> shard_fd;  // total entries, -1 = not local
@@ -256,17 +195,12 @@ struct swec_ec_volume {
     // hundreds of EC volumes; a lookup touches ~25 pages of the page cache (the reference does 25 ReadAt calls)
     const uint8_t* ecx_map = nullptr;
     size_t ecx_bytes = 0;
-    std::string ecj;
+    std::vector<uint8_t> ecj;
     std::vector<uint64_t> deleted;  // ids of .ecj, sorted and unique: the reference's in-memory deletedNeedles set
     int64_t ecj_size_seen = -1, ecj_mtime_ns_seen = 0;
     uint64_t ecj_inode_seen = 0;
     void index_journal() {
-        deleted.clear();
-        for (size_t off = 0; off + 8 <= ecj.size(); off += 8) {
-            uint64_t v = 0;
-            for (int i = 0; i < 8; i++) v = (v << 8) | uint8_t(ecj[off + size_t(i)]);
-            deleted.push_back(v);
-        }
+        deleted = swec::ecj_ids(ecj);
         std::sort(deleted.begin(), deleted.end());
         deleted.erase(std::unique(deleted.begin(), deleted.end()), deleted.end());
     }
@@ -290,7 +224,7 @@ void swec_ec_volume::refresh_journal(bool force) {
     const int64_t mt = have ? int64_t(st.st_mtim.tv_sec) * 1000000000ll + st.st_mtim.tv_nsec : 0;
     const uint64_t ino = have ? uint64_t(st.st_ino) : 0;
     if (!force && now == ecj_size_seen && mt == ecj_mtime_ns_seen && ino == ecj_inode_seen) return;
-    if (now == 0 || !swec::slurp(index_base + ".ecj", &ecj)) ecj.clear();
+    if (now == 0 || !swec::read_file(index_base + ".ecj", &ecj)) ecj.clear();
     ecj_size_seen = now;
     ecj_mtime_ns_seen = mt;
     ecj_inode_seen = ino;
@@ -313,35 +247,24 @@ int swec_ec_volume_open(const char* data_base, const char* index_base, const cha
     v->index_base = ib;
 
     // what NewEcVolume loads: ratio, needle version and datFileSize from .vif (ec_volume.go:114-154)
-    ratio_from_vif(db, &v->k, &v->m);
+    ec_ratio(db, &v->k, &v->m);
     const int total = v->k + v->m;
     int64_t dat_file_size = 0;
     {
-        std::string vif;
-        if (slurp(db + ".vif", &vif) || slurp(ib + ".vif", &vif)) {
+        std::vector<uint8_t> raw;
+        if (read_file(db + ".vif", &raw) || read_file(ib + ".vif", &raw)) {
+            const std::string vif(raw.begin(), raw.end());
             int64_t x = 0;
             if (vif_number(vif, "version", &x) && x > 0) v->version = int(x);
             if (vif_number(vif, "datFileSize", &x)) dat_file_size = x;
         }
     }
     // local shards: data_base's directory, then the other disks
-    std::string base_copy(db);
-    const std::string base_name = basename(&base_copy[0]);
     v->shard_fd.assign(size_t(total), -1);
     int64_t ecd_file_size = -1;
     int nlocal = 0;
     for (int i = 0; i < total; i++) {
-        std::string path = db + ext_of(i);
-        if (!is_file(path)) {
-            path.clear();
-            for (int d = 0; d < n_additional_dirs; d++) {
-                const std::string cand = std::string(additional_dirs[d]) + "/" + base_name + ext_of(i);
-                if (is_file(cand)) {
-                    path = cand;
-                    break;
-                }
-            }
-        }
+        const std::string path = find_shard_file(db, additional_dirs, n_additional_dirs, i);
         if (path.empty()) continue;
         const int fd = open(path.c_str(), O_RDONLY);
         if (fd < 0) continue;  // unreadable = not local; its intervals are recovered from the others
@@ -388,11 +311,11 @@ int swec_ec_volume_read_needles(swec_ec_volume* v, swec_needle_read* reads, int 
     if (!v || (n_reads > 0 && !reads)) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
     std::lock_guard<std::mutex> lock(v->mu);
     const int k = v->k, total = v->k + v->m, version = v->version;
-    const int64_t large = int64_t(1) << 30, small = int64_t(1) << 20;
+    const int64_t large = kLargeBlockSize, small = kSmallBlockSize;
 
     v->refresh_journal();
     const uint8_t* ex = v->ecx_map;
-    const int64_t entries = int64_t(v->ecx_bytes) / 16;
+    const int64_t entries = int64_t(v->ecx_bytes) / kIndexEntrySize;
     auto journalled = [&](uint64_t id) { return std::binary_search(v->deleted.begin(), v->deleted.end(), id); };
 
     // ---- pass 1: locate every needle, read what is local, collect what must be recovered
@@ -412,27 +335,18 @@ int swec_ec_volume_read_needles(swec_ec_volume* v, swec_needle_read* reads, int 
         rd.n_bytes = 0;
         rd.n_recovered_intervals = 0;
         rd.status = SWEC_OK;
-        int64_t lo = 0, hi = entries, found = -1;  // SearchNeedleFromSortedIndex (ec_volume.go:431-458)
-        while (lo < hi) {
-            const int64_t mid = (lo + hi) / 2;
-            const uint64_t key = be64(ex + mid * 16);
-            if (key == rd.needle_id) {
-                found = mid;
-                break;
-            }
-            if (key < rd.needle_id) lo = mid + 1;
-            else hi = mid;
-        }
+        const int64_t found = search_sorted_index(ex, entries, rd.needle_id);
         if (found < 0) {
             rd.status = SWEC_ERR_NOT_FOUND;
             continue;
         }
-        const int64_t offset = int64_t(be32(ex + found * 16 + 8)) * 8;  // Offset.ToActualOffset (offset_4bytes.go)
-        int32_t size = int32_t(be32(ex + found * 16 + 12));
-        if (journalled(rd.needle_id)) size = -1;  // TombstoneFileSize (FindNeedleFromEcx, ec_volume.go:419-429)
+        const IndexEntry entry = index_entry(ex + found * kIndexEntrySize);
+        const int64_t offset = entry.offset;
+        int32_t size = entry.size;
+        if (journalled(rd.needle_id)) size = kTombstone;  // FindNeedleFromEcx (ec_volume.go:419-429)
         rd.offset = offset;
         rd.size = size;
-        if (size < 0) {  // Size.IsDeleted
+        if (size_deleted(size)) {
             rd.status = SWEC_ERR_DELETED;
             continue;
         }
@@ -445,7 +359,7 @@ int swec_ec_volume_read_needles(swec_ec_volume* v, swec_needle_read* reads, int 
             rd.status = SWEC_ERR_INVALID_ARG;
             continue;
         }
-        std::vector<swec_interval> ivs(size_t(want / small) + 4);  // a record crosses at most size/1 MiB + 2 blocks
+        std::vector<swec_interval> ivs(max_intervals(want, small));
         const int niv = swec_locate_data(large, small, v->shard_dat_size, offset, want, k, ivs.data(), int(ivs.size()));
         if (niv < 0) {
             rd.status = niv;
@@ -547,7 +461,7 @@ int swec_ec_volume_scrub_local(swec_ec_volume* v, int64_t* entries, uint32_t* br
         if (k2) add(buf.data()), count += k2 - 1;
     }
     const int k = v->k, total = v->k + v->m;
-    const int64_t large = int64_t(1) << 30, small = int64_t(1) << 20;
+    const int64_t large = kLargeBlockSize, small = kSmallBlockSize;
     std::vector<int64_t> shard_size(size_t(total), -1);
     for (int i = 0; i < total; i++) {
         struct stat st;
@@ -555,16 +469,14 @@ int swec_ec_volume_scrub_local(swec_ec_volume* v, int64_t* entries, uint32_t* br
     }
     std::vector<uint8_t> broken(size_t(total), 0), chunk;
     const uint8_t* ex = v->ecx_map;
-    const int64_t n_entries = int64_t(v->ecx_bytes) / 16;
+    const int64_t n_entries = int64_t(v->ecx_bytes) / kIndexEntrySize;
     int64_t walked = 0;
     for (int64_t e = 0; e < n_entries; e++) {
         walked++;
-        const uint64_t id = be64(ex + e * 16);
-        const int64_t offset = int64_t(be32(ex + e * 16 + 8)) * 8;
-        const int32_t size = int32_t(be32(ex + e * 16 + 12));
-        if (size == -1) continue;  // Size.IsTombstone
+        const auto [id, offset, size] = index_entry(ex + e * kIndexEntrySize);
+        if (size == kTombstone) continue;  // Size.IsTombstone
         const int64_t want = needle_actual_size(size, v->version);
-        std::vector<swec_interval> ivs(size_t(std::max<int64_t>(want, 0) / small) + 4);
+        std::vector<swec_interval> ivs(max_intervals(want, small));
         const int niv = want > 0 ? swec_locate_data(large, small, v->shard_dat_size, offset, want, k, ivs.data(), int(ivs.size())) : 0;
         if (niv < 0) return niv;
         int64_t read = 0;
@@ -641,7 +553,7 @@ int swec_ec_volume_counts(swec_ec_volume* v, uint64_t* file_count, uint64_t* del
     if (!v) return fail(SWEC_ERR_INVALID_ARG, "NULL volume");
     std::lock_guard<std::mutex> lock(v->mu);
     v->refresh_journal();
-    if (file_count) *file_count = uint64_t(v->ecx_bytes / 16);
+    if (file_count) *file_count = uint64_t(v->ecx_bytes / kIndexEntrySize);
     if (delete_count) *delete_count = uint64_t(v->deleted.size());
     return SWEC_OK;
 }
@@ -652,20 +564,9 @@ int swec_ec_volume_counts(swec_ec_volume* v, uint64_t* file_count, uint64_t* del
 int swec_ec_volume_delete_needle(swec_ec_volume* v, uint64_t needle_id) {
     if (!v) return fail(SWEC_ERR_INVALID_ARG, "NULL volume");
     std::lock_guard<std::mutex> lock(v->mu);
-    const uint8_t* ex = v->ecx_map;
-    int64_t lo = 0, hi = int64_t(v->ecx_bytes) / 16, found = -1;
-    while (lo < hi) {
-        const int64_t mid = (lo + hi) / 2;
-        const uint64_t key = be64(ex + mid * 16);
-        if (key == needle_id) {
-            found = mid;
-            break;
-        }
-        if (key < needle_id) lo = mid + 1;
-        else hi = mid;
-    }
-    if (found < 0) return SWEC_OK;                                   // already gone
-    if (int32_t(be32(ex + found * 16 + 12)) < 0) return SWEC_OK;     // folded into .ecx by an earlier rebuild
+    const int64_t found = search_sorted_index(v->ecx_map, int64_t(v->ecx_bytes) / kIndexEntrySize, needle_id);
+    if (found < 0) return SWEC_OK;                                                    // already gone
+    if (size_deleted(index_entry(v->ecx_map + found * kIndexEntrySize).size)) return SWEC_OK;  // folded into .ecx by an earlier rebuild
     // the in-memory set is authoritative between external changes of the file (refresh_journal notices those by
     // size / mtime / inode): an O(log n) membership test and an 8-byte append per delete, like the reference's map
     // check + append — not a re-read of the whole journal
@@ -681,7 +582,7 @@ int swec_ec_volume_delete_needle(swec_ec_volume* v, uint64_t needle_id) {
         return fail(SWEC_ERR_IO, "stat ecj: " + std::string(strerror(e)));
     }
     uint8_t b[8];
-    for (int i = 0; i < 8; i++) b[i] = uint8_t(needle_id >> (8 * (7 - i)));
+    put_be64(b, needle_id);
     const bool ok = pwrite(fd, b, 8, st.st_size) == 8 && fsync(fd) == 0;
     const int e = errno;
     if (!ok) {
@@ -692,7 +593,7 @@ int swec_ec_volume_delete_needle(swec_ec_volume* v, uint64_t needle_id) {
     struct stat after;
     const bool stat_ok = fstat(fd, &after) == 0;
     close(fd);
-    v->ecj.append(reinterpret_cast<const char*>(b), 8);
+    v->ecj.insert(v->ecj.end(), b, b + 8);
     v->deleted.insert(std::upper_bound(v->deleted.begin(), v->deleted.end(), needle_id), needle_id);
     if (stat_ok) {
         v->ecj_size_seen = int64_t(after.st_size);

@@ -1,6 +1,7 @@
 // seaweedfs_b200/csrc/engine.cc — encoder object, matrix→kernel dispatch, host staging pipeline.
 #include "engine.h"
 #include "io_pool.h"
+#include "volume_format.h"
 
 #include <algorithm>
 #include <atomic>
@@ -199,7 +200,6 @@ swec_encoder_impl::~swec_encoder_impl() {
         if (s.done) cudaEventDestroy(s.done);
         if (s.stream) cudaStreamDestroy(s.stream);
     }
-    if (tail_scratch) cudaFree(tail_scratch);
     if (stream) cudaStreamDestroy(stream);
 }
 
@@ -1211,16 +1211,6 @@ int swec_apply_device(swec_encoder* e, int r, int k, const uint8_t* rows, const 
                     Layout{}, pick_stream(e, stream));
 }
 
-int64_t swec_expected_shard_size(int64_t dat_size, int k, int64_t large, int64_t small) {
-    if (k <= 0 || large <= 0 || small <= 0 || dat_size < 0) return 0;
-    const int64_t large_row = large * k, small_row = small * k;
-    const int64_t nlarge = dat_size / large_row;
-    int64_t size = nlarge * large;
-    const int64_t rem = dat_size - nlarge * large_row;
-    if (rem > 0) size += ((rem + small_row - 1) / small_row) * small;
-    return size;
-}
-
 int swec_encode_volume_device(swec_encoder* e, const void* dat_v, int64_t dat_size, int64_t large, int64_t small,
                               void* const* parity, void* stream) {
     if (!e || !dat_v || !parity || dat_size < 0 || large <= 0 || small <= 0)
@@ -1260,65 +1250,48 @@ int swec_encode_volume_device(swec_encoder* e, const void* dat_v, int64_t dat_si
         return SWEC_OK;
     };
 
-    const int64_t large_row = large * k, small_row = small * k;
-    const int64_t nlarge = dat_size / large_row;       // while remaining >= largeRowSize  (ec_encoder.go:304)
-    if (nlarge && (rc = region(dat, large, nlarge, 0))) return rc;
-    const int64_t rem = dat_size - nlarge * large_row;
-    if (rem > 0) {                                     // while remaining > 0             (ec_encoder.go:312)
-        const uint8_t* base = dat + nlarge * large_row;
-        const int64_t nfull = rem / small_row;
-        if (nfull && (rc = region(base, small, nfull, nlarge * large))) return rc;
-        const int64_t tail = rem - nfull * small_row;
-        if (tail > 0) {  // last row: bytes past EOF read as zero (ec_encoder.go:258-262)
-            struct Scratch {  // stream-ordered: freed after the work queued on s, on every exit path
-                uint8_t* p = nullptr;
-                cudaStream_t s;
-                ~Scratch() {
-                    if (p) cudaFreeAsync(p, s);
-                }
-            } scratch{nullptr, s};
-            SWEC_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&scratch.p), size_t(small_row), s));
-            SWEC_CUDA(cudaMemsetAsync(scratch.p, 0, size_t(small_row), s));
-            SWEC_CUDA(cudaMemcpyAsync(scratch.p, base + nfull * small_row, size_t(tail), cudaMemcpyDeviceToDevice, s));
-            rc = region(scratch.p, small, 1, nlarge * large + nfull * small);
-            if (rc) return rc;
-        }
+    const StripeGeometry g(dat_size, k, large, small);
+    if (g.large_rows && (rc = region(dat, large, g.large_rows, 0))) return rc;
+    if (g.small_rows && (rc = region(dat + g.small_dat_offset(), small, g.small_rows, g.small_shard_offset()))) return rc;
+    if (g.tail > 0) {  // last row: bytes past EOF read as zero (ec_encoder.go:258-262)
+        struct Scratch {  // stream-ordered: freed after the work queued on s, on every exit path
+            uint8_t* p = nullptr;
+            cudaStream_t s;
+            ~Scratch() {
+                if (p) cudaFreeAsync(p, s);
+            }
+        } scratch{nullptr, s};
+        SWEC_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&scratch.p), size_t(g.small_row()), s));
+        SWEC_CUDA(cudaMemsetAsync(scratch.p, 0, size_t(g.small_row()), s));
+        SWEC_CUDA(cudaMemcpyAsync(scratch.p, dat + g.tail_dat_offset(), size_t(g.tail), cudaMemcpyDeviceToDevice, s));
+        rc = region(scratch.p, small, 1, g.tail_shard_offset());
+        if (rc) return rc;
     }
     return SWEC_OK;
 }
 
 int swec_extract_data_shard_device(swec_encoder* e, const void* dat_v, int64_t dat_size, int64_t large, int64_t small,
                                    int shard_id, void* shard_out, void* stream) {
-    if (!e || !dat_v || !shard_out || shard_id < 0 || shard_id >= e->k || large <= 0 || small <= 0)
+    if (!e || !dat_v || !shard_out || shard_id < 0 || shard_id >= e->k || dat_size < 0 || large <= 0 || small <= 0)
         return fail(SWEC_ERR_INVALID_ARG, "bad argument");
     const uint8_t* dat = static_cast<const uint8_t*>(dat_v);
     uint8_t* dst = static_cast<uint8_t*>(shard_out);
-    const int k = e->k;
     std::lock_guard<std::mutex> lock(e->mu);
     int rc = e->ensure_device();
     if (rc) return rc;
     cudaStream_t s = pick_stream(e, stream);
-    const int64_t large_row = large * k, small_row = small * k;
-    const int64_t nlarge = dat_size / large_row;
-    if (nlarge)
-        SWEC_CUDA(cudaMemcpy2DAsync(dst, size_t(large), dat + int64_t(shard_id) * large, size_t(large_row), size_t(large),
-                                    size_t(nlarge), cudaMemcpyDeviceToDevice, s));
-    const int64_t rem = dat_size - nlarge * large_row;
-    if (rem > 0) {
-        const uint8_t* base = dat + nlarge * large_row;
-        uint8_t* d2 = dst + nlarge * large;
-        const int64_t nfull = rem / small_row;
-        if (nfull)
-            SWEC_CUDA(cudaMemcpy2DAsync(d2, size_t(small), base + int64_t(shard_id) * small, size_t(small_row),
-                                        size_t(small), size_t(nfull), cudaMemcpyDeviceToDevice, s));
-        const int64_t tail = rem - nfull * small_row;
-        if (tail > 0) {
-            uint8_t* d3 = d2 + nfull * small;
-            int64_t have = tail - int64_t(shard_id) * small;
-            have = std::max<int64_t>(0, std::min(have, small));
-            if (have) SWEC_CUDA(cudaMemcpyAsync(d3, base + nfull * small_row + int64_t(shard_id) * small, size_t(have), cudaMemcpyDeviceToDevice, s));
-            if (have < small) SWEC_CUDA(cudaMemsetAsync(d3 + have, 0, size_t(small - have), s));
-        }
+    const StripeGeometry g(dat_size, e->k, large, small);
+    if (g.large_rows)
+        SWEC_CUDA(cudaMemcpy2DAsync(dst, size_t(large), dat + int64_t(shard_id) * large, size_t(g.large_row()), size_t(large),
+                                    size_t(g.large_rows), cudaMemcpyDeviceToDevice, s));
+    if (g.small_rows)
+        SWEC_CUDA(cudaMemcpy2DAsync(dst + g.small_shard_offset(), size_t(small), dat + g.small_dat_offset() + int64_t(shard_id) * small,
+                                    size_t(g.small_row()), size_t(small), size_t(g.small_rows), cudaMemcpyDeviceToDevice, s));
+    if (g.tail > 0) {
+        uint8_t* d3 = dst + g.tail_shard_offset();
+        const int64_t have = g.tail_bytes(shard_id);
+        if (have) SWEC_CUDA(cudaMemcpyAsync(d3, dat + g.tail_dat_offset() + int64_t(shard_id) * small, size_t(have), cudaMemcpyDeviceToDevice, s));
+        if (have < small) SWEC_CUDA(cudaMemsetAsync(d3 + have, 0, size_t(small - have), s));
     }
     return SWEC_OK;
 }
@@ -1335,29 +1308,20 @@ int swec_write_dat_device(swec_encoder* e, const void* const* data_shards, int64
     int rc = e->ensure_device();
     if (rc) return rc;
     cudaStream_t s = pick_stream(e, stream);
-    const int64_t large_row = large * k, small_row = small * k;
     // WriteDatFile's loops (ec_decoder.go:197-219): `for datFileSize >= dataShards*LargeBlockSize` copies large blocks
     // round-robin, then small blocks until the size is used up — the last block short
-    const int64_t nlarge = dat_size / large_row;
-    const int64_t rem = dat_size - nlarge * large_row;
-    const int64_t nfull = rem / small_row;
-    const int64_t tail = rem - nfull * small_row;
+    const StripeGeometry g(dat_size, k, large, small);
     for (int i = 0; i < k; i++) {
         const uint8_t* sh = static_cast<const uint8_t*>(data_shards[i]);
-        if (nlarge)
-            SWEC_CUDA(cudaMemcpy2DAsync(dat + int64_t(i) * large, size_t(large_row), sh, size_t(large), size_t(large),
-                                        size_t(nlarge), cudaMemcpyDeviceToDevice, s));
-        const uint8_t* sh2 = sh + nlarge * large;
-        uint8_t* base = dat + nlarge * large_row;
-        if (nfull)
-            SWEC_CUDA(cudaMemcpy2DAsync(base + int64_t(i) * small, size_t(small_row), sh2, size_t(small), size_t(small),
-                                        size_t(nfull), cudaMemcpyDeviceToDevice, s));
-        if (tail > 0) {
-            const int64_t have = std::max<int64_t>(0, std::min(tail - int64_t(i) * small, small));
-            if (have)
-                SWEC_CUDA(cudaMemcpyAsync(base + nfull * small_row + int64_t(i) * small, sh2 + nfull * small, size_t(have),
-                                          cudaMemcpyDeviceToDevice, s));
-        }
+        if (g.large_rows)
+            SWEC_CUDA(cudaMemcpy2DAsync(dat + int64_t(i) * large, size_t(g.large_row()), sh, size_t(large), size_t(large),
+                                        size_t(g.large_rows), cudaMemcpyDeviceToDevice, s));
+        if (g.small_rows)
+            SWEC_CUDA(cudaMemcpy2DAsync(dat + g.small_dat_offset() + int64_t(i) * small, size_t(g.small_row()), sh + g.small_shard_offset(),
+                                        size_t(small), size_t(small), size_t(g.small_rows), cudaMemcpyDeviceToDevice, s));
+        if (const int64_t have = g.tail_bytes(i))
+            SWEC_CUDA(cudaMemcpyAsync(dat + g.tail_dat_offset() + int64_t(i) * small, sh + g.tail_shard_offset(), size_t(have),
+                                      cudaMemcpyDeviceToDevice, s));
     }
     return SWEC_OK;
 }

@@ -37,8 +37,6 @@ void* pinned_alloc(int device, size_t bytes);
 void pinned_free(void* p);
 int device_numa_node(int device);
 
-// ecShardConfig.{dataShards,parityShards} of a .vif file (ec_files.cc); false when absent/unreadable
-bool read_vif_ratio(const std::string& path, int* ds, int* ps);
 // "file_direct_io" (SWEC_FILE_DIRECT): bit 0 = O_DIRECT reads of the .dat / shard inputs straight into the pinned
 // ring, bit 1 = O_DIRECT writes of the shard outputs — the page cache is bypassed both ways (disk-backed volumes only;
 // files that refuse O_DIRECT, tmpfs for one, and unaligned pieces silently take the buffered descriptor)
@@ -81,8 +79,6 @@ struct swec_encoder_impl {
     // file pipelines never stall on a kernel compile: a cold matrix is served by the table kernel (100x faster
     // than the I/O around it) while the specialised kernel is built in the background and picked up when ready
     bool never_wait_for_jit = false;
-    uint8_t* tail_scratch = nullptr;  // k*small zero-padded last row
-    size_t tail_scratch_bytes = 0;
 
     ~swec_encoder_impl();
     int ensure_device();  // cudaSetDevice + lazily create stream

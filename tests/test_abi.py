@@ -140,6 +140,9 @@ def test_argument_validation(swec, tmp_path):
     with pytest.raises(swec.SwecError) as e:
         ec.generate_ec_files(str(tmp_path / "missing"), 50, 10000, 100)   # no .dat
     assert e.value.name == "SWEC_ERR_IO"
+    with pytest.raises(swec.SwecError) as e:
+        enc.extract_data_shard_device(1, -1, 0, 1)                         # negative .dat size, before any device work
+    assert e.value.name == "SWEC_ERR_INVALID_ARG"
 
 
 def test_set_option_validation(swec):
@@ -202,16 +205,26 @@ def test_rebuild_prechecks_need_no_gpu(swec, tmp_path):
 
 
 def test_write_dat_file_roundtrip(swec, oracle, tmp_path):
+    """WriteDatFile over every shape of the last row, with k = 10, large = 10,000 and small = 100."""
     ec = swec.erasure_coding
     rng = np.random.default_rng(9)
-    dat = rng.integers(0, 256, 1_234_567, dtype=np.uint8)
-    shards = oracle.encode_dat_image(dat, buffer_size=50, large=10000, small=100)
-    names = []
-    for i in range(10):
-        names.append(str(tmp_path / ("5.ec%02d" % i)))
-        shards[i].tofile(names[-1])
-    ec.write_dat_file(str(tmp_path / "out"), len(dat), names, 10, 10000, 100)
-    assert (np.fromfile(str(tmp_path / "out.dat"), dtype=np.uint8) == dat).all()
+    for dat_size in (
+        300_000,        # 3 whole large rows (k * large = 100,000)
+        307_000,        # large rows + 7 full small rows, no tail
+        307_037,        # a tail shorter than one small block
+        1_234_567,      # a tail of 567 bytes: it ends inside shard 5
+        307_999,        # a tail of k * small - 1 bytes
+    ):
+        d = tmp_path / str(dat_size)
+        d.mkdir()
+        dat = rng.integers(0, 256, dat_size, dtype=np.uint8)
+        shards = oracle.encode_dat_image(dat, buffer_size=50, large=10000, small=100)
+        names = []
+        for i in range(10):
+            names.append(str(d / ("5.ec%02d" % i)))
+            shards[i].tofile(names[-1])
+        ec.write_dat_file(str(d / "out"), len(dat), names, 10, 10000, 100)
+        assert (np.fromfile(str(d / "out.dat"), dtype=np.uint8) == dat).all(), dat_size
 
 
 def test_jit_source_compiles_for_sm90a_without_gpu(swec):
