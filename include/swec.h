@@ -81,8 +81,9 @@ void swec_shutdown(void);
 int swec_device_spread_order(int *order, int capacity, int *count);
 uint64_t swec_kernel_launches(void);          /* kernels this process has launched (all devices) */
 /* Tuning: "enc_threads" {128,256,512}, "enc_unroll" {1,2}, "ctas_per_sm" (0 = auto),
- * "stage_chunk" (bytes per shard per staging slot), "stage_slots", "host_pieces" (a host-buffer call is cut into at
- * least this many pipelined pieces), "host_min_chunk" (but none smaller than this many bytes per shard), "jit" {0,1},
+ * "stage_chunk" (bytes per shard per staging slot), "stage_slots" {2..16} (slots in flight per staging ring, for
+ * host-buffer and file-level calls alike; SWEC_STAGE_SLOTS sets it at load), "host_pieces" (a host-buffer call is cut
+ * into at least this many pipelined pieces), "host_min_chunk" (but none smaller than this many bytes per shard), "jit" {0,1},
  * "jit_min_bytes" (streams at least this long compile their kernel inline, shorter ones in the
  * background), "power_mode" {0 = auto by the device's recent kernel time — for a GPU that sits on its power cap under
  * back-to-back launches, where the variant with fewer instructions can be the faster one; 1 = always the boost-clock

@@ -34,12 +34,6 @@
 namespace swec {
 namespace {
 
-size_t env_sz(const char* name, size_t dflt) {
-    const char* e = getenv(name);
-    const long long v = e ? atoll(e) : 0;
-    return v > 0 ? size_t(v) : dflt;
-}
-
 int io_fail(const std::string& what) { return fail(SWEC_ERR_IO, what + ": " + strerror(errno)); }
 
 // Reserving extents pays on disk filesystems (once instead of 14 files growing 8 MiB at a time) and costs on tmpfs,
@@ -88,13 +82,9 @@ struct Item {
 };
 
 struct Slot {
-    uint8_t* host = nullptr;
-    uint8_t* dev = nullptr;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t done = nullptr;
+    StagingSlot* buf;  // a slot of the pipeline's staging ring
     Item item;
 };
-
 
 // ONE I/O pool per process, shared by every file pipeline: concurrent volumes (the shell runs up to 10 at once) must not
 // multiply the thread count — on an earlier GPU generation's hosts, 4 pipelines x 16 threads on a 16-core cgroup quota ran
@@ -124,40 +114,23 @@ size_t usable_cpus() {
     return n;
 }
 IoPool& file_io_pool() {
-    static IoPool* pool = new IoPool(env_sz("SWEC_IO_THREADS", std::min<size_t>(64, std::max<size_t>(4, usable_cpus()))));
+    static IoPool* pool = new IoPool(env_size("SWEC_IO_THREADS", std::min<size_t>(64, std::max<size_t>(4, usable_cpus()))));
     return *pool;
 }
 
 // Staging rings outlive a call: pinning (mmap + mbind + cudaHostRegister) and un-pinning 3 x 14 x 8 MiB costs
 // 0.1-2 s per call, as much as the pipeline itself spends on an 8 GiB volume.  A volume
-// server encodes volume after volume, so finished pipelines park their ring here (per device and size, a few at
-// most) and the next call picks it up.  swec_shutdown() releases them.
-struct SlotSet {
-    int device = -1;
-    size_t bytes_per_slot = 0;
-    std::vector<Slot> slots;
-};
-std::mutex& slotset_mu() {
+// server encodes volume after volume, so finished pipelines park their ring here (per device, slot size and slot
+// count, a few at most) and the next call picks it up.  swec_shutdown() releases them.
+std::mutex& parked_mu() {
     static std::mutex* m = new std::mutex;
     return *m;
 }
-std::vector<SlotSet>& slotset_cache() {
-    static std::vector<SlotSet>* c = new std::vector<SlotSet>;  // leaked on purpose: no CUDA calls in static destructors
+std::vector<StagingRing>& parked_rings() {
+    static std::vector<StagingRing>* c = new std::vector<StagingRing>;  // leaked on purpose: no CUDA calls in static destructors
     return *c;
 }
-constexpr size_t kMaxCachedSlotSets = 4;
-
-void free_slots(int device, std::vector<Slot>& slots) {
-    if (cudaSetDevice(device) != cudaSuccess) cudaGetLastError();
-    for (auto& s : slots) {
-        if (s.stream) cudaStreamSynchronize(s.stream);
-        if (s.host) pinned_free(s.host);
-        if (s.dev) cudaFree(s.dev);
-        if (s.done) cudaEventDestroy(s.done);
-        if (s.stream) cudaStreamDestroy(s.stream);
-    }
-    slots.clear();
-}
+constexpr size_t kMaxParkedRings = 4;
 
 // wall-clock breakdown of one pipeline run, printed to stderr as JSON when SWEC_PIPE_STATS is set
 struct PipeStats {
@@ -191,7 +164,7 @@ class FilePipeline {
         enc_->never_wait_for_jit = !getenv("SWEC_FILE_JIT_WAIT");
         int rc = enc_->ensure_device();
         if (rc) return rc;
-        const size_t nslots = env_sz("SWEC_STAGE_SLOTS", 3);
+        const size_t nslots = stage_slots();
         const size_t streams = size_t(rows_.cols + rows_.rows * (verify_ ? 2 : 1));
         if (verify_) {
             SWEC_CUDA(cudaMalloc(reinterpret_cast<void**>(&dev_bad_), sizeof(unsigned long long) * size_t(rows_.rows)));
@@ -199,36 +172,20 @@ class FilePipeline {
         }
         // one size for every kind of pipeline of this code on this device (generate: k+m streams, rebuild: k + missing,
         // verify: k+2m), so that a parked ring fits whichever call comes next
-        slot_bytes_ = std::max(streams, size_t(enc_->k + 2 * enc_->m)) * chunk_;
+        const size_t slot_bytes = std::max(streams, size_t(enc_->k + 2 * enc_->m)) * chunk_;
         {
-            std::lock_guard<std::mutex> lk(slotset_mu());
-            auto& cache = slotset_cache();
-            for (size_t i = 0; i < cache.size(); i++)
-                if (cache[i].device == enc_->device && cache[i].bytes_per_slot == slot_bytes_ && cache[i].slots.size() == nslots) {
-                    slots_ = std::move(cache[i].slots);
-                    cache.erase(cache.begin() + long(i));
+            std::lock_guard<std::mutex> lk(parked_mu());
+            auto& parked = parked_rings();
+            for (size_t i = 0; i < parked.size(); i++)
+                if (parked[i].device == enc_->device && parked[i].bytes_per_slot == slot_bytes && parked[i].slots.size() == nslots) {
+                    ring_ = std::move(parked[i]);
+                    parked.erase(parked.begin() + long(i));
                     break;
                 }
         }
-        if (slots_.empty()) {
-            slots_.resize(nslots);
-            for (auto& s : slots_) {
-                s.host = static_cast<uint8_t*>(pinned_alloc(enc_->device, slot_bytes_));
-                cudaError_t e = s.host ? cudaSuccess : cudaErrorMemoryAllocation;
-                if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void**>(&s.dev), slot_bytes_);
-                if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking);
-                if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming);
-                if (e != cudaSuccess) {
-                    const int frc = s.host ? cuda_fail(e, "allocating the staging ring") : fail(SWEC_ERR_NOMEM, "cannot allocate pinned staging memory");
-                    free_slots(enc_->device, slots_);
-                    return frc;
-                }
-            }
-        }
-        for (auto& s : slots_) {
-            s.item = Item{};
-            free_.push_back(&s);
-        }
+        if (ring_.slots.empty() && (rc = ring_.allocate(enc_->device, nslots, slot_bytes))) return rc;
+        for (StagingSlot& b : ring_.slots) slots_.push_back({&b, Item{}});
+        for (Slot& s : slots_) free_.push_back(&s);
         io_ = &file_io_pool();
         writer_ = std::thread([this] { writer_loop(); });
         started_ = true;
@@ -246,6 +203,7 @@ class FilePipeline {
             s = free_.front();
             free_.pop_front();
         }
+        StagingSlot& b = *s->buf;
         double t1 = PipeStats::now();
         stats.wait_slot += t1 - t0;
         stats.items++;
@@ -261,7 +219,7 @@ class FilePipeline {
         const std::function<int(int)> read_one = [&](int idx) -> int {
             const Piece& pc = rpieces[size_t(idx)];
             const ReadOp& r = item.reads[size_t(pc.op)];
-            uint8_t* dst = s->host + size_t(r.stream) * chunk_ + r.dst_off + pc.off;
+            uint8_t* dst = b.host + size_t(r.stream) * chunk_ + r.dst_off + pc.off;
             const int64_t off = r.off + int64_t(pc.off);
             const size_t len = pc.len;
             // O_DIRECT: the device DMAs straight into the pinned slot; short counts only happen at EOF, where the
@@ -293,32 +251,32 @@ class FilePipeline {
         cudaError_t e = cudaSuccess;
         const uint8_t* din[SWEC_MAX_SHARDS];
         uint8_t* dout[SWEC_MAX_SHARDS];
-        for (int i = 0; i < K; i++) din[i] = s->dev + size_t(i) * chunk_;
+        for (int i = 0; i < K; i++) din[i] = b.dev + size_t(i) * chunk_;
         const int nin = K + (verify_ ? R : 0);
         if (len == chunk_) {  // full slot: the input streams are contiguous — one DMA
-            e = cudaMemcpyAsync(s->dev, s->host, size_t(nin) * chunk_, cudaMemcpyHostToDevice, s->stream);
+            e = cudaMemcpyAsync(b.dev, b.host, size_t(nin) * chunk_, cudaMemcpyHostToDevice, b.stream);
         } else {
             for (int i = 0; i < nin && e == cudaSuccess; i++)
-                e = cudaMemcpyAsync(s->dev + size_t(i) * chunk_, s->host + size_t(i) * chunk_, len, cudaMemcpyHostToDevice, s->stream);
+                e = cudaMemcpyAsync(b.dev + size_t(i) * chunk_, b.host + size_t(i) * chunk_, len, cudaMemcpyHostToDevice, b.stream);
         }
         if (e != cudaSuccess) return set_error(cuda_fail(e, "H2D"), s);
-        for (int r = 0; r < R; r++) dout[r] = s->dev + size_t(K + (verify_ ? R : 0) + r) * chunk_;
+        for (int r = 0; r < R; r++) dout[r] = b.dev + size_t(K + (verify_ ? R : 0) + r) * chunk_;
         int rc;
         {
             std::lock_guard<std::mutex> lk(enc_->mu);
-            rc = enc_->apply(rows_, din, dout, len, Layout{}, s->stream);
+            rc = enc_->apply(rows_, din, dout, len, Layout{}, b.stream);
         }
         if (rc) return set_error(rc, s);
         if (verify_) {
             for (int r = 0; r < R && e == cudaSuccess; r++)
-                e = launch_compare(dout[r], s->dev + size_t(K + r) * chunk_, len, dev_bad_ + r, s->stream);
+                e = launch_compare(dout[r], b.dev + size_t(K + r) * chunk_, len, dev_bad_ + r, b.stream);
         } else if (len == chunk_) {
-            e = cudaMemcpyAsync(s->host + size_t(K) * chunk_, dout[0], size_t(R) * chunk_, cudaMemcpyDeviceToHost, s->stream);
+            e = cudaMemcpyAsync(b.host + size_t(K) * chunk_, dout[0], size_t(R) * chunk_, cudaMemcpyDeviceToHost, b.stream);
         } else {
             for (int r = 0; r < R && e == cudaSuccess; r++)
-                e = cudaMemcpyAsync(s->host + size_t(K + r) * chunk_, dout[r], len, cudaMemcpyDeviceToHost, s->stream);
+                e = cudaMemcpyAsync(b.host + size_t(K + r) * chunk_, dout[r], len, cudaMemcpyDeviceToHost, b.stream);
         }
-        if (e == cudaSuccess) e = cudaEventRecord(s->done, s->stream);
+        if (e == cudaSuccess) e = cudaEventRecord(b.done, b.stream);
         if (e != cudaSuccess) return set_error(cuda_fail(e, "D2H"), s);
         s->item = std::move(item);
         {
@@ -361,26 +319,20 @@ class FilePipeline {
         io_ = nullptr;
         cudaSetDevice(enc_->device);
         bool healthy = error_ == 0;
-        for (auto& s : slots_)
-            if (s.stream && cudaStreamSynchronize(s.stream) != cudaSuccess) {
+        for (StagingSlot& b : ring_.slots)
+            if (cudaStreamSynchronize(b.stream) != cudaSuccess) {
                 cudaGetLastError();
                 healthy = false;
             }
         free_.clear();
         inflight_.clear();
-        if (healthy && !slots_.empty() && !getenv("SWEC_NO_RING_CACHE")) {  // park the ring for the next call
-            std::lock_guard<std::mutex> lk(slotset_mu());
-            auto& cache = slotset_cache();
-            if (cache.size() < kMaxCachedSlotSets) {
-                SlotSet set;
-                set.device = enc_->device;
-                set.bytes_per_slot = slot_bytes_;
-                set.slots = std::move(slots_);
-                cache.push_back(std::move(set));
-                slots_.clear();
-            }
+        slots_.clear();
+        if (healthy && !ring_.slots.empty() && !getenv("SWEC_NO_RING_CACHE")) {  // park the ring for the next call
+            std::lock_guard<std::mutex> lk(parked_mu());
+            auto& parked = parked_rings();
+            if (parked.size() < kMaxParkedRings) parked.push_back(std::move(ring_));  // leaves ring_ without slots
         }
-        if (!slots_.empty()) free_slots(enc_->device, slots_);
+        ring_.release();
         if (dev_bad_) cudaFree(dev_bad_);
         dev_bad_ = nullptr;
         started_ = false;
@@ -429,7 +381,7 @@ class FilePipeline {
             }
             int rc = SWEC_OK;
             const double tw0 = PipeStats::now();
-            if (cudaEventSynchronize(s->done) != cudaSuccess) rc = fail(SWEC_ERR_CUDA, "cudaEventSynchronize failed in the shard writer");
+            if (cudaEventSynchronize(s->buf->done) != cudaSuccess) rc = fail(SWEC_ERR_CUDA, "cudaEventSynchronize failed in the shard writer");
             const double tw1 = PipeStats::now();
             stats.wait_gpu += tw1 - tw0;   // writer thread only
             if (!rc) {
@@ -437,14 +389,14 @@ class FilePipeline {
                 std::vector<Piece> wpieces;
                 // one task per shard file: buffered writes take the inode's lock exclusively, so pieces of the same
                 // file would only queue behind each other (SWEC_FILE_WRITE_PIECE splits them anyway, for O_DIRECT devices)
-                const size_t wpiece = std::max<size_t>(4096, env_sz("SWEC_FILE_WRITE_PIECE", s->item.len ? s->item.len : 4096) & ~size_t(4095));
+                const size_t wpiece = std::max<size_t>(4096, env_size("SWEC_FILE_WRITE_PIECE", s->item.len ? s->item.len : 4096) & ~size_t(4095));
                 for (size_t i = 0; i < s->item.writes.size(); i++)
                     for (size_t o = 0; o < s->item.len; o += wpiece)
                         wpieces.push_back({int(i), o, std::min(wpiece, s->item.len - o)});
                 const std::function<int(int)> write_one = [&](int idx) -> int {
                     const Piece& pc = wpieces[size_t(idx)];
                     const WriteOp& w = s->item.writes[size_t(pc.op)];
-                    const uint8_t* src = s->host + size_t(w.stream) * chunk_ + pc.off;
+                    const uint8_t* src = s->buf->host + size_t(w.stream) * chunk_ + pc.off;
                     const int64_t off = w.off + int64_t(pc.off);
                     size_t put = 0;
                     while (put < pc.len) {
@@ -480,12 +432,12 @@ class FilePipeline {
     swec_encoder* enc_;
     Matrix rows_;
     size_t chunk_;
-    const size_t io_piece_ = std::max<size_t>(4096, env_sz("SWEC_FILE_IO_PIECE", size_t(2) << 20) & ~size_t(4095));
+    const size_t io_piece_ = std::max<size_t>(4096, env_size("SWEC_FILE_IO_PIECE", size_t(2) << 20) & ~size_t(4095));
     double t_begin_ = 0;
     bool verify_ = false;
     unsigned long long* dev_bad_ = nullptr;
-    std::vector<Slot> slots_;
-    size_t slot_bytes_ = 0;
+    StagingRing ring_;
+    std::vector<Slot> slots_;  // one per ring slot
     std::deque<Slot*> free_, inflight_;
     std::mutex mu_;
     std::condition_variable cv_;
@@ -502,12 +454,12 @@ class FilePipeline {
 }  // namespace
 
 void file_pipeline_trim() {  // swec_shutdown(): release parked staging rings
-    std::vector<SlotSet> sets;
+    std::vector<StagingRing> rings;
     {
-        std::lock_guard<std::mutex> lk(slotset_mu());
-        sets.swap(slotset_cache());
+        std::lock_guard<std::mutex> lk(parked_mu());
+        rings.swap(parked_rings());
     }
-    for (auto& set : sets) free_slots(set.device, set.slots);
+    for (StagingRing& r : rings) r.release();
 }
 
 }  // namespace swec
@@ -564,9 +516,8 @@ int swec_generate_ec_files(const char* base, int64_t buffer_size, int64_t large,
             }
     }
 
-    Matrix rows(m, k);
-    memcpy(rows.v.data(), enc->gen.row(k), rows.v.size());
-    const int64_t max_chunk = int64_t(env_sz("SWEC_FILE_CHUNK", size_t(8) << 20));
+    const Matrix rows = parity_rows(enc);
+    const int64_t max_chunk = int64_t(env_size("SWEC_FILE_CHUNK", size_t(8) << 20));
     const size_t chunk = size_t(std::min<int64_t>(max_chunk, std::max(large, small)) + 255) & ~size_t(255);
     const double t_opened = PipeStats::now();
     FilePipeline pipe(enc, rows, chunk);
@@ -730,7 +681,7 @@ int swec_rebuild_ec_files(const char* base, const char* const* dirs, int ndirs, 
     Matrix fused;
     if (!rs_reconstruct_plan(enc->gen, k, present.data(), false, &ins, &outs_idx, &fused))
         return fail(SWEC_ERR_TOO_FEW_SHARDS, "not enough shards");
-    const size_t chunk = std::max<size_t>(256, (size_t(std::min<int64_t>(int64_t(env_sz("SWEC_FILE_CHUNK", size_t(8) << 20)), std::max<int64_t>(todo, 1))) + 255) & ~size_t(255));
+    const size_t chunk = std::max<size_t>(256, (size_t(std::min<int64_t>(int64_t(env_size("SWEC_FILE_CHUNK", size_t(8) << 20)), std::max<int64_t>(todo, 1))) + 255) & ~size_t(255));
     FilePipeline pipe(enc, fused, chunk);
     if ((rc = pipe.start())) return rc;
     if (todo > 0 && worth_preallocating(out[size_t(outs_idx[0])]))
@@ -786,9 +737,8 @@ int swec_verify_ec_files(const char* base, const char* const* dirs, int ndirs, i
         else if (size != st.st_size)
             return fail(SWEC_ERR_SHARD_SIZE, "ec shard size expected " + std::to_string(size) + " actual " + std::to_string(st.st_size));
     }
-    Matrix rows(m, k);
-    memcpy(rows.v.data(), enc->gen.row(k), rows.v.size());
-    const size_t chunk = std::max<size_t>(256, (size_t(std::min<int64_t>(int64_t(env_sz("SWEC_FILE_CHUNK", size_t(8) << 20)), std::max<int64_t>(size, 1))) + 255) & ~size_t(255));
+    const Matrix rows = parity_rows(enc);
+    const size_t chunk = std::max<size_t>(256, (size_t(std::min<int64_t>(int64_t(env_size("SWEC_FILE_CHUNK", size_t(8) << 20)), std::max<int64_t>(size, 1))) + 255) & ~size_t(255));
     FilePipeline pipe(enc, rows, chunk, /*verify=*/true);
     if ((rc = pipe.start())) return rc;
     for (int64_t o = 0; rc == SWEC_OK && o < size; o += int64_t(chunk)) {

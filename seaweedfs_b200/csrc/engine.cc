@@ -12,7 +12,6 @@
 #include <execinfo.h>
 #include <signal.h>
 #include <sys/mman.h>
-#include <sys/syscall.h>
 #include <unistd.h>
 
 namespace swec {
@@ -62,7 +61,7 @@ int cuda_fail(cudaError_t e, const char* what) {
     return nodev ? SWEC_ERR_NO_DEVICE : SWEC_ERR_CUDA;
 }
 
-static size_t env_size(const char* name, size_t dflt) {
+size_t env_size(const char* name, size_t dflt) {
     const char* e = getenv(name);
     if (!e || !*e) return dflt;
     const long long v = atoll(e);
@@ -71,6 +70,7 @@ static size_t env_size(const char* name, size_t dflt) {
 
 std::atomic<long> g_opt_stage_chunk{long(env_size("SWEC_STAGE_CHUNK", size_t(16) << 20))};
 std::atomic<long> g_opt_stage_slots{long(env_size("SWEC_STAGE_SLOTS", 3))};
+size_t stage_slots() { return size_t(std::max(2l, g_opt_stage_slots.load())); }
 // Encoder-seam calls (swec_encode & co. on host buffers) are cut into at least this many pieces — never smaller
 // than host_min_chunk — so that the bounce copy / H2D of piece c+1, the kernel of piece c and the D2H / copy-back of
 // piece c-1 overlap INSIDE one call: the Go call sites hand over 256 KiB (encodeDataOneBatch) or 1 MiB
@@ -91,99 +91,6 @@ std::atomic<long> g_opt_file_direct_io{long(env_size("SWEC_FILE_DIRECT", 0)) & 3
 std::atomic<long> g_opt_jit_enabled{1};
 std::atomic<long> g_opt_jit_min_bytes{long(env_size("SWEC_JIT_MIN_BYTES", size_t(64) << 20))};
 
-// ------------------------------------------------------------------ NUMA-local pinned host memory
-// PCIe DMA from the far socket costs ~15-20 % of H2D bandwidth on two-socket hosts, so staging
-// memory is bound (mbind) to the NUMA node the GPU hangs off before it is pinned.
-
-static std::mutex g_pin_mu;
-static std::map<void*, size_t> g_pin_mapped;  // regions we mmap'ed + registered
-
-int device_numa_node(int device) {
-    char bus[32] = {0};
-    if (device < 0 || cudaDeviceGetPCIBusId(bus, sizeof bus, device) != cudaSuccess) {
-        cudaGetLastError();
-        return -1;
-    }
-    for (char* c = bus; *c; c++) *c = char(tolower(*c));
-    const std::string path = std::string("/sys/bus/pci/devices/") + bus + "/numa_node";
-    FILE* f = fopen(path.c_str(), "r");
-    if (!f) return -1;
-    int node = -1;
-    if (fscanf(f, "%d", &node) != 1) node = -1;
-    fclose(f);
-    return node;
-}
-
-// Pinned staging memory is carved out of 2 MiB-aligned anonymous mappings with MADV_HUGEPAGE: when several GPUs of one
-// socket DMA concurrently, every 4 KiB page is its own translation for the root complex / IOMMU, and the pages of a
-// huge page are physically contiguous, which DMA engines split less.  Best effort (the kernel may have THP off);
-// SWEC_NO_THP=1 keeps plain 4 KiB pages for A/B measurements.
-static void* map_aligned(size_t len, size_t* mapped_len) {
-    const size_t huge = size_t(2) << 20;
-    const bool thp = !getenv("SWEC_NO_THP") && len >= huge;
-    const size_t want = thp ? ((len + huge - 1) & ~(huge - 1)) : len;
-    const size_t span = thp ? want + huge : want;
-    uint8_t* raw = static_cast<uint8_t*>(mmap(nullptr, span, PROT_READ | PROT_WRITE, MAP_PRIVATE | MAP_ANONYMOUS, -1, 0));
-    if (raw == MAP_FAILED) return nullptr;
-    uint8_t* p = raw;
-    if (thp) {
-        p = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(raw) + huge - 1) & ~uintptr_t(huge - 1));
-        if (p > raw) munmap(raw, size_t(p - raw));
-        const size_t tail = size_t(raw + span - (p + want));
-        if (tail) munmap(p + want, tail);
-        madvise(p, want, MADV_HUGEPAGE);
-    }
-    *mapped_len = want;
-    return p;
-}
-
-void* pinned_alloc(int device, size_t bytes) {
-    if (bytes == 0) return nullptr;
-    const int node = getenv("SWEC_NO_NUMA") ? -1 : device_numa_node(device);
-    if (node >= 0 && node < 1024) {
-        size_t len = (bytes + 4095) & ~size_t(4095);
-        void* p = map_aligned(len, &len);
-        if (p) {
-            unsigned long mask[16] = {0};
-            mask[node / (8 * sizeof(unsigned long))] |= 1ul << (node % (8 * sizeof(unsigned long)));
-            // MPOL_PREFERRED (1): stay on the GPU's node when it has room, never fail the allocation
-            syscall(SYS_mbind, p, len, 1, mask, sizeof(mask) * 8, 0);
-            if (cudaHostRegister(p, len, cudaHostRegisterPortable | cudaHostRegisterMapped) == cudaSuccess) {
-                std::lock_guard<std::mutex> lk(g_pin_mu);
-                g_pin_mapped[p] = len;
-                return p;
-            }
-            cudaGetLastError();
-            munmap(p, len);
-        }
-    }
-    void* p = nullptr;
-    if (cudaHostAlloc(&p, bytes, cudaHostAllocPortable | cudaHostAllocMapped) != cudaSuccess) {
-        cudaGetLastError();
-        return nullptr;
-    }
-    return p;
-}
-
-void pinned_free(void* p) {
-    if (!p) return;
-    size_t len = 0;
-    {
-        std::lock_guard<std::mutex> lk(g_pin_mu);
-        auto it = g_pin_mapped.find(p);
-        if (it != g_pin_mapped.end()) {
-            len = it->second;
-            g_pin_mapped.erase(it);
-        }
-    }
-    if (len) {
-        cudaHostUnregister(p);
-        munmap(p, len);
-    } else {
-        cudaFreeHost(p);
-    }
-}
-
 // ------------------------------------------------------------------ encoder lifetime
 
 swec_encoder_impl::~swec_encoder_impl() {
@@ -193,13 +100,7 @@ swec_encoder_impl::~swec_encoder_impl() {
         cudaFree(kv.second.compact);
         cudaFree(kv.second.replicated);
     }
-    for (auto& s : slots) {
-        if (s.stream) cudaStreamSynchronize(s.stream);
-        if (s.host) pinned_free(s.host);
-        if (s.dev) cudaFree(s.dev);
-        if (s.done) cudaEventDestroy(s.done);
-        if (s.stream) cudaStreamDestroy(s.stream);
-    }
+    ring.release();
     if (stream) cudaStreamDestroy(stream);
 }
 
@@ -211,50 +112,14 @@ int swec_encoder_impl::ensure_device() {
 }
 
 int swec_encoder_impl::ensure_slots(size_t chunk) {
-    const size_t nslots = size_t(std::max(2l, g_opt_stage_slots.load()));
-    if (!slots.empty() && slot_chunk >= chunk && slots.size() == nslots) return SWEC_OK;
+    const size_t nslots = stage_slots(), streams = size_t(k) + 2 * size_t(m);
+    const size_t have = slot_chunk();
+    if (ring.slots.size() == nslots && have >= chunk) return SWEC_OK;
     // grow geometrically (callers with varying sizes must not re-pin memory on every larger call)
-    if (!slots.empty() && slot_chunk < chunk)
-        chunk = std::min(std::max(chunk, 2 * slot_chunk), std::max(chunk, size_t(g_opt_stage_chunk.load())));
+    if (!ring.slots.empty() && have < chunk)
+        chunk = std::min(std::max(chunk, 2 * have), std::max(chunk, size_t(g_opt_stage_chunk.load())));
     chunk = std::max<size_t>(chunk, 64 * 1024);
-    auto release = [&] {  // the ring is all-or-nothing: a half-built one must never look "big enough"
-        slot_chunk = 0;
-        for (auto& s : slots) {
-            if (s.stream) cudaStreamSynchronize(s.stream);
-            if (s.host) pinned_free(s.host);
-            if (s.dev) cudaFree(s.dev);
-            s.host = s.dev = s.host_dev = nullptr;
-            s.busy = false;
-        }
-    };
-    release();
-    for (size_t i = nslots; i < slots.size(); i++) {
-        if (slots[i].done) cudaEventDestroy(slots[i].done);
-        if (slots[i].stream) cudaStreamDestroy(slots[i].stream);
-    }
-    slots.resize(nslots);
-    const size_t streams = size_t(k) + 2 * size_t(m);
-    for (auto& s : slots) {
-        s.host = static_cast<uint8_t*>(pinned_alloc(device, streams * chunk));
-        s.host_dev = nullptr;
-        cudaError_t e = s.host ? cudaSuccess : cudaErrorMemoryAllocation;
-        if (e == cudaSuccess && cudaHostGetDevicePointer(reinterpret_cast<void**>(&s.host_dev), s.host, 0) != cudaSuccess) {
-            cudaGetLastError();
-            s.host_dev = nullptr;  // not mapped: the ring still works through DMA
-        }
-        if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void**>(&s.dev), streams * chunk);
-        if (e == cudaSuccess && !s.stream) e = cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking);
-        if (e == cudaSuccess && !s.done) e = cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming);
-        if (e != cudaSuccess) {
-            const bool no_host = !s.host;
-            release();
-            cudaGetLastError();
-            return no_host ? fail(SWEC_ERR_NOMEM, "cannot allocate pinned staging memory") : cuda_fail(e, "allocating the staging ring");
-        }
-        s.busy = false;
-    }
-    slot_chunk = chunk;
-    return SWEC_OK;
+    return ring.allocate(device, nslots, streams * chunk);
 }
 
 // ------------------------------------------------------------------ tables
@@ -407,18 +272,6 @@ int swec_encoder_impl::apply(const Matrix& rows, const uint8_t* const* in, uint8
 
 namespace {
 
-// Whatever way a host-path call ends, no DMA may still be aimed at the caller's buffers when it
-// returns ("nothing is retained after a call returns", include/swec.h).
-struct DrainSlotsOnExit {
-    swec_encoder_impl* e;
-    ~DrainSlotsOnExit() {
-        for (StagingSlot& s : e->slots)
-            if (s.busy) {
-                if (s.stream) cudaStreamSynchronize(s.stream);
-                s.busy = false;
-            }
-    }
-};
 struct DeviceCounter {
     unsigned long long* p = nullptr;
     ~DeviceCounter() {
@@ -483,6 +336,23 @@ void parallel_copy(const std::vector<CopyJob>& jobs) {
     };
     pool->parallel_for(int(pieces.size()), one);
 }
+
+// The turn both host pipelines take on the ring: the copy-backs of the piece a slot carries wait in `pending` until the
+// slot's event fires; finish(si) then runs them and frees the slot for its next piece.
+struct SlotTurns {
+    StagingRing& ring;
+    std::vector<std::vector<CopyJob>> pending;
+    explicit SlotTurns(StagingRing& r) : ring(r), pending(r.slots.size()) {}
+    int finish(size_t si) {
+        StagingSlot& s = ring.slots[si];
+        if (!s.busy) return SWEC_OK;
+        SWEC_CUDA(cudaEventSynchronize(s.done));
+        parallel_copy(pending[si]);
+        pending[si].clear();
+        s.busy = false;
+        return SWEC_OK;
+    }
+};
 
 // p[0..n) equally spaced (the k+m slices of ONE allocation, e.g. swec_alloc_pinned_for_device carved up by the caller)?
 bool constant_pitch(const uint8_t* const* p, int n, size_t min_pitch, size_t* pitch) {
@@ -559,9 +429,10 @@ static int apply_host(swec_encoder_impl* e, const Matrix& rows, const uint8_t* c
     chunk = std::min(chunk, (n + 255) & ~size_t(255));
     rc = e->ensure_slots(chunk);
     if (rc) return rc;
-    const size_t stride = e->slot_chunk;  // per-stream pitch inside a slot (>= chunk)
+    const size_t stride = e->slot_chunk();  // per-stream pitch inside a slot (>= chunk)
+    StagingRing& ring = e->ring;
 
-    DrainSlotsOnExit drain{e};
+    StagingRing::DrainOnExit drain{ring};
     DeviceCounter counter;
     if (check) {
         SWEC_CUDA(cudaMalloc(reinterpret_cast<void**>(&counter.p), 8));
@@ -569,16 +440,7 @@ static int apply_host(swec_encoder_impl* e, const Matrix& rows, const uint8_t* c
     }
     unsigned long long* const dev_bad = counter.p;
 
-    std::vector<std::vector<CopyJob>> pending(e->slots.size());
-    auto finish = [&](size_t si) -> int {
-        StagingSlot& s = e->slots[si];
-        if (!s.busy) return SWEC_OK;
-        SWEC_CUDA(cudaEventSynchronize(s.done));
-        parallel_copy(pending[si]);
-        pending[si].clear();
-        s.busy = false;
-        return SWEC_OK;
-    };
+    SlotTurns turns(ring);
 
     bool all_in_bounced = true, all_out_bounced = !check, all_in_direct = true, all_out_direct = !check;
     for (int i = 0; i < K; i++) {
@@ -598,9 +460,9 @@ static int apply_host(swec_encoder_impl* e, const Matrix& rows, const uint8_t* c
     std::vector<CopyJob> bounce;
     size_t ci = 0;
     for (size_t off = 0; off < n; off += chunk, ci++) {
-        const size_t si = ci % e->slots.size();
-        StagingSlot& s = e->slots[si];
-        if ((rc = finish(si))) break;
+        const size_t si = ci % ring.slots.size();
+        StagingSlot& s = ring.slots[si];
+        if ((rc = turns.finish(si))) break;
         const size_t len = std::min(chunk, n - off);
         // Pageable callers (Go heap memory) bounce through the slot anyway, so pack the streams at a
         // pitch that fits this piece: one DMA in, one DMA out instead of k + m small ones.
@@ -619,7 +481,7 @@ static int apply_host(swec_encoder_impl* e, const Matrix& rows, const uint8_t* c
             for (int i = 0; i < K; i++) din[i] = s.host_dev + size_t(i) * pitch;
             for (int r = 0; r < R; r++) dout[r] = s.host_dev + size_t(K + r) * pitch;
             if ((rc = e->apply(rows, din, dout, len, Layout{}, s.stream))) break;
-            for (int r = 0; r < R; r++) pending[si].push_back({out[r] + off, s.host + size_t(K + r) * pitch, len});
+            for (int r = 0; r < R; r++) turns.pending[si].push_back({out[r] + off, s.host + size_t(K + r) * pitch, len});
             SWEC_CUDA(cudaEventRecord(s.done, s.stream));
             s.busy = true;
             continue;
@@ -639,7 +501,7 @@ static int apply_host(swec_encoder_impl* e, const Matrix& rows, const uint8_t* c
         if (packed) {
             SWEC_CUDA(cudaMemcpyAsync(s.host + size_t(K) * pitch, dout[0], size_t(R - 1) * pitch + len,
                                       cudaMemcpyDeviceToHost, s.stream));
-            for (int r = 0; r < R; r++) pending[si].push_back({out[r] + off, s.host + size_t(K + r) * pitch, len});
+            for (int r = 0; r < R; r++) turns.pending[si].push_back({out[r] + off, s.host + size_t(K + r) * pitch, len});
         } else if (out_2d) {
             SWEC_CUDA(cudaMemcpy2DAsync(out[0] + off, out_pitch, dout[0], pitch, len, size_t(R), cudaMemcpyDefault, s.stream));
         } else {
@@ -660,17 +522,16 @@ static int apply_host(swec_encoder_impl* e, const Matrix& rows, const uint8_t* c
                 } else {
                     uint8_t* back = s.host + size_t(K + r) * stride;
                     SWEC_CUDA(cudaMemcpyAsync(back, dout[r], len, cudaMemcpyDeviceToHost, s.stream));
-                    pending[si].push_back({out[r] + off, back, len});
+                    turns.pending[si].push_back({out[r] + off, back, len});
                 }
             }
         }
         SWEC_CUDA(cudaEventRecord(s.done, s.stream));
         s.busy = true;
     }
-    for (size_t i = 0; i < e->slots.size(); i++) {
+    for (size_t i = 0; i < ring.slots.size(); i++) {
         // drain in submission order so that copy-backs of early pieces overlap the GPU work of late ones
-        const size_t si = (ci + i) % e->slots.size();
-        const int rc2 = finish(si);
+        const int rc2 = turns.finish((ci + i) % ring.slots.size());
         if (!rc) rc = rc2;
     }
     if (check && !rc && cudaMemcpy(check, dev_bad, 8, cudaMemcpyDeviceToHost) != cudaSuccess)
@@ -688,8 +549,8 @@ static size_t packed_max_bytes() {
 // back to back (each padded to 16 bytes) into slot-sized launches so the per-call costs — stream
 // round trip, launch, DMA set-up — are paid once per ~chunk instead of once per needle.
 struct Segment {
-    const uint8_t* const* in;  // K pointers
-    uint8_t* const* out;       // R pointers
+    std::vector<const uint8_t*> in;  // K pointers
+    std::vector<uint8_t*> out;       // R pointers
     size_t len;
 };
 
@@ -706,24 +567,14 @@ static int apply_host_packed(swec_encoder_impl* e, const Matrix& rows, const std
     for (const Segment& sg : segs) packed += (sg.len + 15) & ~size_t(15);
     const size_t chunk = std::min(max_chunk, (packed + 65535) & ~size_t(65535));
     if ((rc = e->ensure_slots(chunk))) return rc;
-    const size_t stride = e->slot_chunk;
-    DrainSlotsOnExit drain{e};
-
-    struct Unpack { uint8_t* dst; const uint8_t* src; size_t len; };
-    std::vector<std::vector<Unpack>> pending(e->slots.size());
-    auto finish = [&](size_t si) -> int {
-        StagingSlot& sl = e->slots[si];
-        if (!sl.busy) return SWEC_OK;
-        SWEC_CUDA(cudaEventSynchronize(sl.done));
-        for (const Unpack& u : pending[si]) memcpy(u.dst, u.src, u.len);
-        pending[si].clear();
-        sl.busy = false;
-        return SWEC_OK;
-    };
+    const size_t stride = e->slot_chunk();
+    StagingRing& ring = e->ring;
+    StagingRing::DrainOnExit drain{ring};
+    SlotTurns turns(ring);
     size_t si = 0, fill = 0, nflush = 0;
     auto flush = [&]() -> int {
         if (fill == 0) return SWEC_OK;
-        StagingSlot& sl = e->slots[si];
+        StagingSlot& sl = ring.slots[si];
         const uint8_t* din[SWEC_MAX_INPUTS];
         uint8_t* dout[SWEC_MAX_SHARDS];
         const long zc_mode = g_opt_host_zero_copy.load();
@@ -750,8 +601,8 @@ static int apply_host_packed(swec_encoder_impl* e, const Matrix& rows, const std
         SWEC_CUDA(cudaEventRecord(sl.done, sl.stream));
         sl.busy = true;
         fill = 0;
-        si = (++nflush) % e->slots.size();
-        return finish(si);  // the slot we are about to fill must be drained
+        si = (++nflush) % ring.slots.size();
+        return turns.finish(si);  // the slot we are about to fill must be drained
     };
     for (const Segment& sg : segs) {
         const size_t padded = (sg.len + 15) & ~size_t(15);
@@ -759,18 +610,52 @@ static int apply_host_packed(swec_encoder_impl* e, const Matrix& rows, const std
             return fail(SWEC_ERR_INVALID_ARG, "batched interval larger than the staging chunk");
         }
         if (fill + padded > stride && (rc = flush())) return rc;
-        StagingSlot& sl = e->slots[si];
+        StagingSlot& sl = ring.slots[si];
         for (int i = 0; i < K; i++) {
             uint8_t* dst = sl.host + size_t(i) * stride + fill;
             memcpy(dst, sg.in[i], sg.len);
             if (padded > sg.len) memset(dst + sg.len, 0, padded - sg.len);
         }
-        for (int r = 0; r < R; r++) pending[si].push_back({sg.out[r], sl.host + size_t(K + r) * stride + fill, sg.len});
+        for (int r = 0; r < R; r++) turns.pending[si].push_back({sg.out[r], sl.host + size_t(K + r) * stride + fill, sg.len});
         fill += padded;
     }
     if ((rc = flush())) return rc;
-    for (size_t i = 0; i < e->slots.size(); i++)
-        if ((rc = finish(i))) return rc;
+    for (size_t i = 0; i < ring.slots.size(); i++)
+        if ((rc = turns.finish(i))) return rc;
+    return SWEC_OK;
+}
+
+Matrix parity_rows(const swec_encoder_impl* e) {
+    Matrix rows(e->m, e->k);
+    memcpy(rows.v.data(), e->gen.row(e->k), rows.v.size());
+    return rows;
+}
+
+// What a reconstruct call rebuilds, decided once from the presence mask: the fused matrix, the shards it reads and the
+// shards it writes (none when every shard is present, or when only parity is missing and data_only is set).
+struct ReconstructPlan {
+    bool all_present = false;
+    std::vector<int> ins, outs;
+    Matrix fused;
+
+    // the caller's buffers of the plan's inputs and outputs; every shard to rebuild needs one
+    int gather(uint8_t* const* shards, const uint8_t** in, uint8_t** out) const {
+        for (size_t i = 0; i < ins.size(); i++) in[i] = shards[ins[i]];
+        for (size_t i = 0; i < outs.size(); i++) {
+            out[i] = shards[outs[i]];
+            if (!out[i]) return fail(SWEC_ERR_INVALID_ARG, "missing shard has no buffer");
+        }
+        return SWEC_OK;
+    }
+};
+
+static int plan_reconstruct(const swec_encoder_impl* e, const uint8_t* present, int data_only, ReconstructPlan* p) {
+    int npresent = 0;
+    for (int i = 0; i < e->k + e->m; i++) npresent += present[i] ? 1 : 0;
+    p->all_present = npresent == e->k + e->m;
+    if (p->all_present) return SWEC_OK;
+    if (npresent < e->k || !rs_reconstruct_plan(e->gen, e->k, present, data_only != 0, &p->ins, &p->outs, &p->fused))
+        return fail(SWEC_ERR_TOO_FEW_SHARDS, "fewer than data_shards shards present");
     return SWEC_OK;
 }
 
@@ -831,7 +716,7 @@ int swec_device_spread_order(int* order, int capacity, int* count) {
         return fail(SWEC_ERR_NO_DEVICE, "no CUDA devices");
     }
     std::map<int, std::vector<int>> by_node;  // node → devices, both ascending
-    for (int d = 0; d < n; d++) by_node[getenv("SWEC_NO_NUMA") ? -1 : device_numa_node(d)].push_back(d);
+    for (int d = 0; d < n; d++) by_node[device_numa_node(d)].push_back(d);
     std::vector<int> out;
     for (size_t round = 0; out.size() < size_t(n); round++)
         for (auto& kv : by_node)
@@ -933,12 +818,6 @@ int swec_reconstruct_matrix(const swec_encoder* e, const uint8_t* present, int d
     return SWEC_OK;
 }
 
-static Matrix parity_rows(const swec_encoder* e) {
-    Matrix rows(e->m, e->k);
-    memcpy(rows.v.data(), e->gen.row(e->k), rows.v.size());
-    return rows;
-}
-
 int swec_encode(swec_encoder* e, uint8_t* const* shards, size_t n) {
     if (!e || !shards) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
     if (n == 0) return fail(SWEC_ERR_INVALID_ARG, "shard_len is 0 (ErrShardNoData)");
@@ -949,24 +828,15 @@ int swec_encode(swec_encoder* e, uint8_t* const* shards, size_t n) {
 
 int swec_reconstruct(swec_encoder* e, uint8_t* const* shards, const uint8_t* present, size_t n, int data_only) {
     if (!e || !shards || !present) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
-    int npresent = 0;
-    for (int i = 0; i < e->k + e->m; i++) npresent += present[i] ? 1 : 0;
-    if (npresent == e->k + e->m) return SWEC_OK;  // nothing to do
-    if (npresent < e->k) return fail(SWEC_ERR_TOO_FEW_SHARDS, "fewer than data_shards shards present");
+    ReconstructPlan p;
+    int rc = plan_reconstruct(e, present, data_only, &p);
+    if (rc || p.all_present) return rc;
     if (n == 0) return fail(SWEC_ERR_INVALID_ARG, "shard_len is 0 (ErrShardNoData)");
-    std::vector<int> in, outv;
-    Matrix fused;
-    if (!rs_reconstruct_plan(e->gen, e->k, present, data_only != 0, &in, &outv, &fused))
-        return fail(SWEC_ERR_TOO_FEW_SHARDS, "fewer than data_shards shards present");
-    if (outv.empty()) return SWEC_OK;
+    if (p.outs.empty()) return SWEC_OK;
     const uint8_t* ins[SWEC_MAX_SHARDS];
     uint8_t* outs[SWEC_MAX_SHARDS];
-    for (size_t i = 0; i < in.size(); i++) ins[i] = shards[in[i]];
-    for (size_t i = 0; i < outv.size(); i++) {
-        outs[i] = shards[outv[i]];
-        if (!outs[i]) return fail(SWEC_ERR_INVALID_ARG, "missing shard has no buffer");
-    }
-    return apply_host(e, fused, ins, outs, n, nullptr);
+    if ((rc = p.gather(shards, ins, outs))) return rc;
+    return apply_host(e, p.fused, ins, outs, n, nullptr);
 }
 
 int swec_reconstruct_batch(swec_encoder* e, const swec_reconstruct_item* items, int n_items) {
@@ -975,58 +845,37 @@ int swec_reconstruct_batch(swec_encoder* e, const swec_reconstruct_item* items, 
     const size_t chunk = swec::packed_max_bytes();
     // group by (presence mask, data_only); big items take the ordinary streaming path
     struct Group {
-        std::vector<int> ins, outs;
-        Matrix fused;
+        ReconstructPlan plan;
         std::vector<Segment> segs;
-        std::vector<std::vector<const uint8_t*>> in_ptrs;
-        std::vector<std::vector<uint8_t*>> out_ptrs;
     };
     std::map<std::vector<uint8_t>, Group> groups;
     for (int it = 0; it < n_items; it++) {
         const swec_reconstruct_item& item = items[it];
         if (!item.shards || !item.present) return fail(SWEC_ERR_INVALID_ARG, "NULL item field");
-        int npresent = 0;
-        for (int i = 0; i < total; i++) npresent += item.present[i] ? 1 : 0;
-        if (npresent == total) continue;
-        if (npresent < e->k) return fail(SWEC_ERR_TOO_FEW_SHARDS, "fewer than data_shards shards present");
-        if (item.shard_len == 0) return fail(SWEC_ERR_INVALID_ARG, "shard_len is 0 (ErrShardNoData)");
-        if (((item.shard_len + 15) & ~size_t(15)) > chunk) {
-            const int rc = swec_reconstruct(e, item.shards, item.present, item.shard_len, item.data_only);
-            if (rc) return rc;
-            continue;
-        }
         std::vector<uint8_t> key(item.present, item.present + total);
         for (auto& b : key) b = b ? 1 : 0;
         key.push_back(item.data_only ? 1 : 0);
         auto found = groups.find(key);
         if (found == groups.end()) {
             Group g;
-            if (!rs_reconstruct_plan(e->gen, e->k, key.data(), item.data_only != 0, &g.ins, &g.outs, &g.fused))
-                return fail(SWEC_ERR_TOO_FEW_SHARDS, "fewer than data_shards shards present");
+            if (const int rc = plan_reconstruct(e, key.data(), item.data_only, &g.plan)) return rc;
             found = groups.emplace(key, std::move(g)).first;
         }
         Group& g = found->second;
-        if (g.outs.empty()) continue;
-        std::vector<const uint8_t*> ip;
-        std::vector<uint8_t*> op;
-        for (int idx : g.ins) ip.push_back(item.shards[idx]);
-        for (int idx : g.outs) {
-            if (!item.shards[idx]) return fail(SWEC_ERR_INVALID_ARG, "missing shard has no buffer");
-            op.push_back(item.shards[idx]);
+        if (g.plan.all_present) continue;
+        if (item.shard_len == 0) return fail(SWEC_ERR_INVALID_ARG, "shard_len is 0 (ErrShardNoData)");
+        if (((item.shard_len + 15) & ~size_t(15)) > chunk) {
+            const int rc = swec_reconstruct(e, item.shards, item.present, item.shard_len, item.data_only);
+            if (rc) return rc;
+            continue;
         }
-        g.in_ptrs.push_back(std::move(ip));
-        g.out_ptrs.push_back(std::move(op));
-        g.segs.push_back({nullptr, nullptr, item.shard_len});
+        if (g.plan.outs.empty()) continue;
+        Segment sg{std::vector<const uint8_t*>(g.plan.ins.size()), std::vector<uint8_t*>(g.plan.outs.size()), item.shard_len};
+        if (const int rc = g.plan.gather(item.shards, sg.in.data(), sg.out.data())) return rc;
+        g.segs.push_back(std::move(sg));
     }
-    for (auto& kv : groups) {
-        Group& g = kv.second;
-        for (size_t i = 0; i < g.segs.size(); i++) {  // pointer tables are stable now
-            g.segs[i].in = g.in_ptrs[i].data();
-            g.segs[i].out = g.out_ptrs[i].data();
-        }
-        const int rc = apply_host_packed(e, g.fused, g.segs);
-        if (rc) return rc;
-    }
+    for (auto& kv : groups)
+        if (const int rc = apply_host_packed(e, kv.second.plan.fused, kv.second.segs)) return rc;
     return SWEC_OK;
 }
 
@@ -1113,25 +962,16 @@ int swec_alloc_pinned_shards(swec_encoder* const* encs, int n_encs, int n_shards
     void* base = mmap(nullptr, total, PROT_READ | PROT_WRITE, MAP_PRIVATE | MAP_ANONYMOUS, -1, 0);
     if (base == MAP_FAILED) return fail(SWEC_ERR_NOMEM, "mmap of the shard buffers failed");
     const std::vector<size_t> begin = column_split(n_encs, shard_len);
-    if (!getenv("SWEC_NO_NUMA"))
-        for (int g = 0; g < n_encs; g++) {
-            const int node = device_numa_node(encs[g]->device);
-            if (node < 0 || node >= 1024) continue;
-            unsigned long mask[16] = {0};
-            mask[size_t(node) / (8 * sizeof(unsigned long))] |= 1ul << (size_t(node) % (8 * sizeof(unsigned long)));
-            // the end of the last range is rounded up to the page so that the tail page has a home too
-            const size_t lo = begin[size_t(g)], hi = g + 1 == n_encs ? pitch : begin[size_t(g) + 1];
-            for (int i = 0; i < n_shards && hi > lo; i++)  // MPOL_PREFERRED (1): never fails the allocation
-                syscall(SYS_mbind, static_cast<uint8_t*>(base) + size_t(i) * pitch + lo, hi - lo, 1, mask, sizeof(mask) * 8, 0);
-        }
-    const cudaError_t e = cudaHostRegister(base, total, cudaHostRegisterPortable | cudaHostRegisterMapped);
+    for (int g = 0; g < n_encs; g++) {
+        const int node = device_numa_node(encs[g]->device);
+        // the end of the last range is rounded up to the page so that the tail page has a home too
+        const size_t lo = begin[size_t(g)], hi = g + 1 == n_encs ? pitch : begin[size_t(g) + 1];
+        for (int i = 0; i < n_shards && hi > lo; i++) bind_to_node(static_cast<uint8_t*>(base) + size_t(i) * pitch + lo, hi - lo, node);
+    }
+    const cudaError_t e = register_mapped(base, total);
     if (e != cudaSuccess) {
         munmap(base, total);
         return cuda_fail(e, "cudaHostRegister of the shard buffers");
-    }
-    {
-        std::lock_guard<std::mutex> lk(g_pin_mu);
-        g_pin_mapped[base] = total;
     }
     for (int i = 0; i < n_shards; i++) shards[i] = static_cast<uint8_t*>(base) + size_t(i) * pitch;
     return SWEC_OK;
@@ -1142,14 +982,13 @@ int swec_reconstruct_multi(swec_encoder* const* encs, int n_encs, uint8_t* const
     int rc = check_group(encs, n_encs);
     if (rc) return rc;
     if (!shards || !present) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
-    const int k = encs[0]->k, total = k + encs[0]->m;
-    int npresent = 0;
-    for (int i = 0; i < total; i++) npresent += present[i] ? 1 : 0;
-    if (npresent == total) return SWEC_OK;
-    if (npresent < k) return fail(SWEC_ERR_TOO_FEW_SHARDS, "fewer than data_shards shards present");
+    const int total = encs[0]->k + encs[0]->m;
+    ReconstructPlan p;
+    if ((rc = plan_reconstruct(encs[0], present, data_only, &p)) || p.all_present) return rc;
     if (n == 0) return fail(SWEC_ERR_INVALID_ARG, "shard_len is 0 (ErrShardNoData)");
-    for (int i = 0; i < total; i++)
-        if (!present[i] && (i < k || !data_only) && !shards[i]) return fail(SWEC_ERR_INVALID_ARG, "missing shard has no buffer");
+    const uint8_t* ins[SWEC_MAX_SHARDS];
+    uint8_t* outs[SWEC_MAX_SHARDS];
+    if ((rc = p.gather(shards, ins, outs))) return rc;
     return split_columns(n_encs, n, [&](int g, size_t off, size_t len) {
         uint8_t* sub[SWEC_MAX_SHARDS];
         for (int i = 0; i < total; i++) sub[i] = shards[i] ? shards[i] + off : nullptr;
@@ -1183,19 +1022,15 @@ int swec_encode_device(swec_encoder* e, const void* const* data, void* const* pa
 int swec_reconstruct_device(swec_encoder* e, void* const* shards, const uint8_t* present, size_t n, int data_only,
                             void* stream) {
     if (!e || !shards || !present) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
-    std::vector<int> in, outv;
-    Matrix fused;
-    if (!rs_reconstruct_plan(e->gen, e->k, present, data_only != 0, &in, &outv, &fused))
-        return fail(SWEC_ERR_TOO_FEW_SHARDS, "fewer than data_shards shards present");
-    if (outv.empty()) return SWEC_OK;
+    ReconstructPlan p;
+    int rc = plan_reconstruct(e, present, data_only, &p);
+    if (rc || p.outs.empty()) return rc;
     const uint8_t* ins[SWEC_MAX_SHARDS];
     uint8_t* outs[SWEC_MAX_SHARDS];
-    for (size_t i = 0; i < in.size(); i++) ins[i] = static_cast<const uint8_t*>(shards[in[i]]);
-    for (size_t i = 0; i < outv.size(); i++) outs[i] = static_cast<uint8_t*>(shards[outv[i]]);
+    if ((rc = p.gather(reinterpret_cast<uint8_t* const*>(shards), ins, outs))) return rc;
     std::lock_guard<std::mutex> lock(e->mu);
-    int rc = e->ensure_device();
-    if (rc) return rc;
-    return e->apply(fused, ins, outs, n, Layout{}, pick_stream(e, stream));
+    if ((rc = e->ensure_device())) return rc;
+    return e->apply(p.fused, ins, outs, n, Layout{}, pick_stream(e, stream));
 }
 
 int swec_apply_device(swec_encoder* e, int r, int k, const uint8_t* rows, const void* const* in, void* const* out,

@@ -18,6 +18,7 @@
 #include "../../include/swec.h"
 #include "gf256.h"
 #include "kernels.h"
+#include "staging.h"
 
 namespace swec {
 
@@ -32,10 +33,8 @@ int cuda_fail(cudaError_t e, const char* what);
         if (e__ != cudaSuccess) return cuda_fail(e__, #call); \
     } while (0)
 
-// pinned host memory on the NUMA node of `device` (plain cudaHostAlloc when that is unknown)
-void* pinned_alloc(int device, size_t bytes);
-void pinned_free(void* p);
-int device_numa_node(int device);
+size_t env_size(const char* name, size_t dflt);  // a positive integer from the environment, else dflt
+size_t stage_slots();  // "stage_slots" (SWEC_STAGE_SLOTS): slots of every staging ring, at least 2
 
 // "file_direct_io" (SWEC_FILE_DIRECT): bit 0 = O_DIRECT reads of the .dat / shard inputs straight into the pinned
 // ring, bit 1 = O_DIRECT writes of the shard outputs — the page cache is bypassed both ways (disk-backed volumes only;
@@ -51,15 +50,6 @@ struct DeviceTables {
 
 struct JitKernel;  // jit.cc
 
-struct StagingSlot {
-    uint8_t* host = nullptr;      // pinned, (k+2m)*chunk
-    uint8_t* host_dev = nullptr;  // the same memory as the GPU addresses it (mapped pinned memory), or nullptr
-    uint8_t* dev = nullptr;       // (k+2m)*chunk
-    cudaStream_t stream = nullptr;
-    cudaEvent_t done = nullptr;
-    bool busy = false;
-};
-
 struct Layout {  // how stream i / column x maps to memory; see SwecApplyParams
     bool blocked = false;
     uint64_t block_bytes = 0;
@@ -74,8 +64,7 @@ struct swec_encoder_impl {
     cudaStream_t stream = nullptr;
     std::map<std::vector<uint8_t>, DeviceTables> tables;  // key: R, K, coefficients
     std::map<std::vector<uint8_t>, std::shared_ptr<JitKernel>> jit;  // same key
-    std::vector<StagingSlot> slots;
-    size_t slot_chunk = 0;
+    StagingRing ring;  // (k+2m) streams of slot_chunk() bytes per slot
     // file pipelines never stall on a kernel compile: a cold matrix is served by the table kernel (100x faster
     // than the I/O around it) while the specialised kernel is built in the background and picked up when ready
     bool never_wait_for_jit = false;
@@ -83,12 +72,15 @@ struct swec_encoder_impl {
     ~swec_encoder_impl();
     int ensure_device();  // cudaSetDevice + lazily create stream
     int ensure_slots(size_t chunk);
+    size_t slot_chunk() const { return ring.bytes_per_slot / (size_t(k) + 2 * size_t(m)); }
 
     // out[r][x] = XOR_i rows[r][i] ⊗ in[i][x] on device memory, asynchronous on s.
     int apply(const Matrix& rows, const uint8_t* const* in, uint8_t* const* out, size_t n,
               const Layout& layout, cudaStream_t s);
     int get_tables(const Matrix& rows4, DeviceTables* out, cudaStream_t s);
 };
+
+Matrix parity_rows(const swec_encoder_impl* e);  // the m parity rows of the generator
 
 // true when run-time specialised kernels can be had: NVRTC loaded (SWEC_NO_JIT unset), or the on-disk cubin cache is on
 bool jit_available();

@@ -143,6 +143,9 @@ def test_argument_validation(swec, tmp_path):
     with pytest.raises(swec.SwecError) as e:
         enc.extract_data_shard_device(1, -1, 0, 1)                         # negative .dat size, before any device work
     assert e.value.name == "SWEC_ERR_INVALID_ARG"
+    with pytest.raises(swec.SwecError) as e:                              # a shard to rebuild without a buffer, before
+        enc.reconstruct_device([None] + [1 << 20] * 13, [0] + [1] * 13, 4096)  # any device work
+    assert e.value.name == "SWEC_ERR_INVALID_ARG"
 
 
 def test_set_option_validation(swec):
