@@ -25,6 +25,8 @@
  *   swec_ec_shards_to_volume    VolumeEcShardsToVolume (file work)   weed/server/volume_grpc_erasure_coding.go:578-668
  *   swec_read_ec_needles        Store.ReadEcShardNeedle (local shards, batched)   weed/storage/store_ec.go:252-355,482-560
  *   swec_check_index_file       idx.CheckIndexFile / EcVolume.ScrubIndex   weed/storage/idx/check.go:36-111
+ *   swec_check_needles_device   Needle.ReadBytes on records in HBM   weed/storage/needle/needle_read.go:59-190,
+ *                                                          needle_read_tail.go:11-34, crc.go:12-22
  *   swec_ec_volume_*            EcVolume: mount, ReadEcShardNeedle, DeleteNeedleFromEcx, FileAndDeleteCount, ScrubLocal
  *                                                          weed/storage/erasure_coding/ec_volume.go, ec_volume_delete.go, ec_volume_scrub.go
  *   swec_locate_data            LocateData                weed/storage/erasure_coding/ec_locate.go:16-53
@@ -274,9 +276,18 @@ int swec_ec_volume_delete_needle(swec_ec_volume *vol, uint64_t needle_id);
  * .ecx), then every live entry is located and each of its chunks read from the local shard that should hold it.
  * broken_shards[SWEC_MAX_SHARDS] receives the ids (ascending) of shards that were too short or unreadable for some
  * chunk; findings are newline-separated in errors[], worded like the reference.  Parity is checked by
- * swec_verify_ec_files, record CRCs by the storage engine.                                                    */
+ * swec_verify_ec_files; swec_ec_volume_scrub_needles adds the needle parse.  No GPU work.                     */
 int swec_ec_volume_scrub_local(swec_ec_volume *vol, int64_t *entries, uint32_t *broken_shards, int *n_broken,
                                char *errors, size_t errors_cap, int *n_errors);
+/* The whole EcVolume.ScrubLocal: the walk of swec_ec_volume_scrub_local, and every record whose chunks are all local
+ * is checked like Needle.ReadBytes (size, layout, CRC32-C) on the GPU of the volume's device.  Records are read
+ * straight into pinned staging slots and checked a slot at a time while the walk fills the next slot.  A failed
+ * record adds "needle <id> on volume <volume_id>: <err>" after the findings of the records walked before it, with
+ * <err> as ReadBytes words it ("size mismatch", "index out of range N: needle data corrupted", "invalid CRC for
+ * needle <hex id> (got %08x, want %08x), data on disk corrupted: needle data corrupted").  A walk with nothing to
+ * check does no GPU work; otherwise a volume opened with device < 0 fails with SWEC_ERR_NO_DEVICE.           */
+int swec_ec_volume_scrub_needles(swec_ec_volume *vol, uint32_t volume_id, int64_t *entries, uint32_t *broken_shards,
+                                 int *n_broken, char *errors, size_t errors_cap, int *n_errors);
 /* What mounting derived (NewEcVolume, ec_volume.go:114-154,399-417): EC ratio and needle version from .vif (defaults
  * 10+4, version 3), the shard size LocateData works with, and a bit per shard file found locally.  Any out pointer
  * may be NULL.                                                                                                 */
@@ -285,6 +296,34 @@ int swec_ec_volume_info(swec_ec_volume *vol, int *data_shards, int *parity_shard
 /* EcVolume.FileAndDeleteCount (ec_volume.go:330-349): .ecx entries, distinct journalled deletions.      */
 int swec_ec_volume_counts(swec_ec_volume *vol, uint64_t *file_count, uint64_t *delete_count);
 void swec_ec_volume_close(swec_ec_volume *vol);
+
+/* ---- needle records on the GPU: Needle.ReadBytes (weed/storage/needle/needle_read.go:59-190) ------------------ */
+typedef enum swec_needle_status {
+    SWEC_NEEDLE_OK = 0,
+    SWEC_NEEDLE_SIZE_MISMATCH = 1,  /* header Size != index Size (ErrorSizeMismatch)                       */
+    SWEC_NEEDLE_OUT_OF_RANGE = 2,   /* DataSize or an optional field overruns the body; range_index 1..7  */
+    SWEC_NEEDLE_BAD_CRC = 3,        /* CRC32-C of Data != the stored checksum                             */
+    SWEC_NEEDLE_OUTSIDE_IMAGE = 4   /* the record does not fit inside the image: not read at all          */
+} swec_needle_status;
+typedef struct swec_needle_check {
+    uint64_t needle_id;   /* in  (reported back only)                                                       */
+    int64_t offset;       /* in  byte offset of the record in the image                                     */
+    int32_t size;         /* in  Size of the index entry                                                    */
+    int32_t status;       /* out swec_needle_status                                                         */
+    int32_t range_index;  /* out 1..7 with SWEC_NEEDLE_OUT_OF_RANGE, else 0                                 */
+    uint32_t data_size;   /* out bytes of Data (the whole body in version 1)                                */
+    uint32_t crc_got;     /* out CRC32-C (Castagnoli) of Data, as Go's crc32.Update(0, Castagnoli table, Data) */
+    uint32_t crc_want;    /* out the big-endian checksum stored after the body                              */
+    int32_t legacy_crc;   /* out 1 when crc_want is the pre-3.09 CRC.Value() form of crc_got (crc.go:25-27):  */
+                          /*     ReadBytes still reports the record, but it is old, not corrupt             */
+    int32_t reserved;
+} swec_needle_check;
+/* Check n records of a volume image (.dat bytes, superblock included) resident in HBM, each the way
+ * Needle.ReadBytes(record, 0, size, version) does, stopping at a record's first failure.  `dat` is a device pointer;
+ * checks[] is host memory.  A record that does not end inside dat_size is SWEC_NEEDLE_OUTSIDE_IMAGE and is never
+ * read.  Synchronises `stream` (a cudaStream_t; NULL = the default stream).                                        */
+int swec_check_needles_device(int device, const void *dat, int64_t dat_size, int needle_version,
+                              swec_needle_check *checks, int n, void *stream);
 
 /* ---- index files either side of the path (host only, no GPU) ---------------------------------- */
 /* WriteSortedFileFromIdx(base, ext): base.idx → base+ext (".ecx"), live entries sorted by needle id

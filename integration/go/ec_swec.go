@@ -17,6 +17,7 @@ import (
 	"fmt"
 	"io"
 	"runtime"
+	"strings"
 	"sync/atomic"
 	"unsafe"
 
@@ -381,6 +382,33 @@ func (v *swecEcVolume) ReadNeedles(ids []uint64, capacity int) ([][]byte, []erro
 // DeleteNeedleFromEcx: journal append (ec_volume_delete.go:28-93).
 func (v *swecEcVolume) DeleteNeedleFromEcx(id uint64) error {
 	return swecCall(func() C.int { return C.swec_ec_volume_delete_needle(v.h, C.uint64_t(id)) })
+}
+
+// ScrubLocal is the whole EcVolume.ScrubLocal (ec_volume_scrub.go:27-118): the index check, the chunk walk over the
+// local shards, and Needle.ReadBytes (size, layout, CRC32-C) of every record whose chunks are all local, checked on the
+// GPU.  Findings come back in the reference's order and wording.
+func (v *swecEcVolume) ScrubLocal(volumeId uint32) (int64, []uint32, []error, error) {
+	var entries C.int64_t
+	var broken [C.SWEC_MAX_SHARDS]C.uint32_t
+	var nBroken, nErrors C.int
+	text := make([]byte, 4<<20)
+	if err := swecCall(func() C.int {
+		return C.swec_ec_volume_scrub_needles(v.h, C.uint32_t(volumeId), &entries, &broken[0], &nBroken,
+			(*C.char)(unsafe.Pointer(&text[0])), C.size_t(len(text)), &nErrors)
+	}); err != nil {
+		return 0, nil, nil, err
+	}
+	shards := make([]uint32, int(nBroken))
+	for i := range shards {
+		shards[i] = uint32(broken[i])
+	}
+	var errs []error
+	if nErrors > 0 {
+		for _, line := range strings.Split(C.GoString((*C.char)(unsafe.Pointer(&text[0]))), "\n") {
+			errs = append(errs, fmt.Errorf("%s", line))
+		}
+	}
+	return int64(entries), shards, errs, nil
 }
 
 // ---- pinned batch buffers ---------------------------------------------------------------------------------

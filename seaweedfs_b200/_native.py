@@ -42,6 +42,15 @@ class NeedleRead(C.Structure):
                 ("n_recovered_intervals", C.c_int32), ("reserved", C.c_int32)]
 
 
+class NeedleCheck(C.Structure):
+    _fields_ = [("needle_id", C.c_uint64), ("offset", C.c_int64), ("size", C.c_int32), ("status", C.c_int32),
+                ("range_index", C.c_int32), ("data_size", C.c_uint32), ("crc_got", C.c_uint32), ("crc_want", C.c_uint32),
+                ("legacy_crc", C.c_int32), ("reserved", C.c_int32)]
+
+
+NEEDLE_STATUS = {0: "ok", 1: "size mismatch", 2: "out of range", 3: "bad crc", 4: "outside image"}
+
+
 # name → (restype, argtypes); kept in step with include/swec.h (tests/test_abi.py checks both ways)
 PROTOTYPES = {
     "swec_version": (C.c_char_p, []),
@@ -94,6 +103,10 @@ PROTOTYPES = {
     "swec_ec_volume_delete_needle": (C.c_int, [C.c_void_p, C.c_uint64]),
     "swec_ec_volume_scrub_local": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_uint32), C.POINTER(C.c_int),
                                              C.c_char_p, C.c_size_t, C.POINTER(C.c_int)]),
+    "swec_ec_volume_scrub_needles": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(C.c_int64), C.POINTER(C.c_uint32),
+                                               C.POINTER(C.c_int), C.c_char_p, C.c_size_t, C.POINTER(C.c_int)]),
+    "swec_check_needles_device": (C.c_int, [C.c_int, C.c_void_p, C.c_int64, C.c_int, C.POINTER(NeedleCheck), C.c_int,
+                                            C.c_void_p]),
     "swec_ec_volume_info": (C.c_int, [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int),
                                       C.POINTER(C.c_int64), C.POINTER(C.c_uint32)]),
     "swec_ec_volume_counts": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),

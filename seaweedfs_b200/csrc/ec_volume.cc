@@ -30,6 +30,7 @@
 
 #include "engine.h"
 #include "mini_json.h"
+#include "needles.h"
 #include "volume_format.h"
 
 namespace swec {
@@ -438,28 +439,163 @@ int swec_ec_volume_read_needles(swec_ec_volume* v, swec_needle_read* reads, int 
     return SWEC_OK;
 }
 
-// EcVolume.ScrubLocal (ec_volume_scrub.go:27-118) minus the needle parse: ScrubIndex, then every live entry of .ecx is
-// located (GetActualSize ONCE here, unlike the read path) and each of its chunks read from the local shard that holds it.
-// A shard that is too short for a chunk, or cannot be read, is reported broken; chunks on shards that are not local are
-// skipped like the reference skips remote ones.  The CRC of the record belongs to the storage engine's needle parser.
-int swec_ec_volume_scrub_local(swec_ec_volume* v, int64_t* entries, uint32_t* broken_shards, int* n_broken, char* errors,
-                               size_t errors_cap, int* n_errors) {
+}  // extern "C"
+
+namespace {
+
+// The needle parse of ScrubLocal (Needle.ReadBytes, needle_read.go:59-82), on the GPU.  The walk reads each record
+// that is wholly local straight into a pinned slot of a staging ring, back to back at 8-byte alignment; a full slot
+// goes H2D -> check kernels (needles.cu) -> results D2H on its own stream while the walk fills the next one.  A record
+// larger than a slot gets a device buffer of its own.  Nothing touches the GPU until the first record arrives.
+class NeedleScrub {
+  public:
+    NeedleScrub(int device, int version, uint32_t volume_id) : device_(device), version_(version), vid_(volume_id) {}
+    ~NeedleScrub() { ring_.release(); }
+
+    // room for the `bytes` of the next record: in the current slot (submitted first when it is full), or in a buffer
+    // of its own when the record is larger than a slot
+    int reserve(size_t bytes, uint8_t** out) {
+        if (ring_.slots.empty()) {
+            if (device_ < 0) return fail(SWEC_ERR_NO_DEVICE, "no CUDA device: the needle check runs on the GPU only");
+            SWEC_CUDA(cudaSetDevice(device_));
+            const int rc = ring_.allocate(device_, stage_slots(), kSlotData + kChecksBytes + needle_check_scratch_bytes(kSlotRecords));
+            if (rc) return rc;
+            pending_.resize(ring_.slots.size());
+        }
+        big_ = bytes > kSlotData;
+        if (big_) {
+            big_buf_.resize(bytes);
+            *out = big_buf_.data();
+            return SWEC_OK;
+        }
+        if (used_ + bytes > kSlotData || pending_[cur_].size() == kSlotRecords) {
+            const int rc = submit();
+            if (rc) return rc;
+        }
+        *out = ring_.slots[cur_].host + used_;
+        return SWEC_OK;
+    }
+
+    // the record just read into the reserved room is whole: check it.  `finding` = its place among the findings.
+    int commit(uint64_t id, int32_t size, size_t bytes, size_t finding) {
+        swec_needle_check c{};
+        c.needle_id = id;
+        c.size = size;
+        if (big_) return check_alone(c, bytes, finding);
+        StagingSlot& s = ring_.slots[cur_];
+        c.offset = int64_t(used_);
+        checks(s.host)[pending_[cur_].size()] = c;
+        pending_[cur_].push_back(finding);
+        used_ += (bytes + 7) & ~size_t(7);
+        return SWEC_OK;
+    }
+
+    int finish() {  // check what is still queued and collect every result
+        int rc = submit();
+        for (size_t i = 0; !rc && i < ring_.slots.size(); i++) rc = collect(i);
+        return rc;
+    }
+
+    std::vector<std::pair<size_t, std::string>> failed;  // (finding, text) of every record that failed its check
+
+  private:
+    static constexpr size_t kSlotData = size_t(16) << 20;  // record bytes per slot
+    static constexpr int kSlotRecords = 16384;
+    static constexpr size_t kChecksBytes = kSlotRecords * sizeof(swec_needle_check);
+    static swec_needle_check* checks(uint8_t* slot_base) { return reinterpret_cast<swec_needle_check*>(slot_base + kSlotData); }
+
+    int submit() {
+        const size_t n = pending_.empty() ? 0 : pending_[cur_].size();
+        if (n == 0) return SWEC_OK;
+        StagingSlot& s = ring_.slots[cur_];
+        const size_t cb = n * sizeof(swec_needle_check);
+        SWEC_CUDA(cudaMemcpyAsync(s.dev, s.host, used_, cudaMemcpyHostToDevice, s.stream));
+        SWEC_CUDA(cudaMemcpyAsync(checks(s.dev), checks(s.host), cb, cudaMemcpyHostToDevice, s.stream));
+        SWEC_CUDA(launch_needle_check(s.dev, int64_t(used_), version_, checks(s.dev), int(n), s.dev + kSlotData + kChecksBytes, s.stream));
+        SWEC_CUDA(cudaMemcpyAsync(checks(s.host), checks(s.dev), cb, cudaMemcpyDeviceToHost, s.stream));
+        SWEC_CUDA(cudaEventRecord(s.done, s.stream));
+        s.busy = true;
+        used_ = 0;
+        cur_ = (cur_ + 1) % ring_.slots.size();
+        return collect(cur_);  // the next slot is reused: its results first
+    }
+
+    int collect(size_t i) {
+        StagingSlot& s = ring_.slots[i];
+        if (!s.busy) return SWEC_OK;
+        SWEC_CUDA(cudaEventSynchronize(s.done));
+        s.busy = false;
+        const swec_needle_check* c = checks(s.host);
+        for (size_t j = 0; j < pending_[i].size(); j++) note(c[j], pending_[i][j]);
+        pending_[i].clear();
+        return SWEC_OK;
+    }
+
+    int check_alone(swec_needle_check c, size_t bytes, size_t finding) {
+        StagingSlot& s = ring_.slots[cur_];  // its stream; the slot's buffers stay with the walk
+        uint8_t* d = nullptr;
+        const size_t at = (bytes + 7) & ~size_t(7);
+        SWEC_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&d), at + sizeof c + needle_check_scratch_bytes(1), s.stream));
+        auto* dc = reinterpret_cast<swec_needle_check*>(d + at);
+        cudaError_t e = cudaMemcpyAsync(d, big_buf_.data(), bytes, cudaMemcpyHostToDevice, s.stream);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(dc, &c, sizeof c, cudaMemcpyHostToDevice, s.stream);
+        if (e == cudaSuccess) e = launch_needle_check(d, int64_t(bytes), version_, dc, 1, dc + 1, s.stream);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(&c, dc, sizeof c, cudaMemcpyDeviceToHost, s.stream);
+        cudaFreeAsync(d, s.stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(s.stream);
+        if (e != cudaSuccess) return cuda_fail(e, "needle check of a large record");
+        note(c, finding);
+        return SWEC_OK;
+    }
+
+    void note(const swec_needle_check& c, size_t finding) {
+        std::string err;
+        char buf[160];
+        switch (c.status) {
+            case SWEC_NEEDLE_OK: return;
+            case SWEC_NEEDLE_SIZE_MISMATCH: err = "size mismatch"; break;  // ScrubLocal reads at offset 0: the short form
+            case SWEC_NEEDLE_OUT_OF_RANGE:
+                err = "index out of range " + std::to_string(c.range_index) + ": needle data corrupted";
+                break;
+            case SWEC_NEEDLE_BAD_CRC:  // %v of a NeedleId is hex (types/needle_id_type.go:34-36)
+                snprintf(buf, sizeof buf, "invalid CRC for needle %" PRIx64 " (got %08x, want %08x), data on disk corrupted: needle data corrupted",
+                         c.needle_id, c.crc_got, c.crc_want);
+                err = buf;
+                break;
+            default: err = "record does not fit in its own bytes"; break;
+        }
+        failed.emplace_back(finding, "needle " + std::to_string(c.needle_id) + " on volume " + std::to_string(vid_) + ": " + err);
+    }
+
+    int device_, version_;
+    uint32_t vid_;
+    StagingRing ring_;
+    std::vector<std::vector<size_t>> pending_;  // per slot: the finding index of each queued record
+    size_t cur_ = 0, used_ = 0;
+    bool big_ = false;
+    std::vector<uint8_t> big_buf_;
+};
+
+// EcVolume.ScrubLocal (ec_volume_scrub.go:27-118): ScrubIndex, then every live entry of .ecx is located (GetActualSize
+// ONCE here, unlike the read path) and each of its chunks read from the local shard that holds it.  A shard that is
+// too short for a chunk, or cannot be read, is reported broken; chunks on shards that are not local are skipped like
+// the reference skips remote ones.  With `needles`, every record whose chunks were all read is also checked like
+// Needle.ReadBytes; its finding takes its place in walk order.
+int scrub_walk(swec_ec_volume* v, NeedleScrub* needles, int64_t* entries, uint32_t* broken_shards, int* n_broken,
+               char* errors, size_t errors_cap, int* n_errors) {
     if (!v || !entries || !n_broken || !n_errors || !broken_shards) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
     std::lock_guard<std::mutex> lock(v->mu);
-    std::string text;
-    int count = 0;
-    auto add = [&](const std::string& m) {
-        if (count++) text += "\n";
-        text += m;
-    };
+    std::vector<std::string> found;  // in walk order; "" = a record sent to the needle check
+    int extra_lines = 0;
     {  // ScrubIndex = idx.CheckIndexFile on the sealed index
         int64_t n = 0;
         int k2 = 0;
         std::vector<char> buf(size_t(1) << 20);
         const int rc = swec_check_index_file((v->index_base + ".ecx").c_str(), v->version, &n, buf.data(), buf.size(), &k2);
         if (rc) return rc;
-        if (k2) add(buf.data()), count += k2 - 1;
+        if (k2) found.push_back(buf.data()), extra_lines = k2 - 1;
     }
+    auto add = [&](const std::string& m) { found.push_back(m); };
     const int k = v->k, total = v->k + v->m;
     const int64_t large = kLargeBlockSize, small = kSmallBlockSize;
     std::vector<int64_t> shard_size(size_t(total), -1);
@@ -479,13 +615,29 @@ int swec_ec_volume_scrub_local(swec_ec_volume* v, int64_t* entries, uint32_t* br
         std::vector<swec_interval> ivs(max_intervals(want, small));
         const int niv = want > 0 ? swec_locate_data(large, small, v->shard_dat_size, offset, want, k, ivs.data(), int(ivs.size())) : 0;
         if (niv < 0) return niv;
-        int64_t read = 0;
+        uint8_t* record = nullptr;  // where the record is gathered for the needle check, when all of it is local
+        if (needles && size >= 0) {
+            bool local = true;
+            for (int j = 0; j < niv && local; j++) {
+                int sid = 0;
+                int64_t soff = 0;
+                swec_interval_to_shard(&ivs[size_t(j)], large, small, k, &sid, &soff);
+                local = v->shard_fd[size_t(sid)] >= 0;
+            }
+            if (local) {
+                const int rc = needles->reserve(size_t(want), &record);
+                if (rc) return rc;
+            }
+        }
+        int64_t read = 0, pos = 0;
         for (int j = 0; j < niv; j++) {
             int sid = 0;
             int64_t soff = 0;
             swec_interval_to_shard(&ivs[size_t(j)], large, small, k, &sid, &soff);
             const int64_t ssize = ivs[size_t(j)].size;
             const std::string where = std::to_string(j + 1) + "/" + std::to_string(niv);
+            uint8_t* dst = record ? record + pos : nullptr;
+            pos += ssize;
             if (v->shard_fd[size_t(sid)] < 0) {  // not local: skipped, counted as read
                 read += ssize;
                 continue;
@@ -496,8 +648,11 @@ int swec_ec_volume_scrub_local(swec_ec_volume* v, int64_t* entries, uint32_t* br
                     std::to_string(shard_size[size_t(sid)]) + "), cannot read chunk " + where);
                 continue;
             }
-            chunk.resize(size_t(ssize));
-            const ssize_t got = pread(v->shard_fd[size_t(sid)], chunk.data(), size_t(ssize), off_t(soff));
+            if (!dst) {
+                chunk.resize(size_t(ssize));
+                dst = chunk.data();
+            }
+            const ssize_t got = pread(v->shard_fd[size_t(sid)], dst, size_t(ssize), off_t(soff));
             if (got < 0) {
                 broken[size_t(sid)] = 1;
                 add("failed to read chunk " + where + " for needle " + std::to_string(id) + " from local shard " + std::to_string(sid) +
@@ -516,6 +671,23 @@ int swec_ec_volume_scrub_local(swec_ec_volume* v, int64_t* entries, uint32_t* br
             add("expected " + std::to_string(want) + " bytes for needle " + std::to_string(id) + ", got " + std::to_string(read));
             break;
         }
+        if (record) {
+            const int rc = needles->commit(id, size, size_t(want), found.size());
+            if (rc) return rc;
+            found.emplace_back();
+        }
+    }
+    if (needles) {
+        const int rc = needles->finish();
+        if (rc) return rc;
+        for (auto& [at, text] : needles->failed) found[at] = std::move(text);
+    }
+    std::string text;
+    int count = extra_lines;
+    for (const std::string& f : found) {
+        if (f.empty()) continue;
+        if (count++ > extra_lines) text += "\n";
+        text += f;
     }
     *entries = walked;
     *n_broken = 0;
@@ -528,6 +700,22 @@ int swec_ec_volume_scrub_local(swec_ec_volume* v, int64_t* entries, uint32_t* br
         errors[m] = 0;
     }
     return SWEC_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int swec_ec_volume_scrub_local(swec_ec_volume* v, int64_t* entries, uint32_t* broken_shards, int* n_broken, char* errors,
+                               size_t errors_cap, int* n_errors) {
+    return scrub_walk(v, nullptr, entries, broken_shards, n_broken, errors, errors_cap, n_errors);
+}
+
+int swec_ec_volume_scrub_needles(swec_ec_volume* v, uint32_t volume_id, int64_t* entries, uint32_t* broken_shards, int* n_broken,
+                                 char* errors, size_t errors_cap, int* n_errors) {
+    if (!v) return fail(SWEC_ERR_INVALID_ARG, "NULL volume");
+    NeedleScrub needles(v->device, v->version, volume_id);
+    return scrub_walk(v, &needles, entries, broken_shards, n_broken, errors, errors_cap, n_errors);
 }
 
 // what NewEcVolume derived from .vif and the shard files (ec_volume.go:114-154,399-417)

@@ -11,6 +11,7 @@
 #include <vector>
 
 #include "../../include/swec.h"
+#include "needle_format.h"  // the needle record itself, and GetActualSize
 
 namespace swec {
 
@@ -93,13 +94,6 @@ inline IndexEntry index_entry(const uint8_t* p) { return {be64(p), int64_t(be32(
 
 // SearchNeedleFromSortedIndex (ec_volume.go:431-458): the entry number of `key` in a sorted index, or -1
 int64_t search_sorted_index(const uint8_t* index, int64_t entries, uint64_t key);
-
-// GetActualSize (needle/needle_read.go:292-294, needle_read_tail.go:36-50): header 16 + body + checksum 4
-// (+ 8-byte timestamp in version 3) + padding to 8, where the padding is 1..8 bytes, never 0.
-inline int64_t needle_actual_size(int64_t size, int version) {
-    const int64_t fixed = 16 + size + 4 + (version == 3 ? 8 : 0);
-    return fixed + (8 - fixed % 8);
-}
 
 // the needle ids of a .ecj deletion journal: 8 bytes each, big-endian; a trailing partial id is ignored
 std::vector<uint64_t> ecj_ids(const std::vector<uint8_t>& ecj);

@@ -407,6 +407,16 @@ class EcVolume:
 
     ScrubLocal = scrub_local
 
+    def scrub_needles(self, volume_id: int = 0):
+        """The whole ScrubLocal: scrub_local's walk plus Needle.ReadBytes (size, layout, CRC32-C) of every record whose
+        chunks are all local, on the GPU.  Same result shape as scrub_local."""
+        n, nb, ne = C.c_int64(0), C.c_int(0), C.c_int(0)
+        broken = (C.c_uint32 * MaxShardCount)()
+        buf = C.create_string_buffer(1 << 22)
+        check(lib().swec_ec_volume_scrub_needles(self._h, volume_id, C.byref(n), broken, C.byref(nb), buf, len(buf),
+                                                 C.byref(ne)))
+        return int(n.value), list(broken[: nb.value]), (buf.value.decode().split("\n") if ne.value else [])
+
     def close(self) -> None:
         h, self._h = getattr(self, "_h", None), None
         if h and callable(lib):
@@ -414,6 +424,21 @@ class EcVolume:
 
     __del__ = close
     ReadEcShardNeedles = read_needles
+
+
+def check_needles_device(dat_ptr: int, dat_size: int, records, needle_version: int = 3, device: int = 0,
+                         stream: int | None = None) -> list[dict]:
+    """Needle.ReadBytes on records of a volume image in device memory (swec_check_needles_device).  records: iterable
+    of (needle_id, offset, size).  One dict per record: status (0 ok, 1 size mismatch, 2 out of range, 3 bad crc,
+    4 outside image), range_index, data_size, crc_got, crc_want, legacy_crc."""
+    from ._native import NeedleCheck
+    records = list(records)
+    arr = (NeedleCheck * max(1, len(records)))()
+    for c, (nid, off, size) in zip(arr, records):
+        c.needle_id, c.offset, c.size = nid, off, size
+    check(lib().swec_check_needles_device(device, dat_ptr, dat_size, needle_version, arr, len(records), stream))
+    return [{"needle_id": c.needle_id, "status": c.status, "range_index": c.range_index, "data_size": c.data_size,
+             "crc_got": c.crc_got, "crc_want": c.crc_want, "legacy_crc": c.legacy_crc} for c in arr[:len(records)]]
 
 
 def read_ec_shard_needles(data_base_file_name: str, needle_ids: list[int], index_base_file_name: str | None = None,
