@@ -18,6 +18,7 @@
  *   swec_write_ec_files         WriteEcFiles / generateEcFiles   ec_encoder.go:61-69,110-128
  *   swec_rebuild_ec_files       RebuildEcFiles / generateMissingEcFiles   ec_encoder.go:74-104,146-200
  *   swec_verify_ec_files        (Rust twin) verify_ec_shards   seaweed-volume/src/storage/erasure_coding/ec_encoder.rs:177-278
+ *   swec_locate_ec_damage       what verify_ec_shards cannot tell (ec_encoder.rs:240-258): WHICH shard is wrong
  *   swec_reconstruct_batch      batched ReconstructData   weed/storage/store_ec.go:482-560 (one call per interval today)
  *   swec_write_dat_file         WriteDatFile              weed/storage/erasure_coding/ec_decoder.go:176-223
  *   swec_ec_shards_generate     VolumeEcShardsGenerate (file work)   weed/server/volume_grpc_erasure_coding.go:43-146
@@ -212,6 +213,49 @@ int swec_rebuild_ec_files(const char *base_file_name, const char *const *additio
 int swec_verify_ec_files(const char *base_file_name, const char *const *additional_dirs,
                          int n_additional_dirs, int data_shards, int parity_shards, int device,
                          uint64_t *mismatched_vectors, int *ok);
+
+/* ---- locate the wrong shard when parity does not match ----------------------------------------------------------
+ * Per byte column x, computed parity XOR stored parity is the syndrome s = [P | I]·e of the column's error pattern e.
+ * A GPU kernel decodes every non-zero syndrome within `radius` wrong shards and blames those shards.  RS(k,m) has
+ * minimum distance m+1, so radius-t decoding (t = 1 or 2, 2t <= m) guarantees, per column:
+ *   - at most t wrong shards: exactly those shards are blamed;
+ *   - more than t but at most m-t wrong shards: the column is counted as uncorrectable and no shard is blamed;
+ *   - more than m-t wrong shards: the column may be blamed on the wrong shards.  That is the limit of the code.
+ * For RS(10,4), radius 1 (the default) is always right, or says uncorrectable, for up to 3 damaged shards per column;
+ * radius 2 locates overlapping damage in 2 shards but may misattribute 3.  The remedy for a blamed shard is to delete
+ * its file and run swec_rebuild_ec_files.  The reference cannot do this: verify_ec_shards
+ * (seaweed-volume/src/storage/erasure_coding/ec_encoder.rs:240-258) marks every mismatching PARITY shard as broken, so
+ * one damaged data shard gets all m parity shards reported (and rebuilding those bakes the damage in), and the Go scrub
+ * never checks parity (ec_volume_scrub.go:25).                                                                        */
+typedef struct swec_damage_report {
+    uint64_t columns;                        /* byte columns checked (= shard length)                         */
+    uint64_t damaged_columns;                /* columns with a non-zero syndrome                              */
+    uint64_t uncorrectable_columns;          /* ... that no pattern of <= radius shards explains              */
+    int64_t first_uncorrectable, last_uncorrectable;  /* shard offsets; -1 when none                        */
+    uint64_t shard_bytes[SWEC_MAX_SHARDS];   /* bytes of shard i located as wrong                             */
+    int64_t shard_first[SWEC_MAX_SHARDS], shard_last[SWEC_MAX_SHARDS];  /* -1 when none                      */
+} swec_damage_report;
+typedef struct swec_damage_range {
+    int32_t shard_id; /* -1 = uncorrectable columns                                                          */
+    int32_t reserved;
+    int64_t offset;   /* 4 KiB-aligned shard offset                                                          */
+    int64_t length;   /* whole 4 KiB pages, the last one clipped to the shard length                         */
+} swec_damage_range;
+/* Both calls: ranges are the maximal runs of consecutive 4 KiB pages holding a blamed column, per shard (ascending id,
+ * then offset), followed by the runs holding uncorrectable columns.  *n_ranges (may be NULL) = how many there are; only
+ * the first ranges_cap are written.  radius must be 1 or 2, radius 1 needs m >= 2 and radius 2 needs m >= 4; report
+ * must not be NULL and ranges_cap not negative (SWEC_ERR_INVALID_ARG otherwise).
+ * File level: the shard lookup, ratio rule (data_shards = 0: from base.vif) and errors of swec_verify_ec_files, the same
+ * file pipeline, and the locate kernel in place of the compare.  Every file check happens before any device work; an
+ * encoder without a device fails with SWEC_ERR_NO_DEVICE.  *ok = 1 iff no column has a non-zero syndrome.           */
+int swec_locate_ec_damage(const char *base_file_name, const char *const *additional_dirs, int n_additional_dirs,
+                          int data_shards, int parity_shards, int device, int radius, swec_damage_report *report,
+                          swec_damage_range *ranges, int ranges_cap, int *n_ranges, int *ok);
+/* Device level: shards[k+m] in HBM, shard_len bytes each.  The parity is recomputed with the encode kernel into scratch
+ * of at most 256 MiB per parity shard at a time (no run-time compile for RS(10,4)); synchronises `stream`.           */
+int swec_locate_damage_device(swec_encoder *enc, const void *const *shards, size_t shard_len, int radius,
+                              swec_damage_report *report, swec_damage_range *ranges, int ranges_cap,
+                              int *n_ranges, void *stream);
 int swec_write_dat_file(const char *base_file_name, int64_t dat_file_size,
                         const char *const *shard_file_names, int data_shards,
                         int64_t large_block, int64_t small_block);

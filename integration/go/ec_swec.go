@@ -411,6 +411,41 @@ func (v *swecEcVolume) ScrubLocal(volumeId uint32) (int64, []uint32, []error, er
 	return int64(entries), shards, errs, nil
 }
 
+// swecLocateEcDamage is the parity side of a scrub of a volume whose shards are all local, run before ec.rebuild: it
+// names the shard FILES that are wrong, where verify_ec_shards (seaweed-volume/src/storage/erasure_coding/
+// ec_encoder.rs:240-258) can only name the parity shards that disagree.  broken is ready to become EcShardInfos (delete
+// those files, then rebuild); details say where, one line per blamed shard and one for columns damaged in more shards
+// than one (radius 1) that no single shard explains.
+func swecLocateEcDamage(baseFileName string, ctx *ECContext, additionalDirs []string) (broken []uint32, details []string, err error) {
+	cs := C.CString(baseFileName)
+	defer C.free(unsafe.Pointer(cs))
+	dirs := make([]*C.char, len(additionalDirs)+1)
+	for i, d := range additionalDirs {
+		dirs[i] = C.CString(d)
+		defer C.free(unsafe.Pointer(dirs[i]))
+	}
+	var report C.swec_damage_report
+	var nRanges, ok C.int
+	if err := swecCall(func() C.int {
+		return C.swec_locate_ec_damage(cs, (**C.char)(unsafe.Pointer(&dirs[0])), C.int(len(additionalDirs)),
+			C.int(ctx.DataShards), C.int(ctx.ParityShards), swecPickDevice(), 1, &report, nil, 0, &nRanges, &ok)
+	}); err != nil {
+		return nil, nil, fmt.Errorf("locate ec damage: %w", err)
+	}
+	for i := 0; i < ctx.DataShards+ctx.ParityShards; i++ {
+		if n := uint64(report.shard_bytes[i]); n > 0 {
+			broken = append(broken, uint32(i))
+			details = append(details, fmt.Sprintf("ec shard %d: %d bytes do not match the other shards, offsets %d..%d",
+				i, n, int64(report.shard_first[i]), int64(report.shard_last[i])))
+		}
+	}
+	if report.uncorrectable_columns > 0 {
+		details = append(details, fmt.Sprintf("%d byte columns are damaged in more shards than can be located, offsets %d..%d",
+			uint64(report.uncorrectable_columns), int64(report.first_uncorrectable), int64(report.last_uncorrectable)))
+	}
+	return broken, details, nil
+}
+
 // ---- pinned batch buffers ---------------------------------------------------------------------------------
 // runtime.Pinner only stops the Go GC from moving a slice; to CUDA such memory is PAGEABLE, so every Encode /
 // Reconstruct on it bounces through the library's pinned ring (a memcpy per shard each way).  The batch buffers of

@@ -48,6 +48,17 @@ class NeedleCheck(C.Structure):
                 ("legacy_crc", C.c_int32), ("reserved", C.c_int32)]
 
 
+class DamageReport(C.Structure):
+    _fields_ = [("columns", C.c_uint64), ("damaged_columns", C.c_uint64), ("uncorrectable_columns", C.c_uint64),
+                ("first_uncorrectable", C.c_int64), ("last_uncorrectable", C.c_int64),
+                ("shard_bytes", C.c_uint64 * SWEC_MAX_SHARDS), ("shard_first", C.c_int64 * SWEC_MAX_SHARDS),
+                ("shard_last", C.c_int64 * SWEC_MAX_SHARDS)]
+
+
+class DamageRange(C.Structure):
+    _fields_ = [("shard_id", C.c_int32), ("reserved", C.c_int32), ("offset", C.c_int64), ("length", C.c_int64)]
+
+
 NEEDLE_STATUS = {0: "ok", 1: "size mismatch", 2: "out of range", 3: "bad crc", 4: "outside image"}
 
 
@@ -92,6 +103,11 @@ PROTOTYPES = {
                                         C.c_void_p, C.POINTER(C.c_int)]),
     "swec_verify_ec_files": (C.c_int, [C.c_char_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                        C.POINTER(C.c_int)]),
+    "swec_locate_ec_damage": (C.c_int, [C.c_char_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                        C.POINTER(DamageReport), C.POINTER(DamageRange), C.c_int, C.POINTER(C.c_int),
+                                        C.POINTER(C.c_int)]),
+    "swec_locate_damage_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.POINTER(DamageReport),
+                                            C.POINTER(DamageRange), C.c_int, C.POINTER(C.c_int), C.c_void_p]),
     "swec_write_dat_file": (C.c_int, [C.c_char_p, C.c_int64, C.c_void_p, C.c_int, C.c_int64, C.c_int64]),
     "swec_ec_shards_generate": (C.c_int, [C.c_char_p, C.c_char_p, C.c_uint32, C.c_uint64, C.c_int]),
     "swec_ec_shards_rebuild": (C.c_int, [C.c_char_p, C.c_char_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p,

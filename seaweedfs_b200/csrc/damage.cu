@@ -1,0 +1,416 @@
+// seaweedfs_b200/csrc/damage.cu — locate the wrong shard of every byte column whose parity does not match.
+//
+// For a column c = [d | p] of a shard set, computed parity XOR stored parity is the syndrome s = [P | I]·e of the
+// error pattern e, so it is zero on a clean column and names the damage otherwise.  RS(k,m) has distance m+1: radius t
+// decoding (2t <= m) blames exactly the wrong shards of a column with at most t of them, reports a column with t+1 ..
+// m-t of them as uncorrectable, and may blame the wrong shards beyond that (include/swec.h states the guarantee).
+//
+//   swec_locate_kernel   grid-stride over 16-byte vectors of the 2m parity streams.  Clean vectors (the fast path)
+//                        cost the loads, one OR per stream and one warp vote.  A warp with a non-zero syndrome reloads
+//                        it and decodes every damaged column against log/exp tables and the logs of P in shared memory:
+//                          one shard   exactly one non-zero component p: parity shard k+p; all m non-zero and
+//                                      log s_i - log P[i][j] equal for every i: data shard j
+//                          two shards  two non-zero components: those two parity shards; a data shard j and parity
+//                                      shard k+p: the rows other than p are a multiple of P[:,j]; data shards a < b:
+//                                      rows 0 and 1 solved by Cramer's rule, the other rows checked
+//                        Per-lane runs (set, count, first, last) merge the columns a lane blames on one shard, and a
+//                        warp merges equal runs with __match_any_sync / __reduce_*_sync before one set of atomics.
+//                        Bytes after the last whole vector, and unaligned streams, go through a byte loop.
+#include <cuda_runtime.h>
+
+#include <algorithm>
+#include <cstring>
+#include <string>
+#include <vector>
+
+#include "damage.h"
+#include "device_common.cuh"
+#include "engine.h"
+
+namespace swec {
+
+namespace {
+
+constexpr int kSets = SWEC_MAX_SHARDS + 1;  // one counter set per shard, and one for uncorrectable columns (set k+m)
+constexpr int kCounters = 3 * kSets + 1;    // bytes[kSets], first[kSets], last[kSets], damaged columns
+constexpr int kPageShift = 12;              // 4 KiB pages
+
+struct LocateTables {
+    u8 log[256];
+    u8 exp[512];         // two periods of 2^i: a sum of two logs needs no reduction
+    u8 logp[32 * 32];    // log P[i][j] at i*32 + j
+    u8 logdet[32 * 32];  // log det [P0a P0b; P1a P1b] at a*32 + b (a != b data shards)
+};
+constexpr int kTableWords = int(sizeof(LocateTables) / 4);
+static_assert(sizeof(LocateTables) % 16 == 0, "tables are copied in words");
+
+struct LocateParams {
+    const u8* comp[SWEC_MAX_SHARDS];
+    const u8* stored[SWEC_MAX_SHARDS];
+    u64 n, base;
+    int k, m, radius;
+    const u32* tables;
+    unsigned long long* ctr;
+    u32* pages;
+    u64 page_words;
+};
+
+struct Run {  // columns one lane blamed on one set, in increasing offset order
+    int set;  // valid while cnt > 0
+    u32 cnt;
+    u64 first, last;
+};
+
+__device__ __forceinline__ void set_page(const LocateParams& p, int set, u64 off) {
+    const u64 page = off >> kPageShift;
+    atomicOr(p.pages + u64(set) * p.page_words + (page >> 5), 1u << (page & 31));
+}
+
+// a run of one lane's columns: they lie within 16 bytes (or one byte), so in at most two pages
+__device__ void flush_plain(const LocateParams& p, Run& r) {
+    if (!r.cnt) return;
+    atomicAdd(p.ctr + r.set, (unsigned long long)r.cnt);
+    atomicMin(p.ctr + kSets + r.set, (unsigned long long)r.first);
+    atomicMax(p.ctr + 2 * kSets + r.set, (unsigned long long)r.last);
+    set_page(p, r.set, r.first);
+    if ((r.last >> kPageShift) != (r.first >> kPageShift)) set_page(p, r.set, r.last);
+    r.cnt = 0;
+}
+
+// Whole warp, converged.  The warp's columns lie within 512 bytes of wbase, so in at most two pages, and a set's
+// first and last column are in both of them.
+__device__ __forceinline__ void flush_warp(const LocateParams& p, Run& r, u64 wbase) {
+    const int key = r.cnt ? r.set : -1;
+    const u32 group = __match_any_sync(0xffffffffu, key);
+    if (key < 0) return;
+    const u32 cnt = __reduce_add_sync(group, r.cnt);
+    const u32 lo = __reduce_min_sync(group, u32(r.first - wbase));
+    const u32 hi = __reduce_max_sync(group, u32(r.last - wbase));
+    r.cnt = 0;
+    if ((threadIdx.x & 31) != u32(__ffs(group) - 1)) return;
+    Run w{key, cnt, wbase + lo, wbase + hi};
+    flush_plain(p, w);
+}
+
+__device__ __forceinline__ void record(const LocateParams& p, Run* run, int set, u64 off) {
+    int i;
+    if (run[0].cnt && run[0].set == set) i = 0;
+    else if (run[1].cnt && run[1].set == set) i = 1;
+    else if (!run[0].cnt) i = 0;
+    else {
+        flush_plain(p, run[1]);  // a third set within one lane's columns: rare
+        i = 1;
+    }
+    if (!run[i].cnt) {
+        run[i].set = set;
+        run[i].first = off;
+    }
+    run[i].cnt++;
+    run[i].last = off;
+}
+
+__device__ __forceinline__ u8 gmul(const LocateTables& t, int log_c, u8 v) { return v ? t.exp[log_c + t.log[v]] : 0; }
+
+// rows other than `skip` of s (logs in L, all non-zero) are one multiple of column j of P
+__device__ __forceinline__ bool multiple_of_column(const LocateTables& t, const u8* L, int m, int j, int skip) {
+    int r = -1;
+    for (int i = 0; i < m; i++) {
+        if (i == skip) continue;
+        int d = int(L[i]) - int(t.logp[i * 32 + j]);
+        if (d < 0) d += 255;
+        if (r < 0) r = d;
+        else if (d != r) return false;
+    }
+    return true;
+}
+
+// Shards that explain the non-zero syndrome s within the radius, ascending in *a, *b; returns how many (0: none does).
+__device__ int decode_column(const LocateTables& t, const u8* s, int k, int m, int radius, int* a, int* b) {
+    u8 L[SWEC_MAX_SHARDS];
+    u32 nz = 0;
+    for (int i = 0; i < m; i++) {
+        L[i] = t.log[s[i]];
+        if (s[i]) nz |= 1u << i;
+    }
+    const int w = __popc(nz);
+    if (w == 1) {
+        *a = k + __ffs(nz) - 1;
+        return 1;
+    }
+    if (w == m)  // every entry of an MDS P is non-zero
+        for (int j = 0; j < k; j++)
+            if (multiple_of_column(t, L, m, j, -1)) {
+                *a = j;
+                return 1;
+            }
+    if (radius < 2) return 0;
+    if (w == 2) {
+        *a = k + __ffs(nz) - 1;
+        *b = k + __ffs(nz & (nz - 1)) - 1;
+        return 2;
+    }
+    if (w < m - 1) return 0;  // a data shard in the pattern makes at least m-1 components non-zero
+    for (int q = 0; q < m; q++) {
+        if (w == m - 1 && ((nz >> q) & 1)) continue;  // the zero component can only be the parity shard's
+        for (int j = 0; j < k; j++)
+            if (multiple_of_column(t, L, m, j, q)) {
+                *a = j;
+                *b = k + q;
+                return 2;
+            }
+    }
+    for (int x = 0; x + 1 < k; x++)
+        for (int y = x + 1; y < k; y++) {
+            // [P0x P0y; P1x P1y]·[ex; ey] = [s0; s1]
+            const u8 nx = gmul(t, t.logp[32 + y], s[0]) ^ gmul(t, t.logp[y], s[1]);
+            const u8 ny = gmul(t, t.logp[32 + x], s[0]) ^ gmul(t, t.logp[x], s[1]);
+            if (!nx || !ny) continue;
+            const int ld = t.logdet[x * 32 + y];
+            int lx = int(t.log[nx]) - ld, ly = int(t.log[ny]) - ld;
+            if (lx < 0) lx += 255;
+            if (ly < 0) ly += 255;
+            bool ok = true;
+            for (int i = 2; i < m && ok; i++) ok = (t.exp[lx + t.logp[i * 32 + x]] ^ t.exp[ly + t.logp[i * 32 + y]]) == s[i];
+            if (ok) {
+                *a = x;
+                *b = y;
+                return 2;
+            }
+        }
+    return 0;
+}
+
+__device__ __forceinline__ void blame(const LocateParams& p, const LocateTables& t, const u8* s, int m, u64 off, Run* run) {
+    int a = -1, b = -1;
+    const int found = decode_column(t, s, p.k, m, p.radius, &a, &b);
+    if (!found) {
+        record(p, run, p.k + m, off);
+        return;
+    }
+    record(p, run, a, off);
+    if (found == 2) record(p, run, b, off);
+}
+
+__device__ __forceinline__ u8 byte_of(const uint4& x, int c) {
+    const u32 w = c < 4 ? x.x : c < 8 ? x.y : c < 12 ? x.z : x.w;
+    return u8(w >> ((c & 3) * 8));
+}
+
+__device__ __forceinline__ uint4 xor4(const uint4& a, const uint4& b) {
+    return make_uint4(a.x ^ b.x, a.y ^ b.y, a.z ^ b.z, a.w ^ b.w);
+}
+
+template <int MT>  // MT > 0: m known at compile time; 0: run-time m
+__global__ void __launch_bounds__(256) swec_locate_kernel(const __grid_constant__ LocateParams p) {
+    __shared__ __align__(16) u32 words[kTableWords];
+    for (int i = threadIdx.x; i < kTableWords; i += blockDim.x) words[i] = p.tables[i];
+    __syncthreads();
+    const LocateTables& t = *reinterpret_cast<const LocateTables*>(words);
+    constexpr int kMaxM = MT > 0 ? MT : SWEC_MAX_SHARDS;
+    const int m = MT > 0 ? MT : p.m;
+    unsigned long long align = 0;
+    for (int i = 0; i < m; i++)
+        align |= reinterpret_cast<unsigned long long>(p.comp[i]) | reinterpret_cast<unsigned long long>(p.stored[i]);
+    const u64 nvec = (align & 15) == 0 ? p.n >> 4 : 0;
+    const u32 lane = threadIdx.x & 31;
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    Run run[2] = {{-1, 0, 0, 0}, {-1, 0, 0, 0}};
+
+    // vb is the first vector of this warp: every lane of a warp takes the same number of turns
+    for (u64 vb = (u64)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); vb < nvec; vb += stride) {
+        const u64 v = vb + lane;
+        u32 diff = 0;
+        if (v < nvec) {
+#pragma unroll
+            for (int i = 0; i < kMaxM; i++) {
+                if (MT == 0 && i >= m) break;
+                const uint4 d = xor4(swec_ldg_stream(p.comp[i] + (v << 4)), swec_ldg_stream(p.stored[i] + (v << 4)));
+                diff |= d.x | d.y | d.z | d.w;
+            }
+        }
+        if (!__any_sync(0xffffffffu, diff != 0)) continue;
+        u32 damaged = 0;
+        if (diff) {
+            uint4 x[kMaxM];
+            for (int i = 0; i < m; i++) x[i] = xor4(__ldg(reinterpret_cast<const uint4*>(p.comp[i]) + v),
+                                                    __ldg(reinterpret_cast<const uint4*>(p.stored[i]) + v));
+            for (int c = 0; c < 16; c++) {
+                u8 s[kMaxM];
+                u8 any = 0;
+                for (int i = 0; i < m; i++) {
+                    s[i] = byte_of(x[i], c);
+                    any |= s[i];
+                }
+                if (!any) continue;
+                damaged++;
+                blame(p, t, s, m, p.base + (v << 4) + u64(c), run);
+            }
+        }
+        const u64 wbase = p.base + (vb << 4);
+        flush_warp(p, run[0], wbase);
+        flush_warp(p, run[1], wbase);
+        damaged = __reduce_add_sync(0xffffffffu, damaged);
+        if (lane == 0 && damaged) atomicAdd(p.ctr + 3 * kSets, (unsigned long long)damaged);
+    }
+
+    for (u64 x = (nvec << 4) + (u64)blockIdx.x * blockDim.x + threadIdx.x; x < p.n; x += stride) {
+        u8 s[kMaxM];
+        u8 any = 0;
+        for (int i = 0; i < m; i++) {
+            s[i] = p.comp[i][x] ^ p.stored[i][x];
+            any |= s[i];
+        }
+        if (!any) continue;
+        atomicAdd(p.ctr + 3 * kSets, 1ull);
+        blame(p, t, s, m, p.base + x, run);
+        flush_plain(p, run[0]);
+        flush_plain(p, run[1]);
+    }
+}
+
+template <int MT>
+unsigned locate_grid(u64 n) {
+    static int per_sm = 0;  // resident CTAs per SM, the same on every device of this architecture
+    if (!per_sm && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, swec_locate_kernel<MT>, 256, 0) != cudaSuccess) {
+        cudaGetLastError();
+        per_sm = 4;
+    }
+    int dev = 0, sms = 132;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    const u64 need = (n / 16 + 255) / 256 + 1;
+    return unsigned(std::min<u64>(need, u64(sms) * u64(std::max(1, per_sm))));
+}
+
+}  // namespace
+
+int check_locate_args(int m, int radius, const swec_damage_report* report, const swec_damage_range* ranges,
+                      int ranges_cap) {
+    if (!report) return fail(SWEC_ERR_INVALID_ARG, "report is NULL");
+    if (ranges_cap < 0 || (ranges_cap > 0 && !ranges))
+        return fail(SWEC_ERR_INVALID_ARG, "ranges_cap must be >= 0, and ranges non-NULL when it is > 0");
+    if (radius != 1 && radius != 2) return fail(SWEC_ERR_INVALID_ARG, "radius must be 1 or 2");
+    if (m < 2 * radius)
+        return fail(SWEC_ERR_INVALID_ARG, "radius " + std::to_string(radius) + " needs at least " +
+                                              std::to_string(2 * radius) + " parity shards, the code has " + std::to_string(m));
+    return SWEC_OK;
+}
+
+DamageLocator::~DamageLocator() {
+    if (tables_) cudaFree(tables_);
+    if (counters_) cudaFree(counters_);
+    if (pages_) cudaFree(pages_);
+}
+
+int DamageLocator::init(const Matrix& parity, int64_t shard_len, int radius, cudaStream_t s) {
+    k_ = parity.cols;
+    m_ = parity.rows;
+    radius_ = radius;
+    shard_len_ = shard_len;
+    LocateTables t;
+    memset(&t, 0, sizeof t);
+    unsigned x = 1;
+    for (int i = 0; i < 255; i++) {
+        t.exp[i] = u8(x);
+        t.log[x] = u8(i);
+        x <<= 1;
+        if (x & 0x100) x ^= kFieldPoly;
+    }
+    for (int i = 255; i < 512; i++) t.exp[i] = t.exp[i - 255];
+    const GF& gf = GF::get();
+    for (int i = 0; i < m_; i++)
+        for (int j = 0; j < k_; j++) t.logp[i * 32 + j] = t.log[parity.at(i, j)];
+    for (int a = 0; a < k_ && m_ >= 2; a++)
+        for (int b = 0; b < k_; b++)
+            if (a != b)
+                t.logdet[a * 32 + b] = t.log[gf.mul[parity.at(0, a)][parity.at(1, b)] ^ gf.mul[parity.at(0, b)][parity.at(1, a)]];
+    const int64_t pages = (shard_len + (int64_t(1) << kPageShift) - 1) >> kPageShift;
+    page_words_ = std::max<size_t>(1, size_t((pages + 31) / 32));
+    const size_t page_bytes = size_t(k_ + m_ + 1) * page_words_ * 4;
+    SWEC_CUDA(cudaMalloc(reinterpret_cast<void**>(&tables_), sizeof t));
+    SWEC_CUDA(cudaMalloc(reinterpret_cast<void**>(&counters_), kCounters * sizeof(unsigned long long)));
+    SWEC_CUDA(cudaMalloc(reinterpret_cast<void**>(&pages_), page_bytes));
+    SWEC_CUDA(cudaMemcpyAsync(tables_, &t, sizeof t, cudaMemcpyHostToDevice, s));
+    SWEC_CUDA(cudaMemsetAsync(counters_, 0, kCounters * sizeof(unsigned long long), s));
+    SWEC_CUDA(cudaMemsetAsync(counters_ + kSets, 0xff, kSets * sizeof(unsigned long long), s));  // first = max
+    SWEC_CUDA(cudaMemsetAsync(pages_, 0, page_bytes, s));
+    SWEC_CUDA(cudaStreamSynchronize(s));
+    return SWEC_OK;
+}
+
+int DamageLocator::launch(const uint8_t* const* computed, const uint8_t* const* stored, size_t n, int64_t base,
+                          cudaStream_t s) {
+    if (n == 0) return SWEC_OK;
+    LocateParams p;
+    memset(&p, 0, sizeof p);
+    for (int i = 0; i < m_; i++) {
+        p.comp[i] = computed[i];
+        p.stored[i] = stored[i];
+    }
+    p.n = n;
+    p.base = u64(base);
+    p.k = k_;
+    p.m = m_;
+    p.radius = radius_;
+    p.tables = tables_;
+    p.ctr = counters_;
+    p.pages = pages_;
+    p.page_words = page_words_;
+    if (m_ == 4) swec_locate_kernel<4><<<locate_grid<4>(n), 256, 0, s>>>(p);
+    else swec_locate_kernel<0><<<locate_grid<0>(n), 256, 0, s>>>(p);
+    g_kernel_launches++;
+    SWEC_CUDA(cudaGetLastError());
+    return SWEC_OK;
+}
+
+int DamageLocator::collect(swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges) {
+    const int n = k_ + m_;
+    std::vector<unsigned long long> c(kCounters);
+    std::vector<uint32_t> bits(size_t(n + 1) * page_words_);
+    SWEC_CUDA(cudaMemcpy(c.data(), counters_, c.size() * sizeof c[0], cudaMemcpyDeviceToHost));
+    SWEC_CUDA(cudaMemcpy(bits.data(), pages_, bits.size() * 4, cudaMemcpyDeviceToHost));
+    memset(report, 0, sizeof *report);
+    report->columns = uint64_t(shard_len_);
+    report->damaged_columns = c[3 * kSets];
+    report->uncorrectable_columns = c[size_t(n)];
+    report->first_uncorrectable = c[size_t(n)] ? int64_t(c[size_t(kSets + n)]) : -1;
+    report->last_uncorrectable = c[size_t(n)] ? int64_t(c[size_t(2 * kSets + n)]) : -1;
+    for (int i = 0; i < SWEC_MAX_SHARDS; i++) {
+        const bool hit = i < n && c[size_t(i)];
+        report->shard_bytes[i] = hit ? c[size_t(i)] : 0;
+        report->shard_first[i] = hit ? int64_t(c[size_t(kSets + i)]) : -1;
+        report->shard_last[i] = hit ? int64_t(c[size_t(2 * kSets + i)]) : -1;
+    }
+    // maximal runs of flagged pages: shards in ascending id, then the uncorrectable columns
+    const int64_t pages = (shard_len_ + (int64_t(1) << kPageShift) - 1) >> kPageShift;
+    int total = 0;
+    for (int set = 0; set <= n; set++) {
+        const uint32_t* w = bits.data() + size_t(set) * page_words_;
+        auto flagged = [&](int64_t pg) { return (w[pg >> 5] >> (pg & 31)) & 1u; };
+        for (int64_t pg = 0; pg < pages;) {
+            if ((pg & 31) == 0 && w[pg >> 5] == 0) {
+                pg += 32;
+                continue;
+            }
+            if (!flagged(pg)) {
+                pg++;
+                continue;
+            }
+            int64_t end = pg + 1;
+            while (end < pages && flagged(end)) end++;
+            if (total < ranges_cap) {
+                swec_damage_range& r = ranges[total];
+                r.shard_id = set < n ? set : -1;
+                r.reserved = 0;
+                r.offset = pg << kPageShift;
+                r.length = std::min(end << kPageShift, shard_len_) - r.offset;
+            }
+            total++;
+            pg = end;
+        }
+    }
+    if (n_ranges) *n_ranges = total;
+    return SWEC_OK;
+}
+
+}  // namespace swec

@@ -1,0 +1,45 @@
+// seaweedfs_b200/csrc/damage.h — which shard is wrong, from the parity syndrome of every byte column (damage.cu), for
+// the file pipeline (ec_files.cc) and the device-level call (engine.cc).
+#pragma once
+#include <cuda_runtime.h>
+
+#include <cstddef>
+#include <cstdint>
+
+#include "../../include/swec.h"
+#include "gf256.h"
+
+namespace swec {
+
+// The argument rules both entry points share: radius 1 needs m >= 2 and radius 2 needs m >= 4, a report is required,
+// ranges_cap must not be negative and ranges may only be NULL when ranges_cap is 0.
+int check_locate_args(int m, int radius, const swec_damage_report* report, const swec_damage_range* ranges,
+                      int ranges_cap);
+
+// Accumulates, over any number of launches, the shards blamed for every byte column of a shard set whose syndrome
+// (computed parity XOR stored parity) is not zero.  Device memory lives on the device current at init().
+class DamageLocator {
+  public:
+    DamageLocator() = default;
+    DamageLocator(const DamageLocator&) = delete;
+    DamageLocator& operator=(const DamageLocator&) = delete;
+    ~DamageLocator();
+
+    // parity: the m x k parity rows of the code.  Clears the counters on `s` and synchronises it.
+    int init(const Matrix& parity, int64_t shard_len, int radius, cudaStream_t s);
+    // Columns [base, base + n) of the set: computed[p] is the parity re-encoded from the data shards, stored[p] the
+    // parity as found.  Asynchronous on `s`.
+    int launch(const uint8_t* const* computed, const uint8_t* const* stored, size_t n, int64_t base, cudaStream_t s);
+    // After every launch has completed: the report, the page ranges (first ranges_cap of them) and their total.
+    int collect(swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges);
+
+  private:
+    int k_ = 0, m_ = 0, radius_ = 1;
+    int64_t shard_len_ = 0;
+    size_t page_words_ = 0;  // 32-bit words of one page bitmap
+    uint32_t* tables_ = nullptr;
+    unsigned long long* counters_ = nullptr;
+    uint32_t* pages_ = nullptr;
+};
+
+}  // namespace swec

@@ -27,6 +27,7 @@
 #include <thread>
 #include <time.h>
 
+#include "damage.h"
 #include "engine.h"
 #include "io_pool.h"
 #include "volume_format.h"
@@ -77,6 +78,7 @@ struct ReadOp { int stream, fd; int64_t off; size_t dst_off, len; int dfd = -1; 
 struct WriteOp { int stream, fd; int64_t off; int dfd = -1; };  // drain stream `stream` of the slot to fd@off
 struct Item {
     size_t len = 0;
+    int64_t shard_off = 0;  // shard offset of the item's first column
     std::vector<ReadOp> reads;
     std::vector<WriteOp> writes;
 };
@@ -148,9 +150,10 @@ class FilePipeline {
   public:
     PipeStats stats;
     // verify = true: streams [K, K+R) are the parity bytes read from disk; the computed parity goes to
-    // streams [K+R, K+2R) and is only compared on the device (no D2H, no writes).
-    FilePipeline(swec_encoder* enc, const Matrix& rows, size_t chunk, bool verify = false)
-        : enc_(enc), rows_(rows), chunk_(chunk), verify_(verify) {}
+    // streams [K+R, K+2R) and is only compared on the device (no D2H, no writes) — counted per parity stream, or,
+    // with a locator, decoded into the shards it blames.
+    FilePipeline(swec_encoder* enc, const Matrix& rows, size_t chunk, bool verify = false, DamageLocator* locator = nullptr)
+        : enc_(enc), rows_(rows), chunk_(chunk), verify_(verify), locator_(locator) {}
     ~FilePipeline() { shutdown(); }
 
     int start() {
@@ -166,7 +169,7 @@ class FilePipeline {
         if (rc) return rc;
         const size_t nslots = stage_slots();
         const size_t streams = size_t(rows_.cols + rows_.rows * (verify_ ? 2 : 1));
-        if (verify_) {
+        if (verify_ && !locator_) {
             SWEC_CUDA(cudaMalloc(reinterpret_cast<void**>(&dev_bad_), sizeof(unsigned long long) * size_t(rows_.rows)));
             SWEC_CUDA(cudaMemset(dev_bad_, 0, sizeof(unsigned long long) * size_t(rows_.rows)));
         }
@@ -267,7 +270,11 @@ class FilePipeline {
             rc = enc_->apply(rows_, din, dout, len, Layout{}, b.stream);
         }
         if (rc) return set_error(rc, s);
-        if (verify_) {
+        if (locator_) {
+            const uint8_t* stored[SWEC_MAX_SHARDS];
+            for (int r = 0; r < R; r++) stored[r] = b.dev + size_t(K + r) * chunk_;
+            if ((rc = locator_->launch(dout, stored, len, item.shard_off, b.stream))) return set_error(rc, s);
+        } else if (verify_) {
             for (int r = 0; r < R && e == cudaSuccess; r++)
                 e = launch_compare(dout[r], b.dev + size_t(K + r) * chunk_, len, dev_bad_ + r, b.stream);
         } else if (len == chunk_) {
@@ -435,6 +442,7 @@ class FilePipeline {
     const size_t io_piece_ = std::max<size_t>(4096, env_size("SWEC_FILE_IO_PIECE", size_t(2) << 20) & ~size_t(4095));
     double t_begin_ = 0;
     bool verify_ = false;
+    DamageLocator* locator_ = nullptr;  // not owned
     unsigned long long* dev_bad_ = nullptr;
     StagingRing ring_;
     std::vector<Slot> slots_;  // one per ring slot
@@ -465,6 +473,49 @@ void file_pipeline_trim() {  // swec_shutdown(): release parked staging rings
 }  // namespace swec
 
 using namespace swec;
+
+namespace {
+
+// Every shard of the set opened, all of one length: what a parity scrub needs (verify_ec_shards, ec_encoder.rs:177-278).
+int open_all_shards(const std::string& b, const char* const* dirs, int ndirs, int total, FdSet* fds, std::vector<int>* in,
+                    int64_t* size) {
+    in->assign(static_cast<size_t>(total), -1);
+    *size = -1;
+    for (int i = 0; i < total; i++) {
+        const std::string path = find_shard_file(b, dirs, ndirs, i);
+        if (path.empty()) return fail(SWEC_ERR_TOO_FEW_SHARDS, "verify needs all shards; missing " + shard_ext(i));
+        const int fd = open(path.c_str(), O_RDONLY);
+        if (fd < 0) return io_fail("open " + path);
+        fds->fds.push_back(fd);
+        (*in)[size_t(i)] = fd;
+        struct stat st;
+        if (fstat(fd, &st) != 0) return io_fail("fstat shard");
+        if (*size < 0) *size = st.st_size;
+        else if (*size != st.st_size)
+            return fail(SWEC_ERR_SHARD_SIZE, "ec shard size expected " + std::to_string(*size) + " actual " + std::to_string(st.st_size));
+    }
+    return SWEC_OK;
+}
+
+size_t scrub_chunk(int64_t size) {
+    return std::max<size_t>(256, (size_t(std::min<int64_t>(int64_t(env_size("SWEC_FILE_CHUNK", size_t(8) << 20)), std::max<int64_t>(size, 1))) + 255) & ~size_t(255));
+}
+
+// Every column of the shard set through a started verify pipeline, then wait for it.
+int scrub_columns(FilePipeline& pipe, const std::vector<int>& in, int64_t size, size_t chunk) {
+    int rc = SWEC_OK;
+    for (int64_t o = 0; rc == SWEC_OK && o < size; o += int64_t(chunk)) {
+        Item it;
+        it.len = size_t(std::min<int64_t>(int64_t(chunk), size - o));
+        it.shard_off = o;
+        for (size_t i = 0; i < in.size(); i++) it.reads.push_back({int(i), in[i], o, 0, it.len});
+        rc = pipe.submit(std::move(it));
+    }
+    const int rc2 = pipe.finish();
+    return rc == SWEC_OK ? rc2 : rc;
+}
+
+}  // namespace
 
 extern "C" {
 
@@ -720,35 +771,15 @@ int swec_verify_ec_files(const char* base, const char* const* dirs, int ndirs, i
     int rc = swec_encoder_new(k, m, device, &enc);
     if (rc) return rc;
     std::unique_ptr<swec_encoder, void (*)(swec_encoder*)> guard(enc, swec_encoder_free);
-    const int total = k + m;
     FdSet fds;
-    std::vector<int> in(static_cast<size_t>(total), -1);
+    std::vector<int> in;
     int64_t size = -1;
-    for (int i = 0; i < total; i++) {  // verify needs every shard (verify_ec_shards, ec_encoder.rs:177-278)
-        const std::string path = find_shard_file(b, dirs, ndirs, i);
-        if (path.empty()) return fail(SWEC_ERR_TOO_FEW_SHARDS, "verify needs all shards; missing " + shard_ext(i));
-        const int fd = open(path.c_str(), O_RDONLY);
-        if (fd < 0) return io_fail("open " + path);
-        fds.fds.push_back(fd);
-        in[size_t(i)] = fd;
-        struct stat st;
-        if (fstat(fd, &st) != 0) return io_fail("fstat shard");
-        if (size < 0) size = st.st_size;
-        else if (size != st.st_size)
-            return fail(SWEC_ERR_SHARD_SIZE, "ec shard size expected " + std::to_string(size) + " actual " + std::to_string(st.st_size));
-    }
+    if ((rc = open_all_shards(b, dirs, ndirs, k + m, &fds, &in, &size))) return rc;
     const Matrix rows = parity_rows(enc);
-    const size_t chunk = std::max<size_t>(256, (size_t(std::min<int64_t>(int64_t(env_size("SWEC_FILE_CHUNK", size_t(8) << 20)), std::max<int64_t>(size, 1))) + 255) & ~size_t(255));
+    const size_t chunk = scrub_chunk(size);
     FilePipeline pipe(enc, rows, chunk, /*verify=*/true);
     if ((rc = pipe.start())) return rc;
-    for (int64_t o = 0; rc == SWEC_OK && o < size; o += int64_t(chunk)) {
-        Item it;
-        it.len = size_t(std::min<int64_t>(int64_t(chunk), size - o));
-        for (int i = 0; i < total; i++) it.reads.push_back({i, in[size_t(i)], o, 0, it.len});
-        rc = pipe.submit(std::move(it));
-    }
-    const int rc2 = pipe.finish();
-    if (rc == SWEC_OK) rc = rc2;
+    rc = scrub_columns(pipe, in, size, chunk);
     std::vector<unsigned long long> bad(static_cast<size_t>(m), 0);
     if (rc == SWEC_OK) rc = pipe.mismatches(bad.data());
     const std::string msg = pipe.error_message();
@@ -763,6 +794,39 @@ int swec_verify_ec_files(const char* base, const char* const* dirs, int ndirs, i
         all_ok = all_ok && bad[size_t(p)] == 0;
     }
     *ok = all_ok ? 1 : 0;
+    return SWEC_OK;
+}
+
+int swec_locate_ec_damage(const char* base, const char* const* dirs, int ndirs, int k, int m, int device, int radius,
+                          swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges, int* ok) {
+    if (!base || !ok || (ndirs > 0 && !dirs)) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
+    *ok = 0;
+    const std::string b(base);
+    if (k == 0) ec_ratio(b, &k, &m);
+    int rc = check_locate_args(m, radius, report, ranges, ranges_cap);
+    if (rc) return rc;
+    swec_encoder* enc = nullptr;
+    if ((rc = swec_encoder_new(k, m, device, &enc))) return rc;
+    std::unique_ptr<swec_encoder, void (*)(swec_encoder*)> guard(enc, swec_encoder_free);
+    FdSet fds;
+    std::vector<int> in;
+    int64_t size = -1;
+    if ((rc = open_all_shards(b, dirs, ndirs, k + m, &fds, &in, &size))) return rc;
+    const Matrix rows = parity_rows(enc);
+    const size_t chunk = scrub_chunk(size);
+    DamageLocator locator;
+    FilePipeline pipe(enc, rows, chunk, /*verify=*/true, &locator);
+    if ((rc = pipe.start())) return rc;
+    rc = locator.init(rows, size, radius, enc->stream);
+    if (rc == SWEC_OK) rc = scrub_columns(pipe, in, size, chunk);
+    if (rc == SWEC_OK) rc = locator.collect(report, ranges, ranges_cap, n_ranges);
+    const std::string msg = pipe.error_message();
+    pipe.shutdown();
+    if (rc) {
+        if (!msg.empty()) set_last_error(msg);
+        return rc;
+    }
+    *ok = report->damaged_columns == 0 ? 1 : 0;
     return SWEC_OK;
 }
 

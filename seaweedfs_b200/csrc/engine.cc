@@ -1,5 +1,6 @@
 // seaweedfs_b200/csrc/engine.cc — encoder object, matrix→kernel dispatch, host staging pipeline.
 #include "engine.h"
+#include "damage.h"
 #include "io_pool.h"
 #include "volume_format.h"
 
@@ -1159,6 +1160,48 @@ int swec_write_dat_device(swec_encoder* e, const void* const* data_shards, int64
                                       cudaMemcpyDeviceToDevice, s));
     }
     return SWEC_OK;
+}
+
+int swec_locate_damage_device(swec_encoder* e, const void* const* shards, size_t n, int radius, swec_damage_report* report,
+                              swec_damage_range* ranges, int ranges_cap, int* n_ranges, void* stream) {
+    if (!e || !shards) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
+    int rc = check_locate_args(e->m, radius, report, ranges, ranges_cap);
+    if (rc) return rc;
+    const int k = e->k, m = e->m;
+    for (int i = 0; i < k + m; i++)
+        if (!shards[i]) return fail(SWEC_ERR_INVALID_ARG, "NULL shard");
+    const uint8_t* const* sh = reinterpret_cast<const uint8_t* const*>(shards);
+    std::lock_guard<std::mutex> lock(e->mu);
+    if ((rc = e->ensure_device())) return rc;
+    cudaStream_t s = pick_stream(e, stream);
+    const Matrix rows = parity_rows(e);
+    DamageLocator locator;
+    if ((rc = locator.init(rows, int64_t(n), radius, s))) return rc;
+    // the computed parity goes to scratch a piece at a time: a 3 GiB shard set needs 1 GiB of it, not 12 GiB
+    const size_t piece = std::min(n, size_t(256) << 20);
+    struct Scratch {  // stream-ordered: freed after the work queued on s, on every exit path
+        uint8_t* p = nullptr;
+        cudaStream_t s;
+        ~Scratch() {
+            if (p) cudaFreeAsync(p, s);
+        }
+    } scratch{nullptr, s};
+    if (piece) SWEC_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&scratch.p), size_t(m) * piece, s));
+    for (size_t off = 0; off < n; off += piece) {
+        const size_t len = std::min(piece, n - off);
+        const uint8_t* in[SWEC_MAX_SHARDS];
+        const uint8_t* stored[SWEC_MAX_SHARDS];
+        uint8_t* comp[SWEC_MAX_SHARDS];
+        for (int i = 0; i < k; i++) in[i] = sh[i] + off;
+        for (int p = 0; p < m; p++) {
+            comp[p] = scratch.p + size_t(p) * piece;
+            stored[p] = sh[k + p] + off;
+        }
+        if ((rc = e->apply(rows, in, comp, len, Layout{}, s))) return rc;
+        if ((rc = locator.launch(comp, stored, len, int64_t(off), s))) return rc;
+    }
+    SWEC_CUDA(cudaStreamSynchronize(s));
+    return locator.collect(report, ranges, ranges_cap, n_ranges);
 }
 
 int swec_stream_synchronize(swec_encoder* e, void* stream) {

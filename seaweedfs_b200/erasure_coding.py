@@ -18,7 +18,7 @@ from dataclasses import dataclass
 
 import numpy as np
 
-from ._native import STATUS, Interval, NeedleRead, ReconstructItem, SwecError, check, lib
+from ._native import STATUS, DamageRange, DamageReport, Interval, NeedleRead, ReconstructItem, SwecError, check, lib
 
 DataShardsCount = 10                               # ec_encoder.go:20
 ParityShardsCount = 4                              # ec_encoder.go:21
@@ -174,6 +174,15 @@ class Encoder:
         check(lib().swec_write_dat_device(self._h, _ptrs(data_shard_ptrs), dat_size, large_block, small_block,
                                           dat_out_ptr, stream))
 
+    def locate_damage_device(self, shard_ptrs, shard_len: int, radius: int = 1, max_ranges: int = 4096,
+                             stream: int = 0) -> dict:
+        """Which shards of k+m shards in device memory are wrong, from the parity syndrome of every byte column
+        (swec_locate_damage_device).  Same result as locate_ec_damage, without "ok"."""
+        report, ranges, n = DamageReport(), (DamageRange * max(1, max_ranges))(), C.c_int(0)
+        check(lib().swec_locate_damage_device(self._h, _ptrs(shard_ptrs), shard_len, radius, C.byref(report), ranges,
+                                              max_ranges, C.byref(n), stream))
+        return _damage_result(report, ranges, n.value, max_ranges)
+
     def synchronize(self, stream: int = 0) -> None:
         check(lib().swec_stream_synchronize(self._h, stream))
 
@@ -285,6 +294,29 @@ def verify_ec_files(base_file_name: str, additional_dirs: list[str] | None = Non
     check(lib().swec_verify_ec_files(base_file_name.encode(), arr, len(dirs), k, m, dev, bad, C.byref(ok)))
     nm = ctx.ParityShards if ctx else ParityShardsCount
     return bool(ok.value), list(bad[:nm])
+
+
+def _damage_result(report, ranges, n_ranges: int, max_ranges: int) -> dict:
+    shards = {i: (int(report.shard_bytes[i]), int(report.shard_first[i]), int(report.shard_last[i]))
+              for i in range(MaxShardCount) if report.shard_bytes[i]}
+    return {"columns": int(report.columns), "damaged_columns": int(report.damaged_columns),
+            "uncorrectable_columns": int(report.uncorrectable_columns),
+            "first_uncorrectable": int(report.first_uncorrectable), "last_uncorrectable": int(report.last_uncorrectable),
+            "shards": shards, "ranges": [(r.shard_id, r.offset, r.length) for r in ranges[:min(n_ranges, max_ranges)]],
+            "n_ranges": n_ranges}
+
+
+def locate_ec_damage(base_file_name: str, additional_dirs: list[str] | None = None, ctx: ECContext | None = None,
+                     device: int = 0, radius: int = 1, max_ranges: int = 4096) -> dict:
+    """Which shard files are wrong where parity does not match (swec_locate_ec_damage).  Returns ok, the column
+    counts, "shards" = {shard id: (bytes blamed, first offset, last offset)} for the shards with damage, the
+    uncorrectable summary, "ranges" = [(shard id or -1, offset, length)] (the first max_ranges) and "n_ranges"."""
+    arr, nd = _dirs(additional_dirs)
+    k, m, dev = (ctx.DataShards, ctx.ParityShards, ctx.device) if ctx else (0, 0, device)
+    report, ranges, n, ok = DamageReport(), (DamageRange * max(1, max_ranges))(), C.c_int(0), C.c_int(0)
+    check(lib().swec_locate_ec_damage(base_file_name.encode(), arr, nd, k, m, dev, radius, C.byref(report), ranges,
+                                      max_ranges, C.byref(n), C.byref(ok)))
+    return {"ok": bool(ok.value), **_damage_result(report, ranges, n.value, max_ranges)}
 
 
 def write_dat_file(base_file_name: str, dat_file_size: int, shard_file_names: list[str],
