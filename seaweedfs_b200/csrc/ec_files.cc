@@ -37,6 +37,35 @@ namespace {
 
 int io_fail(const std::string& what) { return fail(SWEC_ERR_IO, what + ": " + strerror(errno)); }
 
+// The first failure of work spread over several threads.  Error texts are thread-local, so the status keeps the
+// last_error() text of the thread that reported it, and get() hands both to the thread that owns the work.
+class FirstError {
+  public:
+    int report(int rc) {  // any thread; returns rc
+        std::lock_guard<std::mutex> lk(mu_);
+        if (rc && !rc_) {
+            rc_ = rc;
+            text_ = last_error();
+        }
+        return rc;
+    }
+    int fail(int rc, const std::string& msg) { return report(swec::fail(rc, msg)); }
+    int status() {
+        std::lock_guard<std::mutex> lk(mu_);
+        return rc_;
+    }
+    int get() {  // the first status, its text set as the calling thread's last error
+        std::lock_guard<std::mutex> lk(mu_);
+        if (rc_) set_last_error(text_);
+        return rc_;
+    }
+
+  private:
+    std::mutex mu_;
+    int rc_ = 0;
+    std::string text_;
+};
+
 // Reserving extents pays on disk filesystems (once instead of 14 files growing 8 MiB at a time) and costs on tmpfs,
 // where it zero-fills every page that the writers overwrite a moment later.  The reservation must NOT change the
 // visible file size: DiskLocation.validateEcVolume (disk_location_ec.go:455-530) and rebuildEcFiles' equal-length
@@ -47,10 +76,6 @@ bool worth_preallocating(int fd) {
     struct statfs fs;
     if (fstatfs(fd, &fs) != 0) return true;
     return fs.f_type != 0x01021994 /* TMPFS_MAGIC */ && fs.f_type != 0x858458f6 /* RAMFS_MAGIC */;
-}
-
-void reserve_extents(int fd, int64_t size) {  // best effort; the file's length stays what has been written
-    if (size > 0 && fallocate(fd, FALLOC_FL_KEEP_SIZE, 0, off_t(size)) != 0) errno = 0;
 }
 
 // a second descriptor on the same file with O_DIRECT, or -1 (tmpfs and friends refuse it; so may the caller's option)
@@ -66,6 +91,10 @@ inline bool direct_ok(int dfd, int64_t off, size_t len, const void* buf) {
 
 struct FdSet {
     std::vector<int> fds;
+    int keep(int fd) {  // closed with the set unless negative; returns fd
+        if (fd >= 0) fds.push_back(fd);
+        return fd;
+    }
     ~FdSet() {
         for (int fd : fds)
             if (fd >= 0) close(fd);
@@ -120,6 +149,13 @@ IoPool& file_io_pool() {
     return *pool;
 }
 
+// Slot pitch of a pipeline over streams of `span` bytes: the configured chunk (8 MiB), or less for a shorter span, in
+// whole 256-byte units.  Parked rings are matched by slot size, so every file-level call takes its chunk from here.
+size_t file_chunk(int64_t span) {
+    const int64_t cap = int64_t(env_size("SWEC_FILE_CHUNK", size_t(8) << 20));
+    return std::max<size_t>(256, (size_t(std::min<int64_t>(cap, std::max<int64_t>(span, 1))) + 255) & ~size_t(255));
+}
+
 // Staging rings outlive a call: pinning (mmap + mbind + cudaHostRegister) and un-pinning 3 x 14 x 8 MiB costs
 // 0.1-2 s per call, as much as the pipeline itself spends on an 8 GiB volume.  A volume
 // server encodes volume after volume, so finished pipelines park their ring here (per device, slot size and slot
@@ -145,6 +181,19 @@ struct PipeStats {
     }
 };
 
+// The outputs' final size is known up front: reserve it (best effort, one I/O thread per file), so that the writers
+// fill extents that already exist instead of growing every file 8 MiB at a time under the filesystem's allocation lock.
+// Returns the seconds spent reserving: 0 where it does not pay.
+double reserve_extents(const std::vector<int>& outs, int64_t size) {
+    if (size <= 0 || !worth_preallocating(outs[0])) return 0;
+    const double t0 = PipeStats::now();
+    file_io_pool().parallel_for(int(outs.size()), [&](int i) -> int {
+        if (fallocate(outs[size_t(i)], FALLOC_FL_KEEP_SIZE, 0, off_t(size)) != 0) errno = 0;  // the length stays as written
+        return 0;
+    });
+    return PipeStats::now() - t0;
+}
+
 // K input streams + R computed streams per slot, pitch = chunk bytes.
 class FilePipeline {
   public:
@@ -157,13 +206,7 @@ class FilePipeline {
     ~FilePipeline() { shutdown(); }
 
     int start() {
-        const double t_start = PipeStats::now();
-        struct SetupTimer {
-            PipeStats& st;
-            double t0;
-            ~SetupTimer() { st.setup += PipeStats::now() - t0; st.total -= 0; }
-        } setup_timer{stats, t_start};
-        t_begin_ = t_start;
+        t_begin_ = PipeStats::now();
         enc_->never_wait_for_jit = !getenv("SWEC_FILE_JIT_WAIT");
         int rc = enc_->ensure_device();
         if (rc) return rc;
@@ -192,6 +235,7 @@ class FilePipeline {
         io_ = &file_io_pool();
         writer_ = std::thread([this] { writer_loop(); });
         started_ = true;
+        stats.setup = PipeStats::now() - t_begin_;  // printed only for a pipeline that started
         return SWEC_OK;
     }
 
@@ -201,8 +245,8 @@ class FilePipeline {
         double t0 = PipeStats::now();
         {
             std::unique_lock<std::mutex> lk(mu_);
-            cv_.wait(lk, [&] { return !free_.empty() || error_; });
-            if (error_) return error_;
+            cv_.wait(lk, [&] { return !free_.empty() || first_.status(); });
+            if (const int rc = first_.status()) return rc;
             s = free_.front();
             free_.pop_front();
         }
@@ -234,9 +278,7 @@ class FilePipeline {
                 const ssize_t n = pread(fd, dst + got, len - got, off_t(off + int64_t(got)));
                 if (n < 0) {
                     if (errno == EINTR) continue;
-                    const int rc = io_fail("pread");
-                    note_error(last_error());
-                    return rc;
+                    return first_.report(io_fail("pread"));
                 }
                 if (n == 0) break;  // EOF: the rest reads as zero (ec_encoder.go:258-262)
                 got += size_t(n);
@@ -244,10 +286,7 @@ class FilePipeline {
             if (got < len) memset(dst + got, 0, len - got);
             return SWEC_OK;
         };
-        if (const int rrc = io_->parallel_for(int(rpieces.size()), read_one)) {
-            set_last_error(noted_error());
-            return set_error(rrc, s);
-        }
+        if (const int rrc = io_->parallel_for(int(rpieces.size()), read_one)) return set_error(rrc, s);
         t0 = PipeStats::now();
         stats.read += t0 - t1;
         if (cudaSetDevice(enc_->device) != cudaSuccess) return set_error(fail(SWEC_ERR_CUDA, "cudaSetDevice"), s);
@@ -295,13 +334,14 @@ class FilePipeline {
         return SWEC_OK;
     }
 
-    int parallel_for(int n, const std::function<int(int)>& fn) { return io_->parallel_for(n, fn); }
-
-    // wait for everything queued so far; returns the first error
+    // wait for everything queued so far, or for the first error of submit(), the reads or the writes: returned, with
+    // its text set as the calling thread's last error
     int finish() {
-        std::unique_lock<std::mutex> lk(mu_);
-        cv_.wait(lk, [&] { return (inflight_.empty() && free_.size() == slots_.size()) || error_; });
-        return error_;
+        {
+            std::unique_lock<std::mutex> lk(mu_);
+            cv_.wait(lk, [&] { return (inflight_.empty() && free_.size() == slots_.size()) || first_.status(); });
+        }
+        return first_.get();
     }
 
     void report(const char* what) {
@@ -325,7 +365,7 @@ class FilePipeline {
         if (writer_.joinable()) writer_.join();
         io_ = nullptr;
         cudaSetDevice(enc_->device);
-        bool healthy = error_ == 0;
+        bool healthy = first_.status() == 0;
         for (StagingSlot& b : ring_.slots)
             if (cudaStreamSynchronize(b.stream) != cudaSuccess) {
                 cudaGetLastError();
@@ -353,24 +393,12 @@ class FilePipeline {
     }
 
   private:
-    // I/O runs on pool threads whose thread-local error text the submitting thread cannot see
-    void note_error(const char* msg) {
-        std::lock_guard<std::mutex> lk(note_mu_);
-        if (noted_.empty()) noted_ = msg;
-    }
-    std::string noted_error() {
-        std::lock_guard<std::mutex> lk(note_mu_);
-        return noted_;
-    }
-    std::mutex note_mu_;
-    std::string noted_;
-
+    // Every failure reaches first_ under mu_, here or in the writer loop, and a wake-up follows, so no waiter can test
+    // first_ just before the report and then sleep through it.  I/O tasks report earlier, without mu_, to keep their
+    // own text; the report under mu_ then finds the status taken.
     int set_error(int rc, Slot* s) {
         std::lock_guard<std::mutex> lk(mu_);
-        if (!error_) {
-            error_ = rc;
-            error_msg_ = last_error();
-        }
+        first_.report(rc);
         if (s) free_.push_back(s);
         cv_.notify_all();
         return rc;
@@ -411,26 +439,20 @@ class FilePipeline {
                         const ssize_t n = pwrite(fd, src + put, pc.len - put, off_t(off + int64_t(put)));
                         if (n < 0) {
                             if (errno == EINTR) continue;
-                            const int rc2 = io_fail("pwrite");
-                            note_error(last_error());
-                            return rc2;
+                            return first_.report(io_fail("pwrite"));
                         }
                         put += size_t(n);
                     }
                     return SWEC_OK;
                 };
                 rc = io_->parallel_for(int(wpieces.size()), write_one);
-                if (rc) set_last_error(noted_error());
                 stats.write += PipeStats::now() - tw1;
             }
             {
                 std::lock_guard<std::mutex> lk(mu_);
                 inflight_.pop_front();
                 free_.push_back(s);
-                if (rc && !error_) {
-                    error_ = rc;
-                    error_msg_ = last_error();
-                }
+                first_.report(rc);
             }
             cv_.notify_all();
         }
@@ -451,12 +473,8 @@ class FilePipeline {
     std::condition_variable cv_;
     std::thread writer_;
     IoPool* io_ = nullptr;  // the process-wide pool (not owned)
-    int error_ = 0;
-    std::string error_msg_;
+    FirstError first_;      // of submit(), the reader's and writer's I/O tasks and the writer
     bool stop_ = false, started_ = false;
-
-  public:
-    const std::string& error_message() const { return error_msg_; }
 };
 
 }  // namespace
@@ -476,43 +494,67 @@ using namespace swec;
 
 namespace {
 
+struct EncoderFree {
+    void operator()(swec_encoder* e) const { swec_encoder_free(e); }
+};
+using CallEncoder = std::unique_ptr<swec_encoder, EncoderFree>;
+
+// the encoder of one file-level call, freed on every way out of it
+int new_call_encoder(int k, int m, int device, CallEncoder* enc) {
+    swec_encoder* e = nullptr;
+    const int rc = swec_encoder_new(k, m, device, &e);
+    enc->reset(e);
+    return rc;
+}
+
+// findShardFile, opened read-only into `fds` (*fd = -1: no such shard) — with its O_DIRECT twin in *dfd when asked for
+int open_shard(const std::string& b, const char* const* dirs, int ndirs, int i, FdSet* fds, int* fd, int* dfd = nullptr,
+               bool direct = false) {
+    *fd = -1;
+    const std::string path = find_shard_file(b, dirs, ndirs, i);
+    if (path.empty()) return SWEC_OK;
+    if ((*fd = fds->keep(open(path.c_str(), O_RDONLY))) < 0) return io_fail("open " + path);
+    if (dfd) *dfd = fds->keep(open_direct(path, O_RDONLY, direct));
+    return SWEC_OK;
+}
+
+int shard_size_error(int64_t expected, int64_t actual) {
+    return fail(SWEC_ERR_SHARD_SIZE, "ec shard size expected " + std::to_string(expected) + " actual " + std::to_string(actual));
+}
+
+// rebuildEcFiles (ec_encoder.go:323-377): every shard has the length of the first one checked (*size < 0: none yet)
+int check_length(int fd, int64_t* size) {
+    struct stat st;
+    if (fstat(fd, &st) != 0) return io_fail("fstat shard");
+    if (*size < 0) *size = st.st_size;
+    return *size == st.st_size ? SWEC_OK : shard_size_error(*size, st.st_size);
+}
+
 // Every shard of the set opened, all of one length: what a parity scrub needs (verify_ec_shards, ec_encoder.rs:177-278).
+// The first problem in shard order wins.
 int open_all_shards(const std::string& b, const char* const* dirs, int ndirs, int total, FdSet* fds, std::vector<int>* in,
                     int64_t* size) {
     in->assign(static_cast<size_t>(total), -1);
     *size = -1;
     for (int i = 0; i < total; i++) {
-        const std::string path = find_shard_file(b, dirs, ndirs, i);
-        if (path.empty()) return fail(SWEC_ERR_TOO_FEW_SHARDS, "verify needs all shards; missing " + shard_ext(i));
-        const int fd = open(path.c_str(), O_RDONLY);
-        if (fd < 0) return io_fail("open " + path);
-        fds->fds.push_back(fd);
-        (*in)[size_t(i)] = fd;
-        struct stat st;
-        if (fstat(fd, &st) != 0) return io_fail("fstat shard");
-        if (*size < 0) *size = st.st_size;
-        else if (*size != st.st_size)
-            return fail(SWEC_ERR_SHARD_SIZE, "ec shard size expected " + std::to_string(*size) + " actual " + std::to_string(st.st_size));
+        int& fd = (*in)[size_t(i)];
+        if (const int rc = open_shard(b, dirs, ndirs, i, fds, &fd)) return rc;
+        if (fd < 0) return fail(SWEC_ERR_TOO_FEW_SHARDS, "verify needs all shards; missing " + shard_ext(i));
+        if (const int rc = check_length(fd, size)) return rc;
     }
     return SWEC_OK;
 }
 
-size_t scrub_chunk(int64_t size) {
-    return std::max<size_t>(256, (size_t(std::min<int64_t>(int64_t(env_size("SWEC_FILE_CHUNK", size_t(8) << 20)), std::max<int64_t>(size, 1))) + 255) & ~size_t(255));
-}
-
-// Every column of the shard set through a started verify pipeline, then wait for it.
+// Every column of the shard set through a started verify pipeline; returns pipe.finish().
 int scrub_columns(FilePipeline& pipe, const std::vector<int>& in, int64_t size, size_t chunk) {
-    int rc = SWEC_OK;
-    for (int64_t o = 0; rc == SWEC_OK && o < size; o += int64_t(chunk)) {
+    for (int64_t o = 0; o < size; o += int64_t(chunk)) {
         Item it;
         it.len = size_t(std::min<int64_t>(int64_t(chunk), size - o));
         it.shard_off = o;
         for (size_t i = 0; i < in.size(); i++) it.reads.push_back({int(i), in[i], o, 0, it.len});
-        rc = pipe.submit(std::move(it));
+        if (pipe.submit(std::move(it))) break;
     }
-    const int rc2 = pipe.finish();
-    return rc == SWEC_OK ? rc2 : rc;
+    return pipe.finish();
 }
 
 }  // namespace
@@ -526,22 +568,19 @@ int swec_generate_ec_files(const char* base, int64_t buffer_size, int64_t large,
     // encodeData: "unexpected zero buffer size" / "unexpected block size %d buffer size %d" (ec_encoder.go:204-212)
     if (buffer_size <= 0 || large <= 0 || small <= 0 || large % buffer_size || small % buffer_size)
         return fail(SWEC_ERR_INVALID_ARG, "block sizes must be positive multiples of buffer_size");
-    swec_encoder* enc = nullptr;
-    int rc = swec_encoder_new(k, m, device, &enc);
+    CallEncoder enc;
+    int rc = new_call_encoder(k, m, device, &enc);
     if (rc) return rc;
-    std::unique_ptr<swec_encoder, void (*)(swec_encoder*)> guard(enc, swec_encoder_free);
 
     const std::string b(base);
     FdSet fds;
-    const int dat = open((b + ".dat").c_str(), O_RDONLY);
+    const int dat = fds.keep(open((b + ".dat").c_str(), O_RDONLY));
     if (dat < 0) return io_fail("failed to open dat file " + b + ".dat");
-    fds.fds.push_back(dat);
     struct stat st;
     if (fstat(dat, &st) != 0) return io_fail("failed to stat dat file");
     const int total = k + m;
     const long direct = g_opt_file_direct_io.load();
-    const int dat_d = open_direct(b + ".dat", O_RDONLY, direct & 1);
-    if (dat_d >= 0) fds.fds.push_back(dat_d);
+    const int dat_d = fds.keep(open_direct(b + ".dat", O_RDONLY, direct & 1));
     std::vector<int> outs(static_cast<size_t>(total), -1), outs_d(static_cast<size_t>(total), -1);
     {
         // openEcFiles (ec_encoder.go:224-238): O_TRUNC|O_CREAT|O_WRONLY 0644 for every shard — all at once.  Truncating
@@ -557,8 +596,8 @@ int swec_generate_ec_files(const char* base, int64_t buffer_size, int64_t large,
             });
         for (auto& t : openers) t.join();
         for (int i = 0; i < total; i++) {
-            if (outs[size_t(i)] >= 0) fds.fds.push_back(outs[size_t(i)]);
-            if (outs_d[size_t(i)] >= 0) fds.fds.push_back(outs_d[size_t(i)]);
+            fds.keep(outs[size_t(i)]);
+            fds.keep(outs_d[size_t(i)]);
         }
         for (int i = 0; i < total; i++)
             if (outs[size_t(i)] < 0) {
@@ -567,27 +606,13 @@ int swec_generate_ec_files(const char* base, int64_t buffer_size, int64_t large,
             }
     }
 
-    const Matrix rows = parity_rows(enc);
-    const int64_t max_chunk = int64_t(env_size("SWEC_FILE_CHUNK", size_t(8) << 20));
-    const size_t chunk = size_t(std::min<int64_t>(max_chunk, std::max(large, small)) + 255) & ~size_t(255);
+    const Matrix rows = parity_rows(enc.get());
+    const size_t chunk = file_chunk(std::max(large, small));
     const double t_opened = PipeStats::now();
-    FilePipeline pipe(enc, rows, chunk);
+    FilePipeline pipe(enc.get(), rows, chunk);
     if ((rc = pipe.start())) return rc;
-
-    // The final shard size is known up front: reserve its extents (visible length unchanged) — one I/O thread per
-    // file — so the writers fill pages/extents that already exist instead of
-    // growing 14 files 8 MiB at a time under the filesystem's allocation lock (best effort).
     const StripeGeometry g(st.st_size, k, large, small);
-    if (worth_preallocating(outs[0])) {
-        const double tp = PipeStats::now();
-        const int64_t shard_size = g.shard_size();
-        if (shard_size > 0)
-            pipe.parallel_for(total, [&](int i) -> int {
-                reserve_extents(outs[size_t(i)], shard_size);
-                return 0;
-            });
-        pipe.stats.prealloc += PipeStats::now() - tp;
-    }
+    pipe.stats.prealloc += reserve_extents(outs, g.shard_size());
 
     int64_t processed = 0, shard_off = 0;
     auto encode_row = [&](int64_t block) -> int {  // encodeData on one row of k blocks, chunk by chunk
@@ -626,17 +651,14 @@ int swec_generate_ec_files(const char* base, int64_t buffer_size, int64_t large,
         processed += n * g.small_row();
         rows_left -= n;
     }
-    const int rc2 = pipe.finish();
-    if (rc == SWEC_OK) rc = rc2;
+    rc = pipe.finish();  // the first error, submit()'s included
     pipe.report("generate_ec_files");
     const double t_piped = PipeStats::now();
-    const std::string msg = pipe.error_message();
     pipe.shutdown();
     if (getenv("SWEC_PIPE_STATS"))
         fprintf(stderr, "{\"call\": \"generate_ec_files\", \"dat_bytes\": %lld, \"open_and_truncate_s\": %.3f, \"pipeline_s\": %.3f, "
                         "\"teardown_s\": %.3f}\n",
                 (long long)st.st_size, t_opened - t_call, t_piped - t_opened, PipeStats::now() - t_piped);
-    if (rc && !msg.empty()) set_last_error(msg);
     return rc;
 }
 
@@ -651,34 +673,23 @@ int swec_rebuild_ec_files(const char* base, const char* const* dirs, int ndirs, 
     *n_rebuilt = 0;
     const std::string b(base);
     if (k == 0) ec_ratio(b, &k, &m);  // RebuildEcFiles (ec_encoder.go:76-95)
-    swec_encoder* enc = nullptr;
-    int rc = swec_encoder_new(k, m, device, &enc);
+    CallEncoder enc;
+    int rc = new_call_encoder(k, m, device, &enc);
     if (rc) return rc;
-    std::unique_ptr<swec_encoder, void (*)(swec_encoder*)> guard(enc, swec_encoder_free);
     const int total = k + m;
 
     // pass 1: which shards exist
     FdSet fds;
     const long direct = g_opt_file_direct_io.load();
-    std::vector<int> in(static_cast<size_t>(total), -1), in_d(static_cast<size_t>(total), -1), out_d(static_cast<size_t>(total), -1);
+    std::vector<int> in(static_cast<size_t>(total), -1), in_d(static_cast<size_t>(total), -1);
     std::vector<uint8_t> present(static_cast<size_t>(total), 0);
-    int npresent = 0;
     std::vector<uint32_t> missing;
     for (int i = 0; i < total; i++) {
-        const std::string path = find_shard_file(b, dirs, ndirs, i);
-        if (path.empty()) {
-            missing.push_back(uint32_t(i));
-            continue;
-        }
-        const int fd = open(path.c_str(), O_RDONLY);
-        if (fd < 0) return io_fail("open " + path);
-        fds.fds.push_back(fd);
-        in[size_t(i)] = fd;
-        in_d[size_t(i)] = open_direct(path, O_RDONLY, direct & 1);
-        if (in_d[size_t(i)] >= 0) fds.fds.push_back(in_d[size_t(i)]);
-        present[size_t(i)] = 1;
-        npresent++;
+        if ((rc = open_shard(b, dirs, ndirs, i, &fds, &in[size_t(i)], &in_d[size_t(i)], direct & 1))) return rc;
+        present[size_t(i)] = in[size_t(i)] >= 0;
+        if (!present[size_t(i)]) missing.push_back(uint32_t(i));
     }
+    const int npresent = total - int(missing.size());
     if (npresent < k)  // before any output file exists — ec_encoder.go:172-175
         return fail(SWEC_ERR_TOO_FEW_SHARDS, "not enough shards to rebuild " + b + ": found " + std::to_string(npresent) +
                                                  " shards, need at least " + std::to_string(k));
@@ -688,7 +699,7 @@ int swec_rebuild_ec_files(const char* base, const char* const* dirs, int ndirs, 
     // pass 2: create the outputs — ec_encoder.go:182-193.  Whatever goes wrong from here on, the caller gets no
     // shard ids (the reference returns nil ids with the error) and no half-written output survives: a shard file
     // that exists is taken for a present input by the next rebuild (findShardFile), so a partial one must not stay.
-    std::vector<int> out(static_cast<size_t>(total), -1);
+    std::vector<int> out, out_d;  // in the order of `missing`
     struct Undo {
         const std::string& b;
         const std::vector<uint32_t>& ids;
@@ -702,61 +713,41 @@ int swec_rebuild_ec_files(const char* base, const char* const* dirs, int ndirs, 
         }
     } undo{b, missing, n_rebuilt};
     for (uint32_t id : missing) {
-        const int fd = open((b + shard_ext(int(id))).c_str(), O_TRUNC | O_WRONLY | O_CREAT, 0644);
+        const int fd = fds.keep(open((b + shard_ext(int(id))).c_str(), O_TRUNC | O_WRONLY | O_CREAT, 0644));
         if (fd < 0) return io_fail("create " + b + shard_ext(int(id)));
         undo.created++;
-        fds.fds.push_back(fd);
-        out[id] = fd;
-        out_d[id] = open_direct(b + shard_ext(int(id)), O_WRONLY, direct & 2);
-        if (out_d[id] >= 0) fds.fds.push_back(out_d[id]);
+        out.push_back(fd);
+        out_d.push_back(fds.keep(open_direct(b + shard_ext(int(id)), O_WRONLY, direct & 2)));
     }
 
-    // rebuildEcFiles (ec_encoder.go:323-377): every present shard must have the same length; the
-    // reference steps in 1 MiB reads and fails at the first short, unequal one.
+    // every present shard must have the same length; the reference steps in 1 MiB reads and fails at the first
+    // short, unequal one
     int64_t size = -1;
-    for (int i = 0; i < total; i++) {
-        if (!present[size_t(i)]) continue;
-        struct stat st;
-        if (fstat(in[size_t(i)], &st) != 0) return io_fail("fstat shard");
-        if (size < 0) size = st.st_size;
-        else if (size != st.st_size)
-            return fail(SWEC_ERR_SHARD_SIZE, "ec shard size expected " + std::to_string(size) + " actual " + std::to_string(st.st_size));
-    }
+    for (int fd : in)
+        if (fd >= 0 && (rc = check_length(fd, &size))) return rc;
     // quirk kept: the reference reads in small-block buffers, and a length above 1 MiB that is not a multiple of
     // 1 MiB errors on the last read
     const int64_t mib = kSmallBlockSize;
     const bool ragged = size > mib && size % mib != 0;
     const int64_t todo = ragged ? size / mib * mib : size;
 
-    std::vector<int> ins, outs_idx;
+    std::vector<int> ins, outs_idx;  // outs_idx == missing: fused row r rebuilds the shard of out[r]
     Matrix fused;
     if (!rs_reconstruct_plan(enc->gen, k, present.data(), false, &ins, &outs_idx, &fused))
         return fail(SWEC_ERR_TOO_FEW_SHARDS, "not enough shards");
-    const size_t chunk = std::max<size_t>(256, (size_t(std::min<int64_t>(int64_t(env_size("SWEC_FILE_CHUNK", size_t(8) << 20)), std::max<int64_t>(todo, 1))) + 255) & ~size_t(255));
-    FilePipeline pipe(enc, fused, chunk);
+    const size_t chunk = file_chunk(todo);
+    FilePipeline pipe(enc.get(), fused, chunk);
     if ((rc = pipe.start())) return rc;
-    if (todo > 0 && worth_preallocating(out[size_t(outs_idx[0])]))
-        pipe.parallel_for(int(outs_idx.size()), [&](int r) -> int {
-            reserve_extents(out[size_t(outs_idx[size_t(r)])], todo);
-            return 0;
-        });
+    reserve_extents(out, todo);
     for (int64_t o = 0; rc == SWEC_OK && o < todo; o += int64_t(chunk)) {
         Item it;
         it.len = size_t(std::min<int64_t>(int64_t(chunk), todo - o));
         for (int i = 0; i < k; i++) it.reads.push_back({i, in[size_t(ins[size_t(i)])], o, 0, it.len, in_d[size_t(ins[size_t(i)])]});
-        for (size_t r = 0; r < outs_idx.size(); r++)
-            it.writes.push_back({k + int(r), out[size_t(outs_idx[r])], o, out_d[size_t(outs_idx[r])]});
+        for (size_t r = 0; r < out.size(); r++) it.writes.push_back({k + int(r), out[r], o, out_d[r]});
         rc = pipe.submit(std::move(it));
     }
-    const int rc2 = pipe.finish();
-    if (rc == SWEC_OK) rc = rc2;
-    const std::string msg = pipe.error_message();
-    pipe.shutdown();
-    if (rc) {
-        if (!msg.empty()) set_last_error(msg);
-        return rc;
-    }
-    if (ragged) return fail(SWEC_ERR_SHARD_SIZE, "ec shard size expected 1048576 actual " + std::to_string(size % mib));
+    if ((rc = pipe.finish())) return rc;
+    if (ragged) return shard_size_error(mib, size % mib);
     undo.armed = false;
     return SWEC_OK;
 }
@@ -767,27 +758,19 @@ int swec_verify_ec_files(const char* base, const char* const* dirs, int ndirs, i
     *ok = 0;
     const std::string b(base);
     if (k == 0) ec_ratio(b, &k, &m);
-    swec_encoder* enc = nullptr;
-    int rc = swec_encoder_new(k, m, device, &enc);
+    CallEncoder enc;
+    int rc = new_call_encoder(k, m, device, &enc);
     if (rc) return rc;
-    std::unique_ptr<swec_encoder, void (*)(swec_encoder*)> guard(enc, swec_encoder_free);
     FdSet fds;
     std::vector<int> in;
     int64_t size = -1;
     if ((rc = open_all_shards(b, dirs, ndirs, k + m, &fds, &in, &size))) return rc;
-    const Matrix rows = parity_rows(enc);
-    const size_t chunk = scrub_chunk(size);
-    FilePipeline pipe(enc, rows, chunk, /*verify=*/true);
+    const Matrix rows = parity_rows(enc.get());
+    const size_t chunk = file_chunk(size);
+    FilePipeline pipe(enc.get(), rows, chunk, /*verify=*/true);
     if ((rc = pipe.start())) return rc;
-    rc = scrub_columns(pipe, in, size, chunk);
     std::vector<unsigned long long> bad(static_cast<size_t>(m), 0);
-    if (rc == SWEC_OK) rc = pipe.mismatches(bad.data());
-    const std::string msg = pipe.error_message();
-    pipe.shutdown();
-    if (rc) {
-        if (!msg.empty()) set_last_error(msg);
-        return rc;
-    }
+    if ((rc = scrub_columns(pipe, in, size, chunk)) || (rc = pipe.mismatches(bad.data()))) return rc;
     bool all_ok = true;
     for (int p = 0; p < m; p++) {
         if (mismatched_vectors) mismatched_vectors[p] = bad[size_t(p)];
@@ -805,27 +788,21 @@ int swec_locate_ec_damage(const char* base, const char* const* dirs, int ndirs, 
     if (k == 0) ec_ratio(b, &k, &m);
     int rc = check_locate_args(m, radius, report, ranges, ranges_cap);
     if (rc) return rc;
-    swec_encoder* enc = nullptr;
-    if ((rc = swec_encoder_new(k, m, device, &enc))) return rc;
-    std::unique_ptr<swec_encoder, void (*)(swec_encoder*)> guard(enc, swec_encoder_free);
+    CallEncoder enc;
+    if ((rc = new_call_encoder(k, m, device, &enc))) return rc;
     FdSet fds;
     std::vector<int> in;
     int64_t size = -1;
     if ((rc = open_all_shards(b, dirs, ndirs, k + m, &fds, &in, &size))) return rc;
-    const Matrix rows = parity_rows(enc);
-    const size_t chunk = scrub_chunk(size);
+    const Matrix rows = parity_rows(enc.get());
+    const size_t chunk = file_chunk(size);
     DamageLocator locator;
-    FilePipeline pipe(enc, rows, chunk, /*verify=*/true, &locator);
+    FilePipeline pipe(enc.get(), rows, chunk, /*verify=*/true, &locator);
     if ((rc = pipe.start())) return rc;
     rc = locator.init(rows, size, radius, enc->stream);
     if (rc == SWEC_OK) rc = scrub_columns(pipe, in, size, chunk);
     if (rc == SWEC_OK) rc = locator.collect(report, ranges, ranges_cap, n_ranges);
-    const std::string msg = pipe.error_message();
-    pipe.shutdown();
-    if (rc) {
-        if (!msg.empty()) set_last_error(msg);
-        return rc;
-    }
+    if (rc) return rc;
     *ok = report->damaged_columns == 0 ? 1 : 0;
     return SWEC_OK;
 }
@@ -835,15 +812,12 @@ int swec_write_dat_file(const char* base, int64_t dat_size, const char* const* s
     if (!base || !shard_names || k <= 0 || k > SWEC_MAX_SHARDS || large <= 0 || small <= 0 || dat_size < 0)
         return fail(SWEC_ERR_INVALID_ARG, "bad argument");
     FdSet fds;
-    const int dat = open((std::string(base) + ".dat").c_str(), O_WRONLY | O_CREAT | O_TRUNC, 0644);
+    const int dat = fds.keep(open((std::string(base) + ".dat").c_str(), O_WRONLY | O_CREAT | O_TRUNC, 0644));
     if (dat < 0) return io_fail("cannot write volume .dat");
-    fds.fds.push_back(dat);
     std::vector<int> in;
     for (int i = 0; i < k; i++) {
-        const int fd = open(shard_names[i], O_RDONLY);
-        if (fd < 0) return io_fail(std::string("open ") + shard_names[i]);
-        fds.fds.push_back(fd);
-        in.push_back(fd);
+        in.push_back(fds.keep(open(shard_names[i], O_RDONLY)));
+        if (in.back() < 0) return io_fail(std::string("open ") + shard_names[i]);
     }
     // The copy plan of the reference's two loops (ec_decoder.go:200-219) — shard s is read sequentially, the .dat is
     // written sequentially — as independent (shard offset → .dat offset) pieces, executed in parallel: every piece
@@ -873,9 +847,7 @@ int swec_write_dat_file(const char* base, int64_t dat_size, const char* const* s
         if (st.st_size < pos[size_t(s2)]) return fail(SWEC_ERR_IO, "short read copying shard " + std::to_string(s2));
     }
     if (ftruncate(dat, off_t(dat_size)) != 0) return io_fail("size .dat");
-    IoPool& pool = file_io_pool();
-    std::mutex err_mu;
-    std::string err_text;
+    FirstError first;
     const std::function<int(int)> copy_piece = [&](int idx) -> int {
         const Piece& pc = pieces[size_t(idx)];
         int64_t done = 0;
@@ -893,29 +865,19 @@ int swec_write_dat_file(const char* base, int64_t dat_size, const char* const* s
             const size_t want = size_t(std::min<int64_t>(pc.len - done, int64_t(buf.size())));
             const ssize_t got = pread(in[size_t(pc.shard)], buf.data(), want, off_t(pc.shard_off + done));
             if (got < 0 && errno == EINTR) continue;
-            if (got <= 0) {
-                std::lock_guard<std::mutex> lk(err_mu);
-                if (err_text.empty()) err_text = "short read copying shard " + std::to_string(pc.shard);
-                return SWEC_ERR_IO;
-            }
+            if (got <= 0) return first.fail(SWEC_ERR_IO, "short read copying shard " + std::to_string(pc.shard));
             ssize_t put = 0;
             while (put < got) {
                 const ssize_t w = pwrite(dat, buf.data() + put, size_t(got - put), off_t(pc.dat_off + done + put));
                 if (w < 0 && errno == EINTR) continue;
-                if (w <= 0) {
-                    std::lock_guard<std::mutex> lk(err_mu);
-                    if (err_text.empty()) err_text = std::string("write .dat: ") + strerror(errno);
-                    return SWEC_ERR_IO;
-                }
+                if (w <= 0) return first.fail(SWEC_ERR_IO, std::string("write .dat: ") + strerror(errno));
                 put += w;
             }
             done += got;
         }
         return SWEC_OK;
     };
-    const int rc = pool.parallel_for(int(pieces.size()), copy_piece);
-    if (rc) return fail(rc, err_text);
-    return SWEC_OK;
+    return file_io_pool().parallel_for(int(pieces.size()), copy_piece) ? first.get() : SWEC_OK;
 }
 
 }  // extern "C"
