@@ -533,17 +533,15 @@ class NeedleScrub {
 
     int check_alone(swec_needle_check c, size_t bytes, size_t finding) {
         StagingSlot& s = ring_.slots[cur_];  // its stream; the slot's buffers stay with the walk
-        uint8_t* d = nullptr;
         const size_t at = (bytes + 7) & ~size_t(7);
-        SWEC_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&d), at + sizeof c + needle_check_scratch_bytes(1), s.stream));
-        auto* dc = reinterpret_cast<swec_needle_check*>(d + at);
-        cudaError_t e = cudaMemcpyAsync(d, big_buf_.data(), bytes, cudaMemcpyHostToDevice, s.stream);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(dc, &c, sizeof c, cudaMemcpyHostToDevice, s.stream);
-        if (e == cudaSuccess) e = launch_needle_check(d, int64_t(bytes), version_, dc, 1, dc + 1, s.stream);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(&c, dc, sizeof c, cudaMemcpyDeviceToHost, s.stream);
-        cudaFreeAsync(d, s.stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(s.stream);
-        if (e != cudaSuccess) return cuda_fail(e, "needle check of a large record");
+        StreamScratch d(s.stream);
+        SWEC_CUDA(d.alloc(at + sizeof c + needle_check_scratch_bytes(1)));
+        auto* dc = reinterpret_cast<swec_needle_check*>(d.as<uint8_t>() + at);
+        SWEC_CUDA(cudaMemcpyAsync(d.p, big_buf_.data(), bytes, cudaMemcpyHostToDevice, s.stream));
+        SWEC_CUDA(cudaMemcpyAsync(dc, &c, sizeof c, cudaMemcpyHostToDevice, s.stream));
+        SWEC_CUDA(launch_needle_check(d.p, int64_t(bytes), version_, dc, 1, dc + 1, s.stream));
+        SWEC_CUDA(cudaMemcpyAsync(&c, dc, sizeof c, cudaMemcpyDeviceToHost, s.stream));
+        SWEC_CUDA(cudaStreamSynchronize(s.stream));
         note(c, finding);
         return SWEC_OK;
     }

@@ -1,7 +1,7 @@
-// seaweedfs_b200/csrc/engine.cc — encoder object, matrix→kernel dispatch, host staging pipeline.
+// seaweedfs_b200/csrc/engine.cc — encoder object, matrix→kernel dispatch, reconstruct plans and the C ABI.
 #include "engine.h"
 #include "damage.h"
-#include "io_pool.h"
+#include "host_seam.h"
 #include "volume_format.h"
 
 #include <algorithm>
@@ -72,22 +72,6 @@ size_t env_size(const char* name, size_t dflt) {
 std::atomic<long> g_opt_stage_chunk{long(env_size("SWEC_STAGE_CHUNK", size_t(16) << 20))};
 std::atomic<long> g_opt_stage_slots{long(env_size("SWEC_STAGE_SLOTS", 3))};
 size_t stage_slots() { return size_t(std::max(2l, g_opt_stage_slots.load())); }
-// Encoder-seam calls (swec_encode & co. on host buffers) are cut into at least this many pieces — never smaller
-// than host_min_chunk — so that the bounce copy / H2D of piece c+1, the kernel of piece c and the D2H / copy-back of
-// piece c-1 overlap INSIDE one call: the Go call sites hand over 256 KiB (encodeDataOneBatch) or 1 MiB
-// (rebuildEcFiles) per shard and wait for the result.
-std::atomic<long> g_opt_host_pieces{long(env_size("SWEC_HOST_PIECES", 4))};
-std::atomic<long> g_opt_host_min_chunk{long(env_size("SWEC_HOST_MIN_CHUNK", size_t(256) << 10))};
-// Zero-copy at the Encoder seam: the kernel reads the (mapped, pinned) host shards over PCIe itself and writes the
-// parity straight back to host memory — no staging in HBM, no DMA enqueue, one launch per piece.  What a short
-// synchronous call costs is API round trips, not bytes: 0 = never, 1 = whenever the buffers allow it,
-// 2 = auto: calls of at most host_zero_copy_max bytes per shard (bigger ones stream through the DMA ring).
-// The 2 MiB threshold was chosen on an earlier GPU generation (zero-copy ahead up to ~1-2 MiB per shard, the 4-piece
-// DMA ring from 4 MiB); not yet re-measured on the H100 (scripts/bench_host_api.py sweeps it).
-std::atomic<long> g_opt_host_zero_copy{long(env_size("SWEC_HOST_ZERO_COPY", 2))};
-std::atomic<long> g_opt_host_zero_copy_max{long(env_size("SWEC_HOST_ZERO_COPY_MAX", size_t(2) << 20))};
-std::atomic<long> g_opt_host_copy_spin_us{long(env_size("SWEC_HOST_COPY_SPIN_US", 200))};
-std::atomic<long> g_opt_host_copy_threads{long(env_size("SWEC_HOST_COPY_THREADS", 0))};  // 0 = auto
 std::atomic<long> g_opt_file_direct_io{long(env_size("SWEC_FILE_DIRECT", 0)) & 3};
 std::atomic<long> g_opt_jit_enabled{1};
 std::atomic<long> g_opt_jit_min_bytes{long(env_size("SWEC_JIT_MIN_BYTES", size_t(64) << 20))};
@@ -206,6 +190,21 @@ int swec_encoder_impl::apply(const Matrix& rows, const uint8_t* const* in, uint8
             p.row_extra = uint64_t(K - 1) * layout.block_bytes;
         }
     };
+    // the table kernels, one launch per group of at most 4 rows: over the vectors, or over the byte tail
+    auto table_groups = [&](bool byte_tail) -> int {
+        for (int r0 = 0; r0 < R; r0 += 4) {
+            const int rn = std::min(4, R - r0);
+            Matrix sub(rn, K);
+            memcpy(sub.v.data(), rows.row(r0), size_t(rn) * size_t(K));
+            DeviceTables t;
+            if (const int rc = get_tables(sub, &t, s)) return rc;
+            SwecApplyParams p;
+            fill(p, r0, rn, byte_tail ? tail_off : 0);
+            if (byte_tail) SWEC_CUDA(launch_bytes_apply(p, t.compact, K, rn, tail, s));
+            else SWEC_CUDA(launch_table_apply(p, t.replicated, K, rn, s));
+        }
+        return SWEC_OK;
+    };
 
     if (nvec) {
         SwecApplyParams p;
@@ -236,394 +235,11 @@ int swec_encoder_impl::apply(const Matrix& rows, const uint8_t* const* in, uint8
                 SWEC_CUDA(jit_launch(*jk, p, layout.blocked, s));
             } else {
                 if (layout.blocked) return fail(SWEC_ERR_INVALID_ARG, "blocked layout needs a specialised kernel");
-                for (int r0 = 0; r0 < R; r0 += 4) {
-                    const int rn = std::min(4, R - r0);
-                    Matrix sub(rn, K);
-                    for (int r = 0; r < rn; r++) memcpy(&sub.v[size_t(r) * K], rows.row(r0 + r), size_t(K));
-                    DeviceTables t;
-                    int rc = get_tables(sub, &t, s);
-                    if (rc) return rc;
-                    fill(p, r0, rn, 0);
-                    SWEC_CUDA(launch_table_apply(p, t.replicated, K, rn, s));
-                }
+                if (const int rc = table_groups(false)) return rc;
             }
         }
     }
-    if (tail) {
-        for (int r0 = 0; r0 < R; r0 += 4) {
-            const int rn = std::min(4, R - r0);
-            Matrix sub(rn, K);
-            for (int r = 0; r < rn; r++) memcpy(&sub.v[size_t(r) * K], rows.row(r0 + r), size_t(K));
-            DeviceTables t;
-            int rc = get_tables(sub, &t, s);
-            if (rc) return rc;
-            SwecApplyParams p;
-            fill(p, r0, rn, tail_off);
-            SWEC_CUDA(launch_bytes_apply(p, t.compact, K, rn, tail, s));
-        }
-    }
-    return SWEC_OK;
-}
-
-// ------------------------------------------------------------------ host staging pipeline
-// Chunks of every stream travel pinned-host → HBM → kernel → pinned-host on one of a few slots,
-// each with its own stream, so H2D of chunk c+1, the kernel of chunk c and D2H of chunk c-1
-// overlap.  Caller buffers that are already pinned (swec_alloc_pinned / cudaHostRegister) are
-// DMA'd directly; pageable ones bounce through the slot's pinned buffer.
-
-namespace {
-
-struct DeviceCounter {
-    unsigned long long* p = nullptr;
-    ~DeviceCounter() {
-        if (p) cudaFree(p);
-    }
-};
-
-// *gpu_ptr: the address the GPU uses for this memory (device memory: itself; mapped pinned host memory: its device
-// alias, the same value under unified addressing), nullptr if a kernel cannot reach it
-bool is_pinned_or_device(const void* p, bool* is_device, const void** gpu_ptr = nullptr) {
-    cudaPointerAttributes a;
-    if (gpu_ptr) *gpu_ptr = nullptr;
-    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
-        cudaGetLastError();
-        *is_device = false;
-        return false;
-    }
-    *is_device = a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
-    const bool direct = a.type == cudaMemoryTypeHost || *is_device;
-    if (gpu_ptr && direct) *gpu_ptr = a.devicePointer;
-    return direct;
-}
-
-}  // namespace
-
-// ---- bounce copies between pageable caller memory and the pinned ring run across a few threads: one core moves
-// ~10 GB/s, far less than a PCIe x16 link, so a single memcpy loop would be the whole cost of an Encoder-level call
-// from Go heap memory.
-namespace {
-
-struct CopyJob {
-    uint8_t* dst;
-    const uint8_t* src;
-    size_t len;
-};
-
-IoPool* host_pool() {  // leaked on purpose (threads must outlive static destructors); nullptr = copy inline
-    static IoPool* pool = [] () -> IoPool* {
-        long n = g_opt_host_copy_threads.load();
-        if (n <= 0) n = std::min<long>(8, std::max<long>(2, long(std::thread::hardware_concurrency()) / 8));
-        return n > 1 ? new IoPool(size_t(n - 1), unsigned(g_opt_host_copy_spin_us.load())) : nullptr;  // the caller takes a share too
-    }();
-    return pool;
-}
-
-void parallel_copy(const std::vector<CopyJob>& jobs) {
-    constexpr size_t kPiece = size_t(128) << 10, kInlineBelow = size_t(256) << 10;
-    size_t total = 0;
-    for (const CopyJob& j : jobs) total += j.len;
-    IoPool* pool = total > kInlineBelow ? host_pool() : nullptr;
-    if (!pool) {
-        for (const CopyJob& j : jobs) memcpy(j.dst, j.src, j.len);
-        return;
-    }
-    std::vector<CopyJob> pieces;
-    pieces.reserve(total / kPiece + jobs.size());
-    for (const CopyJob& j : jobs)
-        for (size_t o = 0; o < j.len; o += kPiece) pieces.push_back({j.dst + o, j.src + o, std::min(kPiece, j.len - o)});
-    const std::function<int(int)> one = [&](int i) {
-        memcpy(pieces[size_t(i)].dst, pieces[size_t(i)].src, pieces[size_t(i)].len);
-        return 0;
-    };
-    pool->parallel_for(int(pieces.size()), one);
-}
-
-// The turn both host pipelines take on the ring: the copy-backs of the piece a slot carries wait in `pending` until the
-// slot's event fires; finish(si) then runs them and frees the slot for its next piece.
-struct SlotTurns {
-    StagingRing& ring;
-    std::vector<std::vector<CopyJob>> pending;
-    explicit SlotTurns(StagingRing& r) : ring(r), pending(r.slots.size()) {}
-    int finish(size_t si) {
-        StagingSlot& s = ring.slots[si];
-        if (!s.busy) return SWEC_OK;
-        SWEC_CUDA(cudaEventSynchronize(s.done));
-        parallel_copy(pending[si]);
-        pending[si].clear();
-        s.busy = false;
-        return SWEC_OK;
-    }
-};
-
-// p[0..n) equally spaced (the k+m slices of ONE allocation, e.g. swec_alloc_pinned_for_device carved up by the caller)?
-bool constant_pitch(const uint8_t* const* p, int n, size_t min_pitch, size_t* pitch) {
-    if (n < 2) return false;
-    if (p[1] <= p[0]) return false;
-    const size_t d = size_t(p[1] - p[0]);
-    if (d < min_pitch) return false;
-    if (d > size_t(0x7fffffff)) return false;  // cudaMemcpy2D pitches are limited (cudaDevAttrMaxPitch): huge shards go one by one
-    for (int i = 2; i < n; i++)
-        if (p[i] != p[0] + size_t(i) * d) return false;
-    *pitch = d;
-    return true;
-}
-
-}  // namespace
-
-// check = nullptr: out[r] receive the results.  check != nullptr: out[r] are read and compared
-// with the computed rows; *check receives the number of mismatching 16-byte vectors.
-static int apply_host(swec_encoder_impl* e, const Matrix& rows, const uint8_t* const* in, uint8_t* const* out,
-                      size_t n, unsigned long long* check) {
-    const int K = rows.cols, R = rows.rows;
-    if (R == 0 || n == 0) return SWEC_OK;
-    std::lock_guard<std::mutex> lock(e->mu);
-    int rc = e->ensure_device();
-    if (rc) return rc;
-
-    std::vector<char> in_direct(static_cast<size_t>(K), 0), out_direct(static_cast<size_t>(R), 0);
-    const uint8_t* gin[SWEC_MAX_INPUTS];
-    uint8_t* gout[SWEC_MAX_SHARDS];
-    int ndev = 0, nreach = 0;
-    uintptr_t align = 0;
-    for (int i = 0; i < K; i++) {
-        bool dev;
-        const void* g = nullptr;
-        in_direct[size_t(i)] = is_pinned_or_device(in[i], &dev, &g);
-        gin[i] = static_cast<const uint8_t*>(g);
-        ndev += dev;
-        nreach += g != nullptr;
-        align |= reinterpret_cast<uintptr_t>(g);
-    }
-    for (int r = 0; r < R; r++) {
-        bool dev;
-        const void* g = nullptr;
-        out_direct[size_t(r)] = is_pinned_or_device(out[r], &dev, &g);
-        gout[r] = static_cast<uint8_t*>(const_cast<void*>(g));
-        ndev += dev;
-        nreach += g != nullptr;
-        align |= reinterpret_cast<uintptr_t>(g);
-    }
-    if (ndev == K + R && !check) {  // everything already lives in HBM
-        rc = e->apply(rows, in, out, n, Layout{}, e->stream);
-        if (rc) return rc;
-        SWEC_CUDA(cudaStreamSynchronize(e->stream));
-        return SWEC_OK;
-    }
-    const long zc_mode = g_opt_host_zero_copy.load();
-    const bool zero_copy = !check && (zc_mode == 1 || (zc_mode == 2 && n <= size_t(g_opt_host_zero_copy_max.load())));
-    if (zero_copy && nreach == K + R && (align & 15) == 0) {
-        // every buffer is mapped pinned (or device) memory: ONE launch reads the data shards over PCIe and writes
-        // the parity back; what a 256 KiB-per-shard Encode call costs is this launch and one stream synchronise
-        rc = e->apply(rows, gin, gout, n, Layout{}, e->stream);
-        if (rc) return rc;
-        SWEC_CUDA(cudaStreamSynchronize(e->stream));
-        return SWEC_OK;
-    }
-
-    // piece size: the call is cut into >= host_pieces pieces (>= host_min_chunk, <= stage_chunk each) travelling on
-    // the ring's slots, so that copies in, kernel and copies out of neighbouring pieces overlap inside this one call
-    const size_t max_chunk = size_t(std::max(4096l, g_opt_stage_chunk.load()));
-    const size_t min_chunk = std::min(max_chunk, size_t(std::max(4096l, g_opt_host_min_chunk.load())));
-    const size_t pieces = size_t(std::max(1l, g_opt_host_pieces.load()));
-    size_t chunk = (((n + pieces - 1) / pieces) + 4095) & ~size_t(4095);
-    chunk = std::min(max_chunk, std::max(min_chunk, chunk));
-    chunk = std::min(chunk, (n + 255) & ~size_t(255));
-    rc = e->ensure_slots(chunk);
-    if (rc) return rc;
-    const size_t stride = e->slot_chunk();  // per-stream pitch inside a slot (>= chunk)
-    StagingRing& ring = e->ring;
-
-    StagingRing::DrainOnExit drain{ring};
-    DeviceCounter counter;
-    if (check) {
-        SWEC_CUDA(cudaMalloc(reinterpret_cast<void**>(&counter.p), 8));
-        SWEC_CUDA(cudaMemset(counter.p, 0, 8));
-    }
-    unsigned long long* const dev_bad = counter.p;
-
-    SlotTurns turns(ring);
-
-    bool all_in_bounced = true, all_out_bounced = !check, all_in_direct = true, all_out_direct = !check;
-    for (int i = 0; i < K; i++) {
-        all_in_bounced = all_in_bounced && !in_direct[size_t(i)];
-        all_in_direct = all_in_direct && in_direct[size_t(i)];
-    }
-    for (int r = 0; r < R; r++) {
-        all_out_bounced = all_out_bounced && !out_direct[size_t(r)];
-        all_out_direct = all_out_direct && out_direct[size_t(r)];
-    }
-    // pinned callers whose k+m buffers are slices of one allocation: ONE strided DMA each way instead of k + m
-    size_t in_pitch = 0, out_pitch = 0;
-    const bool in_2d = all_in_direct && constant_pitch(in, K, n, &in_pitch);
-    const bool out_2d = all_out_direct && R > 1 && constant_pitch(out, R, n, &out_pitch);
-    const bool packed = all_in_bounced && all_out_bounced;
-
-    std::vector<CopyJob> bounce;
-    size_t ci = 0;
-    for (size_t off = 0; off < n; off += chunk, ci++) {
-        const size_t si = ci % ring.slots.size();
-        StagingSlot& s = ring.slots[si];
-        if ((rc = turns.finish(si))) break;
-        const size_t len = std::min(chunk, n - off);
-        // Pageable callers (Go heap memory) bounce through the slot anyway, so pack the streams at a
-        // pitch that fits this piece: one DMA in, one DMA out instead of k + m small ones.
-        const size_t pitch = packed ? ((len + 255) & ~size_t(255)) : stride;
-        const uint8_t* din[SWEC_MAX_INPUTS];
-        uint8_t* dout[SWEC_MAX_SHARDS];
-        bounce.clear();
-        for (int i = 0; i < K; i++) {
-            din[i] = s.dev + size_t(i) * pitch;
-            if (!in_direct[size_t(i)]) bounce.push_back({s.host + size_t(i) * pitch, in[i] + off, len});
-        }
-        parallel_copy(bounce);
-        if (packed && zero_copy && s.host_dev) {
-            // pageable caller, short call: the kernel works on the mapped ring itself (reads and writes cross PCIe
-            // inside the kernel), so a piece costs one launch instead of H2D + launch + D2H
-            for (int i = 0; i < K; i++) din[i] = s.host_dev + size_t(i) * pitch;
-            for (int r = 0; r < R; r++) dout[r] = s.host_dev + size_t(K + r) * pitch;
-            if ((rc = e->apply(rows, din, dout, len, Layout{}, s.stream))) break;
-            for (int r = 0; r < R; r++) turns.pending[si].push_back({out[r] + off, s.host + size_t(K + r) * pitch, len});
-            SWEC_CUDA(cudaEventRecord(s.done, s.stream));
-            s.busy = true;
-            continue;
-        }
-        if (packed) {
-            SWEC_CUDA(cudaMemcpyAsync(s.dev, s.host, size_t(K - 1) * pitch + len, cudaMemcpyHostToDevice, s.stream));
-        } else if (in_2d) {
-            SWEC_CUDA(cudaMemcpy2DAsync(s.dev, pitch, in[0] + off, in_pitch, len, size_t(K), cudaMemcpyDefault, s.stream));
-        } else {
-            for (int i = 0; i < K; i++) {
-                const uint8_t* src = in_direct[size_t(i)] ? in[i] + off : s.host + size_t(i) * pitch;
-                SWEC_CUDA(cudaMemcpyAsync(s.dev + size_t(i) * pitch, src, len, cudaMemcpyDefault, s.stream));
-            }
-        }
-        for (int r = 0; r < R; r++) dout[r] = s.dev + size_t(K + r) * pitch;
-        if ((rc = e->apply(rows, din, dout, len, Layout{}, s.stream))) break;
-        if (packed) {
-            SWEC_CUDA(cudaMemcpyAsync(s.host + size_t(K) * pitch, dout[0], size_t(R - 1) * pitch + len,
-                                      cudaMemcpyDeviceToHost, s.stream));
-            for (int r = 0; r < R; r++) turns.pending[si].push_back({out[r] + off, s.host + size_t(K + r) * pitch, len});
-        } else if (out_2d) {
-            SWEC_CUDA(cudaMemcpy2DAsync(out[0] + off, out_pitch, dout[0], pitch, len, size_t(R), cudaMemcpyDefault, s.stream));
-        } else {
-            if (check) {  // bring the caller's copy of every row next to the computed one and compare in HBM
-                bounce.clear();
-                for (int r = 0; r < R; r++)
-                    if (!out_direct[size_t(r)]) bounce.push_back({s.host + size_t(K + r) * stride, out[r] + off, len});
-                parallel_copy(bounce);
-            }
-            for (int r = 0; r < R; r++) {
-                if (check) {
-                    uint8_t* theirs = s.dev + size_t(K + R + r) * stride;
-                    const uint8_t* src = out_direct[size_t(r)] ? out[r] + off : s.host + size_t(K + r) * stride;
-                    SWEC_CUDA(cudaMemcpyAsync(theirs, src, len, cudaMemcpyDefault, s.stream));
-                    SWEC_CUDA(launch_compare(dout[r], theirs, len, dev_bad, s.stream));
-                } else if (out_direct[size_t(r)]) {
-                    SWEC_CUDA(cudaMemcpyAsync(out[r] + off, dout[r], len, cudaMemcpyDefault, s.stream));
-                } else {
-                    uint8_t* back = s.host + size_t(K + r) * stride;
-                    SWEC_CUDA(cudaMemcpyAsync(back, dout[r], len, cudaMemcpyDeviceToHost, s.stream));
-                    turns.pending[si].push_back({out[r] + off, back, len});
-                }
-            }
-        }
-        SWEC_CUDA(cudaEventRecord(s.done, s.stream));
-        s.busy = true;
-    }
-    for (size_t i = 0; i < ring.slots.size(); i++) {
-        // drain in submission order so that copy-backs of early pieces overlap the GPU work of late ones
-        const int rc2 = turns.finish((ci + i) % ring.slots.size());
-        if (!rc) rc = rc2;
-    }
-    if (check && !rc && cudaMemcpy(check, dev_bad, 8, cudaMemcpyDeviceToHost) != cudaSuccess)
-        rc = cuda_fail(cudaGetLastError(), "reading the mismatch counter");
-    return rc;
-}
-
-// Largest interval the packed path takes (bigger ones stream through apply_host): small on purpose — the
-// ring behind it is 3 slots x (k+2m) streams x this, and needle-sized intervals gain nothing from more.
-static size_t packed_max_bytes() {
-    return std::min(size_t(std::max(4096l, g_opt_stage_chunk.load())), size_t(2) << 20);
-}
-
-// Many small intervals that share one matrix (degraded reads behind one dead server): pack them
-// back to back (each padded to 16 bytes) into slot-sized launches so the per-call costs — stream
-// round trip, launch, DMA set-up — are paid once per ~chunk instead of once per needle.
-struct Segment {
-    std::vector<const uint8_t*> in;  // K pointers
-    std::vector<uint8_t*> out;       // R pointers
-    size_t len;
-};
-
-static int apply_host_packed(swec_encoder_impl* e, const Matrix& rows, const std::vector<Segment>& segs) {
-    const int K = rows.cols, R = rows.rows;
-    if (R == 0 || segs.empty()) return SWEC_OK;
-    std::lock_guard<std::mutex> lock(e->mu);
-    int rc = e->ensure_device();
-    if (rc) return rc;
-    // size the ring for THIS batch (a lone degraded read must not pin 3 x 18 x 16 MiB): everything packed
-    // back to back, capped by the configured chunk; ensure_slots only ever grows an existing ring
-    const size_t max_chunk = packed_max_bytes();
-    size_t packed = 0;
-    for (const Segment& sg : segs) packed += (sg.len + 15) & ~size_t(15);
-    const size_t chunk = std::min(max_chunk, (packed + 65535) & ~size_t(65535));
-    if ((rc = e->ensure_slots(chunk))) return rc;
-    const size_t stride = e->slot_chunk();
-    StagingRing& ring = e->ring;
-    StagingRing::DrainOnExit drain{ring};
-    SlotTurns turns(ring);
-    size_t si = 0, fill = 0, nflush = 0;
-    auto flush = [&]() -> int {
-        if (fill == 0) return SWEC_OK;
-        StagingSlot& sl = ring.slots[si];
-        const uint8_t* din[SWEC_MAX_INPUTS];
-        uint8_t* dout[SWEC_MAX_SHARDS];
-        const long zc_mode = g_opt_host_zero_copy.load();
-        // zero-copy pays for one needle per call and costs when many needles fill slot after slot (earlier GPU
-        // generation; scripts/bench_needles.py measures it) — full slots keep the strided-DMA pipeline
-        const size_t packed_zero_copy_max = std::min(size_t(g_opt_host_zero_copy_max.load()), size_t(256) << 10);
-        if (sl.host_dev && (zc_mode == 1 || (zc_mode == 2 && fill <= packed_zero_copy_max))) {
-            // needle-sized batches: the kernel works on the mapped ring itself — one launch instead of
-            // strided DMA in + launch + strided DMA out (what a degraded read waits for is API round trips)
-            for (int i = 0; i < K; i++) din[i] = sl.host_dev + size_t(i) * stride;
-            for (int r = 0; r < R; r++) dout[r] = sl.host_dev + size_t(K + r) * stride;
-            const int rc2 = e->apply(rows, din, dout, fill, Layout{}, sl.stream);
-            if (rc2) return rc2;
-        } else {
-            for (int i = 0; i < K; i++) din[i] = sl.dev + size_t(i) * stride;
-            // the K input streams sit at pitch `stride` in both buffers: one strided DMA instead of K small ones
-            SWEC_CUDA(cudaMemcpy2DAsync(sl.dev, stride, sl.host, stride, fill, size_t(K), cudaMemcpyHostToDevice, sl.stream));
-            for (int r = 0; r < R; r++) dout[r] = sl.dev + size_t(K + r) * stride;
-            const int rc2 = e->apply(rows, din, dout, fill, Layout{}, sl.stream);
-            if (rc2) return rc2;
-            SWEC_CUDA(cudaMemcpy2DAsync(sl.host + size_t(K) * stride, stride, dout[0], stride, fill, size_t(R),
-                                        cudaMemcpyDeviceToHost, sl.stream));
-        }
-        SWEC_CUDA(cudaEventRecord(sl.done, sl.stream));
-        sl.busy = true;
-        fill = 0;
-        si = (++nflush) % ring.slots.size();
-        return turns.finish(si);  // the slot we are about to fill must be drained
-    };
-    for (const Segment& sg : segs) {
-        const size_t padded = (sg.len + 15) & ~size_t(15);
-        if (padded > stride) {  // larger than a slot: not a "small interval" — caller should not batch it
-            return fail(SWEC_ERR_INVALID_ARG, "batched interval larger than the staging chunk");
-        }
-        if (fill + padded > stride && (rc = flush())) return rc;
-        StagingSlot& sl = ring.slots[si];
-        for (int i = 0; i < K; i++) {
-            uint8_t* dst = sl.host + size_t(i) * stride + fill;
-            memcpy(dst, sg.in[i], sg.len);
-            if (padded > sg.len) memset(dst + sg.len, 0, padded - sg.len);
-        }
-        for (int r = 0; r < R; r++) turns.pending[si].push_back({sg.out[r], sl.host + size_t(K + r) * stride + fill, sg.len});
-        fill += padded;
-    }
-    if ((rc = flush())) return rc;
-    for (size_t i = 0; i < ring.slots.size(); i++)
-        if ((rc = turns.finish(i))) return rc;
-    return SWEC_OK;
+    return tail ? table_groups(true) : SWEC_OK;
 }
 
 Matrix parity_rows(const swec_encoder_impl* e) {
@@ -1090,17 +706,11 @@ int swec_encode_volume_device(swec_encoder* e, const void* dat_v, int64_t dat_si
     if (g.large_rows && (rc = region(dat, large, g.large_rows, 0))) return rc;
     if (g.small_rows && (rc = region(dat + g.small_dat_offset(), small, g.small_rows, g.small_shard_offset()))) return rc;
     if (g.tail > 0) {  // last row: bytes past EOF read as zero (ec_encoder.go:258-262)
-        struct Scratch {  // stream-ordered: freed after the work queued on s, on every exit path
-            uint8_t* p = nullptr;
-            cudaStream_t s;
-            ~Scratch() {
-                if (p) cudaFreeAsync(p, s);
-            }
-        } scratch{nullptr, s};
-        SWEC_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&scratch.p), size_t(g.small_row()), s));
-        SWEC_CUDA(cudaMemsetAsync(scratch.p, 0, size_t(g.small_row()), s));
-        SWEC_CUDA(cudaMemcpyAsync(scratch.p, dat + g.tail_dat_offset(), size_t(g.tail), cudaMemcpyDeviceToDevice, s));
-        rc = region(scratch.p, small, 1, g.tail_shard_offset());
+        StreamScratch row(s);
+        SWEC_CUDA(row.alloc(size_t(g.small_row())));
+        SWEC_CUDA(cudaMemsetAsync(row.p, 0, size_t(g.small_row()), s));
+        SWEC_CUDA(cudaMemcpyAsync(row.p, dat + g.tail_dat_offset(), size_t(g.tail), cudaMemcpyDeviceToDevice, s));
+        rc = region(row.as<uint8_t>(), small, 1, g.tail_shard_offset());
         if (rc) return rc;
     }
     return SWEC_OK;
@@ -1179,14 +789,8 @@ int swec_locate_damage_device(swec_encoder* e, const void* const* shards, size_t
     if ((rc = locator.init(rows, int64_t(n), radius, s))) return rc;
     // the computed parity goes to scratch a piece at a time: a 3 GiB shard set needs 1 GiB of it, not 12 GiB
     const size_t piece = std::min(n, size_t(256) << 20);
-    struct Scratch {  // stream-ordered: freed after the work queued on s, on every exit path
-        uint8_t* p = nullptr;
-        cudaStream_t s;
-        ~Scratch() {
-            if (p) cudaFreeAsync(p, s);
-        }
-    } scratch{nullptr, s};
-    if (piece) SWEC_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&scratch.p), size_t(m) * piece, s));
+    StreamScratch scratch(s);
+    if (piece) SWEC_CUDA(scratch.alloc(size_t(m) * piece));
     for (size_t off = 0; off < n; off += piece) {
         const size_t len = std::min(piece, n - off);
         const uint8_t* in[SWEC_MAX_SHARDS];
@@ -1194,7 +798,7 @@ int swec_locate_damage_device(swec_encoder* e, const void* const* shards, size_t
         uint8_t* comp[SWEC_MAX_SHARDS];
         for (int i = 0; i < k; i++) in[i] = sh[i] + off;
         for (int p = 0; p < m; p++) {
-            comp[p] = scratch.p + size_t(p) * piece;
+            comp[p] = scratch.as<uint8_t>() + size_t(p) * piece;
             stored[p] = sh[k + p] + off;
         }
         if ((rc = e->apply(rows, in, comp, len, Layout{}, s))) return rc;
@@ -1236,12 +840,10 @@ int swec_digest_device(int device, const void* src, size_t bytes, uint64_t* dige
     if (!src || !digest) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
     SWEC_CUDA(cudaSetDevice(device));
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    u64* d = nullptr;
-    SWEC_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&d), 8, s));
-    cudaError_t e = launch_digest(src, bytes, d, s);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(digest, d, 8, cudaMemcpyDeviceToHost, s);
-    cudaFreeAsync(d, s);
-    if (e != cudaSuccess) return cuda_fail(e, "digest");
+    StreamScratch d(s);
+    SWEC_CUDA(d.alloc(8));
+    SWEC_CUDA(launch_digest(src, bytes, d.as<u64>(), s));
+    SWEC_CUDA(cudaMemcpyAsync(digest, d.p, 8, cudaMemcpyDeviceToHost, s));
     SWEC_CUDA(cudaStreamSynchronize(s));
     return SWEC_OK;
 }

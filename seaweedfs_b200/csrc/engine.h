@@ -35,6 +35,18 @@ int cuda_fail(cudaError_t e, const char* what);
 
 size_t env_size(const char* name, size_t dflt);  // a positive integer from the environment, else dflt
 size_t stage_slots();  // "stage_slots" (SWEC_STAGE_SLOTS): slots of every staging ring, at least 2
+extern std::atomic<long> g_opt_stage_chunk;  // "stage_chunk" (SWEC_STAGE_CHUNK): largest piece per stream of a host call
+
+// Device scratch in stream order: cudaMallocAsync on `s`, and freed after the work queued on s, on every exit path.
+struct StreamScratch {
+    void* p = nullptr;
+    cudaStream_t s;
+    explicit StreamScratch(cudaStream_t stream) : s(stream) {}
+    StreamScratch(const StreamScratch&) = delete;
+    ~StreamScratch() { if (p) cudaFreeAsync(p, s); }
+    cudaError_t alloc(size_t bytes) { return cudaMallocAsync(&p, bytes, s); }
+    template <class T> T* as() const { return static_cast<T*>(p); }
+};
 
 // "file_direct_io" (SWEC_FILE_DIRECT): bit 0 = O_DIRECT reads of the .dat / shard inputs straight into the pinned
 // ring, bit 1 = O_DIRECT writes of the shard outputs — the page cache is bypassed both ways (disk-backed volumes only;

@@ -1,6 +1,6 @@
 // seaweedfs_b200/csrc/io_pool.h — a small blocking fork-join pool for host-side work that the GPU cannot do:
 // the k preads / k+m pwrites of a stripe in the file pipeline (ec_files.cc) and the bounce copies between
-// pageable caller memory and the pinned staging ring at the Encoder seam (engine.cc apply_host).  No GF arithmetic
+// pageable caller memory and the pinned staging ring at the Encoder seam (host_seam.cc).  No GF arithmetic
 // ever runs here.  tests/test_iopool.py compiles this class on its own under ThreadSanitizer and AddressSanitizer.
 #pragma once
 #include <algorithm>

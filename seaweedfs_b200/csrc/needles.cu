@@ -311,14 +311,12 @@ extern "C" int swec_check_needles_device(int device, const void* dat, int64_t da
     SWEC_CUDA(cudaSetDevice(device));
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     const size_t table_bytes = size_t(n) * sizeof(swec_needle_check);
-    uint8_t* buf = nullptr;
-    SWEC_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&buf), table_bytes + needle_check_scratch_bytes(n), s));
-    auto* dev_checks = reinterpret_cast<swec_needle_check*>(buf);
-    cudaError_t e = cudaMemcpyAsync(dev_checks, checks, table_bytes, cudaMemcpyHostToDevice, s);
-    if (e == cudaSuccess) e = launch_needle_check(dat, dat_size, needle_version, dev_checks, n, buf + table_bytes, s);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(checks, dev_checks, table_bytes, cudaMemcpyDeviceToHost, s);
-    cudaFreeAsync(buf, s);
-    if (e != cudaSuccess) return cuda_fail(e, "needle check");
+    StreamScratch buf(s);
+    SWEC_CUDA(buf.alloc(table_bytes + needle_check_scratch_bytes(n)));
+    auto* dev_checks = buf.as<swec_needle_check>();
+    SWEC_CUDA(cudaMemcpyAsync(dev_checks, checks, table_bytes, cudaMemcpyHostToDevice, s));
+    SWEC_CUDA(launch_needle_check(dat, dat_size, needle_version, dev_checks, n, buf.as<uint8_t>() + table_bytes, s));
+    SWEC_CUDA(cudaMemcpyAsync(checks, dev_checks, table_bytes, cudaMemcpyDeviceToHost, s));
     SWEC_CUDA(cudaStreamSynchronize(s));
     return SWEC_OK;
 }

@@ -1,5 +1,5 @@
 // seaweedfs_b200/csrc/staging.h — pinned host memory near the GPU, and the staging ring host data travels through on
-// its way to the kernels and back: the Encoder seam (engine.cc) and the file pipelines (ec_files.cc) each use one.
+// its way to the kernels and back: the Encoder seam (host_seam.cc) and the file pipelines (ec_files.cc) each use one.
 #pragma once
 #include <cuda_runtime.h>
 

@@ -40,6 +40,18 @@ def _ptrs(arrs) -> C.Array:
     return out
 
 
+def _fill_missing(shards: list, n: int, data_shards: int, data_only: bool, need_data_shards: bool = True):
+    """The presence mask of a reconstruct call's shards, with the shards it rebuilds put in place as new zeroed
+    arrays, and the pointer list it takes (NULL for a shard that stays missing)."""
+    present = np.array([s is not None and len(s) > 0 for s in shards], dtype=np.uint8)
+    if need_data_shards and present.sum() < data_shards:
+        raise SwecError(-2, "too few shards given (ErrTooFewShards)")
+    for i in range(len(shards)):
+        if not present[i] and (i < data_shards or not data_only):
+            shards[i] = np.zeros(n, dtype=np.uint8)
+    return present, _ptrs([s if s is not None and len(s) else None for s in shards])
+
+
 class Encoder:
     """reedsolomon.Encoder backed by the GPU engine (swec_encoder)."""
 
@@ -103,14 +115,8 @@ class Encoder:
     def reconstruct(self, shards: list, data_only: bool = False) -> None:
         """Reconstruct(shards): None / empty entries are missing and are replaced by new arrays."""
         n = self._check_shards(shards, allow_missing=True)
-        present = np.array([s is not None and len(s) > 0 for s in shards], dtype=np.uint8)
-        if present.sum() < self.data_shards:
-            raise SwecError(-2, "too few shards given (ErrTooFewShards)")
-        for i in range(self.total_shards):
-            if not present[i] and (i < self.data_shards or not data_only):
-                shards[i] = np.zeros(n, dtype=np.uint8)
-        bufs = [s if s is not None and len(s) else None for s in shards]
-        check(lib().swec_reconstruct(self._h, _ptrs(bufs), present.ctypes.data, n, int(data_only)))
+        present, ptrs = _fill_missing(shards, n, self.data_shards, data_only)
+        check(lib().swec_reconstruct(self._h, ptrs, present.ctypes.data, n, int(data_only)))
 
     def reconstruct_data(self, shards: list) -> None:
         self.reconstruct(shards, data_only=True)
@@ -122,11 +128,7 @@ class Encoder:
         keep = []
         for j, shards in enumerate(batch):
             n = self._check_shards(shards, allow_missing=True)
-            present = np.array([s is not None and len(s) > 0 for s in shards], dtype=np.uint8)
-            for i in range(self.total_shards):
-                if not present[i] and (i < self.data_shards or not data_only):
-                    shards[i] = np.zeros(n, dtype=np.uint8)
-            ptrs = _ptrs([s if s is not None and len(s) else None for s in shards])
+            present, ptrs = _fill_missing(shards, n, self.data_shards, data_only, need_data_shards=False)
             keep.append((ptrs, present))
             items[j].shards = C.cast(ptrs, C.POINTER(C.c_void_p))
             items[j].present = present.ctypes.data_as(C.POINTER(C.c_uint8))
@@ -215,15 +217,8 @@ class EncoderGroup:
     def reconstruct(self, shards: list, data_only: bool = False) -> None:
         e0 = self.encoders[0]
         n = e0._check_shards(shards, allow_missing=True)
-        present = np.array([s is not None and len(s) > 0 for s in shards], dtype=np.uint8)
-        if present.sum() < self.data_shards:
-            raise SwecError(-2, "too few shards given (ErrTooFewShards)")
-        for i in range(self.total_shards):
-            if not present[i] and (i < self.data_shards or not data_only):
-                shards[i] = np.zeros(n, dtype=np.uint8)
-        bufs = [s if s is not None and len(s) else None for s in shards]
-        check(lib().swec_reconstruct_multi(self._arr, len(self.encoders), _ptrs(bufs), present.ctypes.data, n,
-                                           int(data_only)))
+        present, ptrs = _fill_missing(shards, n, self.data_shards, data_only)
+        check(lib().swec_reconstruct_multi(self._arr, len(self.encoders), ptrs, present.ctypes.data, n, int(data_only)))
 
     Encode, Reconstruct = encode, reconstruct
 
