@@ -19,6 +19,7 @@
  *   swec_rebuild_ec_files       RebuildEcFiles / generateMissingEcFiles   ec_encoder.go:74-104,146-200
  *   swec_verify_ec_files        (Rust twin) verify_ec_shards   seaweed-volume/src/storage/erasure_coding/ec_encoder.rs:177-278
  *   swec_locate_ec_damage       what verify_ec_shards cannot tell (ec_encoder.rs:240-258): WHICH shard is wrong
+ *   swec_repair_ec_damage       (no counterpart) corrects the located bytes in place instead of rebuilding whole shards
  *   swec_reconstruct_batch      batched ReconstructData   weed/storage/store_ec.go:482-560 (one call per interval today)
  *   swec_write_dat_file         WriteDatFile              weed/storage/erasure_coding/ec_decoder.go:176-223
  *   swec_ec_shards_generate     VolumeEcShardsGenerate (file work)   weed/server/volume_grpc_erasure_coding.go:43-146
@@ -222,8 +223,9 @@ int swec_verify_ec_files(const char *base_file_name, const char *const *addition
  *   - more than t but at most m-t wrong shards: the column is counted as uncorrectable and no shard is blamed;
  *   - more than m-t wrong shards: the column may be blamed on the wrong shards.  That is the limit of the code.
  * For RS(10,4), radius 1 (the default) is always right, or says uncorrectable, for up to 3 damaged shards per column;
- * radius 2 locates overlapping damage in 2 shards but may misattribute 3.  The remedy for a blamed shard is to delete
- * its file and run swec_rebuild_ec_files.  The reference cannot do this: verify_ec_shards
+ * radius 2 locates overlapping damage in 2 shards but may misattribute 3.  swec_repair_ec_damage (below) corrects the
+ * located bytes in place; where it leaves uncorrectable columns, or a shard file is missing, the remedy is to delete the
+ * blamed shard files and run swec_rebuild_ec_files.  The reference cannot do this: verify_ec_shards
  * (seaweed-volume/src/storage/erasure_coding/ec_encoder.rs:240-258) marks every mismatching PARITY shard as broken, so
  * one damaged data shard gets all m parity shards reported (and rebuilding those bakes the damage in), and the Go scrub
  * never checks parity (ec_volume_scrub.go:25).                                                                        */
@@ -256,6 +258,33 @@ int swec_locate_ec_damage(const char *base_file_name, const char *const *additio
 int swec_locate_damage_device(swec_encoder *enc, const void *const *shards, size_t shard_len, int radius,
                               swec_damage_report *report, swec_damage_range *ranges, int ranges_cap,
                               int *n_ranges, void *stream);
+/* ---- repair in place: the locate calls, which also write the corrections --------------------------------------------
+ * Same arguments, argument rules and report as the locate calls; the report is the one they return for the same input
+ * before the call, so shard_bytes[i] = the bytes corrected in shard i.
+ *   - In every column where at most `radius` shards are blamed, the blamed bytes are replaced by the decoded values, and
+ *     the column is a codeword again.  Uncorrectable columns are left byte for byte as they were.
+ *   - The guarantee above carries over unchanged, and so does its limit: a column with more than m-t wrong shards can be
+ *     MISCORRECTED, that is rewritten into a different codeword.  For RS(10,4), radius 1 never miscorrects a column
+ *     with up to 3 wrong shards; radius 2 can miscorrect a column with 3 or more.  Radius 1 is the default of every
+ *     binding; take radius 2 only for damage known to overlap in at most 2 shards.
+ *   - A clean set is never written to, so a second call on a repaired set reports damaged_columns == 0.
+ * File level: pass 1 is swec_locate_ec_damage (same shard lookup, ratio rule, errors and kernel launches), and a set
+ * without damage is left there, never opened for writing.  A missing shard is SWEC_ERR_TOO_FEW_SHARDS (rebuild first)
+ * and unequal lengths SWEC_ERR_SHARD_SIZE, both before any device work and before anything is opened for writing.
+ * Pass 2 reads again only the 4 KiB pages pass 1 flagged, corrects them on the GPU, and pwrites each blamed shard's own
+ * flagged pages back to the file where the shard was found (base directory or an additional dir), with O_DIRECT when
+ * "file_direct_io" bit 1 is set; every modified file is fdatasync'ed before the call returns.  *ok = 1 iff no
+ * uncorrectable column remains.  As for rebuild, nobody else may write the shard files during the call.  Each byte is
+ * written once, old or corrected, so a repair cut short by a crash leaves every column as it was, corrected, or (at
+ * radius 2) corrected in one of its two shards, which is still within the radius: running the call again finishes it.
+ * Device level: the shards in HBM are corrected the same way, each 256 MiB piece after its parity was recomputed, in
+ * stream order; synchronises `stream`.                                                                               */
+int swec_repair_ec_damage(const char *base_file_name, const char *const *additional_dirs, int n_additional_dirs,
+                          int data_shards, int parity_shards, int device, int radius, swec_damage_report *report,
+                          swec_damage_range *ranges, int ranges_cap, int *n_ranges, int *ok);
+int swec_correct_damage_device(swec_encoder *enc, void *const *shards, size_t shard_len, int radius,
+                               swec_damage_report *report, swec_damage_range *ranges, int ranges_cap,
+                               int *n_ranges, void *stream);
 int swec_write_dat_file(const char *base_file_name, int64_t dat_file_size,
                         const char *const *shard_file_names, int data_shards,
                         int64_t large_block, int64_t small_block);

@@ -446,6 +446,43 @@ func swecLocateEcDamage(baseFileName string, ctx *ECContext, additionalDirs []st
 	return broken, details, nil
 }
 
+// swecRepairEcDamage is swecLocateEcDamage, which also corrects the located bytes in the shard files: only the damaged
+// pages of the damaged shards are rewritten, so scattered bit rot in more than ParityShards shards is still repaired,
+// where deleting and rebuilding that many shards is impossible.  repaired are the shards written; details say where.
+// Fall back to delete-and-rebuild in two cases: details report uncorrectable columns (more wrong shards in a column
+// than radius 1 corrects; those columns are left as they were), or a shard file is missing (the call fails with
+// SWEC_ERR_TOO_FEW_SHARDS: rebuild first, then repair).  Radius 1 never miscorrects a column with up to ParityShards-1
+// wrong shards.  Nobody else may write the shard files during the call.
+func swecRepairEcDamage(baseFileName string, ctx *ECContext, additionalDirs []string) (repaired []uint32, details []string, err error) {
+	cs := C.CString(baseFileName)
+	defer C.free(unsafe.Pointer(cs))
+	dirs := make([]*C.char, len(additionalDirs)+1)
+	for i, d := range additionalDirs {
+		dirs[i] = C.CString(d)
+		defer C.free(unsafe.Pointer(dirs[i]))
+	}
+	var report C.swec_damage_report
+	var nRanges, ok C.int
+	if err := swecCall(func() C.int {
+		return C.swec_repair_ec_damage(cs, (**C.char)(unsafe.Pointer(&dirs[0])), C.int(len(additionalDirs)),
+			C.int(ctx.DataShards), C.int(ctx.ParityShards), swecPickDevice(), 1, &report, nil, 0, &nRanges, &ok)
+	}); err != nil {
+		return nil, nil, fmt.Errorf("repair ec damage: %w", err)
+	}
+	for i := 0; i < ctx.DataShards+ctx.ParityShards; i++ {
+		if n := uint64(report.shard_bytes[i]); n > 0 {
+			repaired = append(repaired, uint32(i))
+			details = append(details, fmt.Sprintf("ec shard %d: %d bytes corrected, offsets %d..%d",
+				i, n, int64(report.shard_first[i]), int64(report.shard_last[i])))
+		}
+	}
+	if report.uncorrectable_columns > 0 {
+		details = append(details, fmt.Sprintf("%d byte columns are damaged in more shards than can be corrected, offsets %d..%d",
+			uint64(report.uncorrectable_columns), int64(report.first_uncorrectable), int64(report.last_uncorrectable)))
+	}
+	return repaired, details, nil
+}
+
 // ---- pinned batch buffers ---------------------------------------------------------------------------------
 // runtime.Pinner only stops the Go GC from moving a slice; to CUDA such memory is PAGEABLE, so every Encode /
 // Reconstruct on it bounces through the library's pinned ring (a memcpy per shard each way).  The batch buffers of

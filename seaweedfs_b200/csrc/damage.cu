@@ -16,6 +16,9 @@
 //                        Per-lane runs (set, count, first, last) merge the columns a lane blames on one shard, and a
 //                        warp merges equal runs with __match_any_sync / __reduce_*_sync before one set of atomics.
 //                        Bytes after the last whole vector, and unaligned streams, go through a byte loop.
+//                        The correcting instantiation (CORRECT) also XORs each blamed shard's error value into that
+//                        shard's byte of the column, which makes the column a codeword again; it reads stored parity
+//                        with coherent loads, because it writes it.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -53,6 +56,7 @@ struct LocateParams {
     unsigned long long* ctr;
     u32* pages;
     u64 page_words;
+    u8* fix[SWEC_MAX_SHARDS];  // correcting kernel: the k+m shards' bytes of these columns (fix[k+p] == stored[p])
 };
 
 struct Run {  // columns one lane blamed on one set, in increasing offset order
@@ -111,9 +115,10 @@ __device__ __forceinline__ void record(const LocateParams& p, Run* run, int set,
 
 __device__ __forceinline__ u8 gmul(const LocateTables& t, int log_c, u8 v) { return v ? t.exp[log_c + t.log[v]] : 0; }
 
-// rows other than `skip` of s (logs in L, all non-zero) are one multiple of column j of P
-__device__ __forceinline__ bool multiple_of_column(const LocateTables& t, const u8* L, int m, int j, int skip) {
-    int r = -1;
+// rows other than `skip` of s (logs in L, all non-zero) are one multiple of column j of P; r is the log of that
+// multiple, the error value of data shard j
+__device__ __forceinline__ bool multiple_of_column(const LocateTables& t, const u8* L, int m, int j, int skip, int& r) {
+    r = -1;
     for (int i = 0; i < m; i++) {
         if (i == skip) continue;
         int d = int(L[i]) - int(t.logp[i * 32 + j]);
@@ -125,7 +130,9 @@ __device__ __forceinline__ bool multiple_of_column(const LocateTables& t, const 
 }
 
 // Shards that explain the non-zero syndrome s within the radius, ascending in *a, *b; returns how many (0: none does).
-__device__ int decode_column(const LocateTables& t, const u8* s, int k, int m, int radius, int* a, int* b) {
+// CORRECT: also their error values in *ea, *eb, the bytes that XORed into the shards turn the column into a codeword.
+template <bool CORRECT>
+__device__ int decode_column(const LocateTables& t, const u8* s, int k, int m, int radius, int* a, int* b, u8* ea, u8* eb) {
     u8 L[SWEC_MAX_SHARDS];
     u32 nz = 0;
     for (int i = 0; i < m; i++) {
@@ -135,29 +142,43 @@ __device__ int decode_column(const LocateTables& t, const u8* s, int k, int m, i
     const int w = __popc(nz);
     if (w == 1) {
         *a = k + __ffs(nz) - 1;
+        if (CORRECT) *ea = s[*a - k];
         return 1;
     }
     if (w == m)  // every entry of an MDS P is non-zero
-        for (int j = 0; j < k; j++)
-            if (multiple_of_column(t, L, m, j, -1)) {
+        for (int j = 0; j < k; j++) {
+            int r;
+            if (multiple_of_column(t, L, m, j, -1, r)) {
                 *a = j;
+                if (CORRECT) *ea = t.exp[r];
                 return 1;
             }
+        }
     if (radius < 2) return 0;
     if (w == 2) {
         *a = k + __ffs(nz) - 1;
         *b = k + __ffs(nz & (nz - 1)) - 1;
+        if (CORRECT) {
+            *ea = s[*a - k];
+            *eb = s[*b - k];
+        }
         return 2;
     }
     if (w < m - 1) return 0;  // a data shard in the pattern makes at least m-1 components non-zero
     for (int q = 0; q < m; q++) {
         if (w == m - 1 && ((nz >> q) & 1)) continue;  // the zero component can only be the parity shard's
-        for (int j = 0; j < k; j++)
-            if (multiple_of_column(t, L, m, j, q)) {
+        for (int j = 0; j < k; j++) {
+            int r;
+            if (multiple_of_column(t, L, m, j, q, r)) {
                 *a = j;
                 *b = k + q;
+                if (CORRECT) {  // s_q = P[q][j]·e_j ^ e_q
+                    *ea = t.exp[r];
+                    *eb = s[q] ^ t.exp[r + t.logp[q * 32 + j]];
+                }
                 return 2;
             }
+        }
     }
     for (int x = 0; x + 1 < k; x++)
         for (int y = x + 1; y < k; y++) {
@@ -174,21 +195,40 @@ __device__ int decode_column(const LocateTables& t, const u8* s, int k, int m, i
             if (ok) {
                 *a = x;
                 *b = y;
+                if (CORRECT) {
+                    *ea = t.exp[lx];
+                    *eb = t.exp[ly];
+                }
                 return 2;
             }
         }
     return 0;
 }
 
-__device__ __forceinline__ void blame(const LocateParams& p, const LocateTables& t, const u8* s, int m, u64 off, Run* run) {
+// column x of the launch (shard offset p.base + x); the correcting kernel XORs the error values into the shards
+template <bool CORRECT>
+__device__ __forceinline__ void blame(const LocateParams& p, const LocateTables& t, const u8* s, int m, u64 x, Run* run) {
     int a = -1, b = -1;
-    const int found = decode_column(t, s, p.k, m, p.radius, &a, &b);
+    u8 ea = 0, eb = 0;
+    const u64 off = p.base + x;
+    const int found = decode_column<CORRECT>(t, s, p.k, m, p.radius, &a, &b, &ea, &eb);
     if (!found) {
         record(p, run, p.k + m, off);
         return;
     }
     record(p, run, a, off);
-    if (found == 2) record(p, run, b, off);
+    if (CORRECT) p.fix[a][x] ^= ea;
+    if (found == 2) {
+        record(p, run, b, off);
+        if (CORRECT) p.fix[b][x] ^= eb;
+    }
+}
+
+// Stored parity is read through the non-coherent path only by the kernel that does not write it.
+template <bool CORRECT>
+__device__ __forceinline__ uint4 load_stored(const u8* p) {
+    if (CORRECT) return *reinterpret_cast<const uint4*>(p);
+    return swec_ldg_stream(p);
 }
 
 __device__ __forceinline__ u8 byte_of(const uint4& x, int c) {
@@ -200,7 +240,9 @@ __device__ __forceinline__ uint4 xor4(const uint4& a, const uint4& b) {
     return make_uint4(a.x ^ b.x, a.y ^ b.y, a.z ^ b.z, a.w ^ b.w);
 }
 
-template <int MT>  // MT > 0: m known at compile time; 0: run-time m
+// MT > 0: m known at compile time; 0: run-time m.  CORRECT: fix every column decoded within the radius in place.  A
+// column's bytes are read and written only by the thread that owns its vector (or its byte in the tail loop).
+template <int MT, bool CORRECT>
 __global__ void __launch_bounds__(256) swec_locate_kernel(const __grid_constant__ LocateParams p) {
     __shared__ __align__(16) u32 words[kTableWords];
     for (int i = threadIdx.x; i < kTableWords; i += blockDim.x) words[i] = p.tables[i];
@@ -224,7 +266,7 @@ __global__ void __launch_bounds__(256) swec_locate_kernel(const __grid_constant_
 #pragma unroll
             for (int i = 0; i < kMaxM; i++) {
                 if (MT == 0 && i >= m) break;
-                const uint4 d = xor4(swec_ldg_stream(p.comp[i] + (v << 4)), swec_ldg_stream(p.stored[i] + (v << 4)));
+                const uint4 d = xor4(swec_ldg_stream(p.comp[i] + (v << 4)), load_stored<CORRECT>(p.stored[i] + (v << 4)));
                 diff |= d.x | d.y | d.z | d.w;
             }
         }
@@ -232,8 +274,10 @@ __global__ void __launch_bounds__(256) swec_locate_kernel(const __grid_constant_
         u32 damaged = 0;
         if (diff) {
             uint4 x[kMaxM];
-            for (int i = 0; i < m; i++) x[i] = xor4(__ldg(reinterpret_cast<const uint4*>(p.comp[i]) + v),
-                                                    __ldg(reinterpret_cast<const uint4*>(p.stored[i]) + v));
+            for (int i = 0; i < m; i++)
+                x[i] = xor4(__ldg(reinterpret_cast<const uint4*>(p.comp[i]) + v),
+                            CORRECT ? reinterpret_cast<const uint4*>(p.stored[i])[v]
+                                    : __ldg(reinterpret_cast<const uint4*>(p.stored[i]) + v));
             for (int c = 0; c < 16; c++) {
                 u8 s[kMaxM];
                 u8 any = 0;
@@ -243,7 +287,7 @@ __global__ void __launch_bounds__(256) swec_locate_kernel(const __grid_constant_
                 }
                 if (!any) continue;
                 damaged++;
-                blame(p, t, s, m, p.base + (v << 4) + u64(c), run);
+                blame<CORRECT>(p, t, s, m, (v << 4) + u64(c), run);
             }
         }
         const u64 wbase = p.base + (vb << 4);
@@ -262,16 +306,17 @@ __global__ void __launch_bounds__(256) swec_locate_kernel(const __grid_constant_
         }
         if (!any) continue;
         atomicAdd(p.ctr + 3 * kSets, 1ull);
-        blame(p, t, s, m, p.base + x, run);
+        blame<CORRECT>(p, t, s, m, x, run);
         flush_plain(p, run[0]);
         flush_plain(p, run[1]);
     }
 }
 
-template <int MT>
+template <int MT, bool CORRECT>
 unsigned locate_grid(u64 n) {
     static int per_sm = 0;  // resident CTAs per SM, the same on every device of this architecture
-    if (!per_sm && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, swec_locate_kernel<MT>, 256, 0) != cudaSuccess) {
+    if (!per_sm &&
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, swec_locate_kernel<MT, CORRECT>, 256, 0) != cudaSuccess) {
         cudaGetLastError();
         per_sm = 4;
     }
@@ -302,10 +347,11 @@ DamageLocator::~DamageLocator() {
     if (pages_) cudaFree(pages_);
 }
 
-int DamageLocator::init(const Matrix& parity, int64_t shard_len, int radius, cudaStream_t s) {
+int DamageLocator::init(const Matrix& parity, int64_t shard_len, int radius, cudaStream_t s, bool correct) {
     k_ = parity.cols;
     m_ = parity.rows;
     radius_ = radius;
+    correct_ = correct;
     shard_len_ = shard_len;
     LocateTables t;
     memset(&t, 0, sizeof t);
@@ -338,15 +384,17 @@ int DamageLocator::init(const Matrix& parity, int64_t shard_len, int radius, cud
     return SWEC_OK;
 }
 
-int DamageLocator::launch(const uint8_t* const* computed, const uint8_t* const* stored, size_t n, int64_t base,
+int DamageLocator::launch(const uint8_t* const* computed, uint8_t* const* shards, size_t n, int64_t base,
                           cudaStream_t s) {
     if (n == 0) return SWEC_OK;
     LocateParams p;
     memset(&p, 0, sizeof p);
     for (int i = 0; i < m_; i++) {
         p.comp[i] = computed[i];
-        p.stored[i] = stored[i];
+        p.stored[i] = shards[k_ + i];
     }
+    if (correct_)
+        for (int i = 0; i < k_ + m_; i++) p.fix[i] = shards[i];
     p.n = n;
     p.base = u64(base);
     p.k = k_;
@@ -356,14 +404,20 @@ int DamageLocator::launch(const uint8_t* const* computed, const uint8_t* const* 
     p.ctr = counters_;
     p.pages = pages_;
     p.page_words = page_words_;
-    if (m_ == 4) swec_locate_kernel<4><<<locate_grid<4>(n), 256, 0, s>>>(p);
-    else swec_locate_kernel<0><<<locate_grid<0>(n), 256, 0, s>>>(p);
+    if (correct_) {
+        if (m_ == 4) swec_locate_kernel<4, true><<<locate_grid<4, true>(n), 256, 0, s>>>(p);
+        else swec_locate_kernel<0, true><<<locate_grid<0, true>(n), 256, 0, s>>>(p);
+    } else {
+        if (m_ == 4) swec_locate_kernel<4, false><<<locate_grid<4, false>(n), 256, 0, s>>>(p);
+        else swec_locate_kernel<0, false><<<locate_grid<0, false>(n), 256, 0, s>>>(p);
+    }
     g_kernel_launches++;
     SWEC_CUDA(cudaGetLastError());
     return SWEC_OK;
 }
 
-int DamageLocator::collect(swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges) {
+int DamageLocator::collect(swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges,
+                           std::vector<swec_damage_range>* all) {
     const int n = k_ + m_;
     std::vector<unsigned long long> c(kCounters);
     std::vector<uint32_t> bits(size_t(n + 1) * page_words_);
@@ -384,6 +438,7 @@ int DamageLocator::collect(swec_damage_report* report, swec_damage_range* ranges
     // maximal runs of flagged pages: shards in ascending id, then the uncorrectable columns
     const int64_t pages = (shard_len_ + (int64_t(1) << kPageShift) - 1) >> kPageShift;
     int total = 0;
+    if (all) all->clear();
     for (int set = 0; set <= n; set++) {
         const uint32_t* w = bits.data() + size_t(set) * page_words_;
         auto flagged = [&](int64_t pg) { return (w[pg >> 5] >> (pg & 31)) & 1u; };
@@ -398,13 +453,13 @@ int DamageLocator::collect(swec_damage_report* report, swec_damage_range* ranges
             }
             int64_t end = pg + 1;
             while (end < pages && flagged(end)) end++;
-            if (total < ranges_cap) {
-                swec_damage_range& r = ranges[total];
-                r.shard_id = set < n ? set : -1;
-                r.reserved = 0;
-                r.offset = pg << kPageShift;
-                r.length = std::min(end << kPageShift, shard_len_) - r.offset;
-            }
+            swec_damage_range r;
+            r.shard_id = set < n ? set : -1;
+            r.reserved = 0;
+            r.offset = pg << kPageShift;
+            r.length = std::min(end << kPageShift, shard_len_) - r.offset;
+            if (total < ranges_cap) ranges[total] = r;
+            if (all) all->push_back(r);
             total++;
             pg = end;
         }

@@ -104,7 +104,8 @@ struct FdSet {
 // fill bytes [dst_off, dst_off+len) of the slot's stream `stream` from fd@off (zero past EOF)
 // dfd: the same file opened O_DIRECT (-1 = none): used when offset, length and buffer are all 4 KiB aligned
 struct ReadOp { int stream, fd; int64_t off; size_t dst_off, len; int dfd = -1; };
-struct WriteOp { int stream, fd; int64_t off; int dfd = -1; };  // drain stream `stream` of the slot to fd@off
+// drain bytes [src_off, src_off+len) of the slot's stream `stream` to fd@off
+struct WriteOp { int stream, fd; int64_t off; size_t src_off, len; int dfd = -1; };
 struct Item {
     size_t len = 0;
     int64_t shard_off = 0;  // shard offset of the item's first column
@@ -200,7 +201,8 @@ class FilePipeline {
     PipeStats stats;
     // verify = true: streams [K, K+R) are the parity bytes read from disk; the computed parity goes to
     // streams [K+R, K+2R) and is only compared on the device (no D2H, no writes) — counted per parity stream, or,
-    // with a locator, decoded into the shards it blames.
+    // with a locator, decoded into the shards it blames.  A correcting locator also fixes those shards in the slot,
+    // and the streams the item writes come back to be written.
     FilePipeline(swec_encoder* enc, const Matrix& rows, size_t chunk, bool verify = false, DamageLocator* locator = nullptr)
         : enc_(enc), rows_(rows), chunk_(chunk), verify_(verify), locator_(locator) {}
     ~FilePipeline() { shutdown(); }
@@ -310,9 +312,17 @@ class FilePipeline {
         }
         if (rc) return set_error(rc, s);
         if (locator_) {
-            const uint8_t* stored[SWEC_MAX_SHARDS];
-            for (int r = 0; r < R; r++) stored[r] = b.dev + size_t(K + r) * chunk_;
-            if ((rc = locator_->launch(dout, stored, len, item.shard_off, b.stream))) return set_error(rc, s);
+            uint8_t* shards[SWEC_MAX_SHARDS];
+            for (int i = 0; i < K + R; i++) shards[i] = b.dev + size_t(i) * chunk_;
+            if ((rc = locator_->launch(dout, shards, len, item.shard_off, b.stream))) return set_error(rc, s);
+            // corrected shards that are written back: their streams come back whole, once each
+            uint64_t back = 0;
+            for (const WriteOp& w : item.writes) {
+                if ((back >> w.stream) & 1) continue;
+                back |= uint64_t(1) << w.stream;
+                if (e == cudaSuccess)
+                    e = cudaMemcpyAsync(b.host + size_t(w.stream) * chunk_, shards[w.stream], len, cudaMemcpyDeviceToHost, b.stream);
+            }
         } else if (verify_) {
             for (int r = 0; r < R && e == cudaSuccess; r++)
                 e = launch_compare(dout[r], b.dev + size_t(K + r) * chunk_, len, dev_bad_ + r, b.stream);
@@ -426,12 +436,12 @@ class FilePipeline {
                 // file would only queue behind each other (SWEC_FILE_WRITE_PIECE splits them anyway, for O_DIRECT devices)
                 const size_t wpiece = std::max<size_t>(4096, env_size("SWEC_FILE_WRITE_PIECE", s->item.len ? s->item.len : 4096) & ~size_t(4095));
                 for (size_t i = 0; i < s->item.writes.size(); i++)
-                    for (size_t o = 0; o < s->item.len; o += wpiece)
-                        wpieces.push_back({int(i), o, std::min(wpiece, s->item.len - o)});
+                    for (size_t o = 0; o < s->item.writes[i].len; o += wpiece)
+                        wpieces.push_back({int(i), o, std::min(wpiece, s->item.writes[i].len - o)});
                 const std::function<int(int)> write_one = [&](int idx) -> int {
                     const Piece& pc = wpieces[size_t(idx)];
                     const WriteOp& w = s->item.writes[size_t(pc.op)];
-                    const uint8_t* src = s->buf->host + size_t(w.stream) * chunk_ + pc.off;
+                    const uint8_t* src = s->buf->host + size_t(w.stream) * chunk_ + w.src_off + pc.off;
                     const int64_t off = w.off + int64_t(pc.off);
                     size_t put = 0;
                     while (put < pc.len) {
@@ -557,6 +567,108 @@ int scrub_columns(FilePipeline& pipe, const std::vector<int>& in, int64_t size, 
     return pipe.finish();
 }
 
+// Pass 2 of swec_repair_ec_damage.  `runs` are every page run pass 1 found, of the blamed shards and of the
+// uncorrectable columns.  Only the columns of those pages go through the pipeline again, with a correcting locator, and
+// the report and ranges are collected from that.  Each blamed shard gets back only its own pages, in the file where it
+// was found, made durable before the call returns.
+int repair_pages(swec_encoder* enc, const Matrix& rows, const std::string& b, const char* const* dirs, int ndirs,
+                 const std::vector<int>& in, int64_t size, int radius, const std::vector<swec_damage_range>& runs,
+                 swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges) {
+    const int total = int(in.size());
+    // each shard's slice of `runs`, which lists them shard by shard in ascending offset; an empty one: not blamed
+    std::vector<size_t> next(static_cast<size_t>(total), 0), stop(static_cast<size_t>(total), 0);
+    for (size_t r = runs.size(); r-- > 0;)
+        if (runs[r].shard_id >= 0) {
+            const size_t id = size_t(runs[r].shard_id);
+            if (!stop[id]) stop[id] = r + 1;
+            next[id] = r;
+        }
+    FdSet fds;
+    const long direct = g_opt_file_direct_io.load();
+    std::vector<int> in_d(static_cast<size_t>(total), -1), out(static_cast<size_t>(total), -1),
+        out_d(static_cast<size_t>(total), -1);
+    for (int i = 0; i < total; i++) {
+        const std::string path = find_shard_file(b, dirs, ndirs, i);
+        in_d[size_t(i)] = fds.keep(open_direct(path, O_RDONLY, direct & 1));
+        if (!stop[size_t(i)]) continue;
+        if ((out[size_t(i)] = fds.keep(open(path.c_str(), O_RDWR))) < 0) return io_fail("open " + path);
+        out_d[size_t(i)] = fds.keep(open_direct(path, O_RDWR, direct & 2));
+    }
+    // the union of the runs, as maximal spans [begin, end)
+    std::vector<std::pair<int64_t, int64_t>> spans;
+    for (const swec_damage_range& r : runs) spans.push_back({r.offset, r.offset + r.length});
+    std::sort(spans.begin(), spans.end());
+    size_t nspans = 0;
+    for (const auto& sp : spans) {
+        if (nspans && sp.first <= spans[nspans - 1].second) spans[nspans - 1].second = std::max(spans[nspans - 1].second, sp.second);
+        else spans[nspans++] = sp;
+    }
+    spans.resize(nspans);
+
+    const size_t chunk = file_chunk(size);
+    DamageLocator locator;
+    FilePipeline pipe(enc, rows, chunk, /*verify=*/true, &locator);
+    int rc = pipe.start();
+    if (rc) return rc;
+    if ((rc = locator.init(rows, size, radius, enc->stream, /*correct=*/true))) return rc;
+    for (size_t sp = 0; rc == SWEC_OK && sp < spans.size(); sp++)
+        for (int64_t o = spans[sp].first; rc == SWEC_OK && o < spans[sp].second; o += int64_t(chunk)) {
+            Item it;
+            it.len = size_t(std::min<int64_t>(int64_t(chunk), spans[sp].second - o));
+            it.shard_off = o;
+            const int64_t end = o + int64_t(it.len);
+            for (int i = 0; i < total; i++) {
+                it.reads.push_back({i, in[size_t(i)], o, 0, it.len, in_d[size_t(i)]});
+                for (size_t& r = next[size_t(i)]; r < stop[size_t(i)]; r++) {  // shard i's own pages in the item
+                    const int64_t lo = std::max(runs[r].offset, o), hi = std::min(runs[r].offset + runs[r].length, end);
+                    if (lo >= end) break;
+                    it.writes.push_back({i, out[size_t(i)], lo, size_t(lo - o), size_t(hi - lo), out_d[size_t(i)]});
+                    if (hi < runs[r].offset + runs[r].length) break;  // the run goes on in the next item
+                }
+            }
+            rc = pipe.submit(std::move(it));
+        }
+    if ((rc = pipe.finish())) return rc;
+    for (int i = 0; i < total; i++)
+        if (out[size_t(i)] >= 0 && fdatasync(out[size_t(i)]) != 0) return io_fail("fdatasync " + b + shard_ext(i));
+    return locator.collect(report, ranges, ranges_cap, n_ranges);
+}
+
+// swec_locate_ec_damage, and with `repair` swec_repair_ec_damage, whose pass 1 is the locate call itself: a set without
+// damage is never opened for writing.
+int damage_files(const char* base, const char* const* dirs, int ndirs, int k, int m, int device, int radius, bool repair,
+                 swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges, int* ok) {
+    if (!base || !ok || (ndirs > 0 && !dirs)) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
+    *ok = 0;
+    const std::string b(base);
+    if (k == 0) ec_ratio(b, &k, &m);
+    int rc = check_locate_args(m, radius, report, ranges, ranges_cap);
+    if (rc) return rc;
+    CallEncoder enc;
+    if ((rc = new_call_encoder(k, m, device, &enc))) return rc;
+    FdSet fds;
+    std::vector<int> in;
+    int64_t size = -1;
+    if ((rc = open_all_shards(b, dirs, ndirs, k + m, &fds, &in, &size))) return rc;
+    const Matrix rows = parity_rows(enc.get());
+    std::vector<swec_damage_range> runs;
+    {
+        const size_t chunk = file_chunk(size);
+        DamageLocator locator;
+        FilePipeline pipe(enc.get(), rows, chunk, /*verify=*/true, &locator);
+        if ((rc = pipe.start())) return rc;
+        rc = locator.init(rows, size, radius, enc->stream);
+        if (rc == SWEC_OK) rc = scrub_columns(pipe, in, size, chunk);
+        if (rc == SWEC_OK) rc = locator.collect(report, ranges, ranges_cap, n_ranges, repair ? &runs : nullptr);
+        if (rc) return rc;
+    }  // the pipeline parks its staging ring for pass 2
+    if (repair && report->damaged_columns &&
+        (rc = repair_pages(enc.get(), rows, b, dirs, ndirs, in, size, radius, runs, report, ranges, ranges_cap, n_ranges)))
+        return rc;
+    *ok = (repair ? report->uncorrectable_columns : report->damaged_columns) == 0 ? 1 : 0;
+    return SWEC_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -620,7 +732,7 @@ int swec_generate_ec_files(const char* base, int64_t buffer_size, int64_t large,
             Item it;
             it.len = size_t(std::min<int64_t>(int64_t(chunk), block - o));
             for (int i = 0; i < k; i++) it.reads.push_back({i, dat, processed + block * i + o, 0, it.len, dat_d});
-            for (int i = 0; i < total; i++) it.writes.push_back({i, outs[size_t(i)], shard_off + o, outs_d[size_t(i)]});
+            for (int i = 0; i < total; i++) it.writes.push_back({i, outs[size_t(i)], shard_off + o, 0, it.len, outs_d[size_t(i)]});
             const int r = pipe.submit(std::move(it));
             if (r) return r;
         }
@@ -645,7 +757,7 @@ int swec_generate_ec_files(const char* base, int64_t buffer_size, int64_t large,
         for (int64_t j = 0; j < n; j++)
             for (int i = 0; i < k; i++)
                 it.reads.push_back({i, dat, processed + j * g.small_row() + int64_t(i) * small, size_t(j * small), size_t(small), dat_d});
-        for (int i = 0; i < total; i++) it.writes.push_back({i, outs[size_t(i)], shard_off, outs_d[size_t(i)]});
+        for (int i = 0; i < total; i++) it.writes.push_back({i, outs[size_t(i)], shard_off, 0, it.len, outs_d[size_t(i)]});
         rc = pipe.submit(std::move(it));
         shard_off += n * small;
         processed += n * g.small_row();
@@ -743,7 +855,7 @@ int swec_rebuild_ec_files(const char* base, const char* const* dirs, int ndirs, 
         Item it;
         it.len = size_t(std::min<int64_t>(int64_t(chunk), todo - o));
         for (int i = 0; i < k; i++) it.reads.push_back({i, in[size_t(ins[size_t(i)])], o, 0, it.len, in_d[size_t(ins[size_t(i)])]});
-        for (size_t r = 0; r < out.size(); r++) it.writes.push_back({k + int(r), out[r], o, out_d[r]});
+        for (size_t r = 0; r < out.size(); r++) it.writes.push_back({k + int(r), out[r], o, 0, it.len, out_d[r]});
         rc = pipe.submit(std::move(it));
     }
     if ((rc = pipe.finish())) return rc;
@@ -782,29 +894,12 @@ int swec_verify_ec_files(const char* base, const char* const* dirs, int ndirs, i
 
 int swec_locate_ec_damage(const char* base, const char* const* dirs, int ndirs, int k, int m, int device, int radius,
                           swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges, int* ok) {
-    if (!base || !ok || (ndirs > 0 && !dirs)) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
-    *ok = 0;
-    const std::string b(base);
-    if (k == 0) ec_ratio(b, &k, &m);
-    int rc = check_locate_args(m, radius, report, ranges, ranges_cap);
-    if (rc) return rc;
-    CallEncoder enc;
-    if ((rc = new_call_encoder(k, m, device, &enc))) return rc;
-    FdSet fds;
-    std::vector<int> in;
-    int64_t size = -1;
-    if ((rc = open_all_shards(b, dirs, ndirs, k + m, &fds, &in, &size))) return rc;
-    const Matrix rows = parity_rows(enc.get());
-    const size_t chunk = file_chunk(size);
-    DamageLocator locator;
-    FilePipeline pipe(enc.get(), rows, chunk, /*verify=*/true, &locator);
-    if ((rc = pipe.start())) return rc;
-    rc = locator.init(rows, size, radius, enc->stream);
-    if (rc == SWEC_OK) rc = scrub_columns(pipe, in, size, chunk);
-    if (rc == SWEC_OK) rc = locator.collect(report, ranges, ranges_cap, n_ranges);
-    if (rc) return rc;
-    *ok = report->damaged_columns == 0 ? 1 : 0;
-    return SWEC_OK;
+    return damage_files(base, dirs, ndirs, k, m, device, radius, false, report, ranges, ranges_cap, n_ranges, ok);
+}
+
+int swec_repair_ec_damage(const char* base, const char* const* dirs, int ndirs, int k, int m, int device, int radius,
+                          swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges, int* ok) {
+    return damage_files(base, dirs, ndirs, k, m, device, radius, true, report, ranges, ranges_cap, n_ranges, ok);
 }
 
 int swec_write_dat_file(const char* base, int64_t dat_size, const char* const* shard_names, int k, int64_t large,

@@ -772,40 +772,58 @@ int swec_write_dat_device(swec_encoder* e, const void* const* data_shards, int64
     return SWEC_OK;
 }
 
-int swec_locate_damage_device(swec_encoder* e, const void* const* shards, size_t n, int radius, swec_damage_report* report,
-                              swec_damage_range* ranges, int ranges_cap, int* n_ranges, void* stream) {
+}  // extern "C"
+
+namespace {
+
+// swec_locate_damage_device, and with `correct` swec_correct_damage_device: the shards are written only then.
+int damage_device(swec_encoder* e, const void* const* shards, size_t n, int radius, bool correct,
+                  swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges, void* stream) {
     if (!e || !shards) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
     int rc = check_locate_args(e->m, radius, report, ranges, ranges_cap);
     if (rc) return rc;
     const int k = e->k, m = e->m;
     for (int i = 0; i < k + m; i++)
         if (!shards[i]) return fail(SWEC_ERR_INVALID_ARG, "NULL shard");
-    const uint8_t* const* sh = reinterpret_cast<const uint8_t* const*>(shards);
+    uint8_t* const* sh = reinterpret_cast<uint8_t* const*>(const_cast<void* const*>(shards));
     std::lock_guard<std::mutex> lock(e->mu);
     if ((rc = e->ensure_device())) return rc;
     cudaStream_t s = pick_stream(e, stream);
     const Matrix rows = parity_rows(e);
     DamageLocator locator;
-    if ((rc = locator.init(rows, int64_t(n), radius, s))) return rc;
-    // the computed parity goes to scratch a piece at a time: a 3 GiB shard set needs 1 GiB of it, not 12 GiB
+    if ((rc = locator.init(rows, int64_t(n), radius, s, correct))) return rc;
+    // The computed parity goes to scratch a piece at a time: a 3 GiB shard set needs 1 GiB of it, not 12 GiB.  A data
+    // byte corrected in a piece has already been encoded, and no later piece reads it.
     const size_t piece = std::min(n, size_t(256) << 20);
     StreamScratch scratch(s);
     if (piece) SWEC_CUDA(scratch.alloc(size_t(m) * piece));
     for (size_t off = 0; off < n; off += piece) {
         const size_t len = std::min(piece, n - off);
         const uint8_t* in[SWEC_MAX_SHARDS];
-        const uint8_t* stored[SWEC_MAX_SHARDS];
+        uint8_t* at[SWEC_MAX_SHARDS];
         uint8_t* comp[SWEC_MAX_SHARDS];
-        for (int i = 0; i < k; i++) in[i] = sh[i] + off;
-        for (int p = 0; p < m; p++) {
-            comp[p] = scratch.as<uint8_t>() + size_t(p) * piece;
-            stored[p] = sh[k + p] + off;
-        }
+        for (int i = 0; i < k + m; i++) at[i] = sh[i] + off;
+        for (int i = 0; i < k; i++) in[i] = at[i];
+        for (int p = 0; p < m; p++) comp[p] = scratch.as<uint8_t>() + size_t(p) * piece;
         if ((rc = e->apply(rows, in, comp, len, Layout{}, s))) return rc;
-        if ((rc = locator.launch(comp, stored, len, int64_t(off), s))) return rc;
+        if ((rc = locator.launch(comp, at, len, int64_t(off), s))) return rc;
     }
     SWEC_CUDA(cudaStreamSynchronize(s));
     return locator.collect(report, ranges, ranges_cap, n_ranges);
+}
+
+}  // namespace
+
+extern "C" {
+
+int swec_locate_damage_device(swec_encoder* e, const void* const* shards, size_t n, int radius, swec_damage_report* report,
+                              swec_damage_range* ranges, int ranges_cap, int* n_ranges, void* stream) {
+    return damage_device(e, shards, n, radius, false, report, ranges, ranges_cap, n_ranges, stream);
+}
+
+int swec_correct_damage_device(swec_encoder* e, void* const* shards, size_t n, int radius, swec_damage_report* report,
+                               swec_damage_range* ranges, int ranges_cap, int* n_ranges, void* stream) {
+    return damage_device(e, shards, n, radius, true, report, ranges, ranges_cap, n_ranges, stream);
 }
 
 int swec_stream_synchronize(swec_encoder* e, void* stream) {

@@ -185,6 +185,16 @@ class Encoder:
                                               max_ranges, C.byref(n), stream))
         return _damage_result(report, ranges, n.value, max_ranges)
 
+    def correct_damage_device(self, shard_ptrs, shard_len: int, radius: int = 1, max_ranges: int = 4096,
+                              stream: int = 0) -> dict:
+        """locate_damage_device, which also corrects the located bytes in place (swec_correct_damage_device).  Returns
+        the report of the shards as they were; uncorrectable columns are left as they were.  Radius 2 can miscorrect a
+        column with 3 or more wrong shards (include/swec.h)."""
+        report, ranges, n = DamageReport(), (DamageRange * max(1, max_ranges))(), C.c_int(0)
+        check(lib().swec_correct_damage_device(self._h, _ptrs(shard_ptrs), shard_len, radius, C.byref(report), ranges,
+                                               max_ranges, C.byref(n), stream))
+        return _damage_result(report, ranges, n.value, max_ranges)
+
     def synchronize(self, stream: int = 0) -> None:
         check(lib().swec_stream_synchronize(self._h, stream))
 
@@ -310,6 +320,19 @@ def locate_ec_damage(base_file_name: str, additional_dirs: list[str] | None = No
     k, m, dev = (ctx.DataShards, ctx.ParityShards, ctx.device) if ctx else (0, 0, device)
     report, ranges, n, ok = DamageReport(), (DamageRange * max(1, max_ranges))(), C.c_int(0), C.c_int(0)
     check(lib().swec_locate_ec_damage(base_file_name.encode(), arr, nd, k, m, dev, radius, C.byref(report), ranges,
+                                      max_ranges, C.byref(n), C.byref(ok)))
+    return {"ok": bool(ok.value), **_damage_result(report, ranges, n.value, max_ranges)}
+
+
+def repair_ec_damage(base_file_name: str, additional_dirs: list[str] | None = None, ctx: ECContext | None = None,
+                     device: int = 0, radius: int = 1, max_ranges: int = 4096) -> dict:
+    """locate_ec_damage, which also corrects the located bytes in the shard files (swec_repair_ec_damage): only the
+    blamed shards' damaged pages are rewritten.  Returns the report of the files as they were; "ok" is True iff no
+    uncorrectable column remains.  Radius 2 can miscorrect a column with 3 or more wrong shards (include/swec.h)."""
+    arr, nd = _dirs(additional_dirs)
+    k, m, dev = (ctx.DataShards, ctx.ParityShards, ctx.device) if ctx else (0, 0, device)
+    report, ranges, n, ok = DamageReport(), (DamageRange * max(1, max_ranges))(), C.c_int(0), C.c_int(0)
+    check(lib().swec_repair_ec_damage(base_file_name.encode(), arr, nd, k, m, dev, radius, C.byref(report), ranges,
                                       max_ranges, C.byref(n), C.byref(ok)))
     return {"ok": bool(ok.value), **_damage_result(report, ranges, n.value, max_ranges)}
 
