@@ -20,6 +20,8 @@
  *   swec_verify_ec_files        (Rust twin) verify_ec_shards   seaweed-volume/src/storage/erasure_coding/ec_encoder.rs:177-278
  *   swec_locate_ec_damage       what verify_ec_shards cannot tell (ec_encoder.rs:240-258): WHICH shard is wrong
  *   swec_repair_ec_damage       (no counterpart) corrects the located bytes in place instead of rebuilding whole shards
+ *   swec_rebuild_ec_files_checked  rebuildEcFiles reading every present shard (ec_encoder.go:342-357), which corrects
+ *                               damage in the shards it rebuilds from instead of copying it into the rebuilt ones
  *   swec_reconstruct_batch      batched ReconstructData   weed/storage/store_ec.go:482-560 (one call per interval today)
  *   swec_write_dat_file         WriteDatFile              weed/storage/erasure_coding/ec_decoder.go:176-223
  *   swec_ec_shards_generate     VolumeEcShardsGenerate (file work)   weed/server/volume_grpc_erasure_coding.go:43-146
@@ -285,6 +287,43 @@ int swec_repair_ec_damage(const char *base_file_name, const char *const *additio
 int swec_correct_damage_device(swec_encoder *enc, void *const *shards, size_t shard_len, int radius,
                                swec_damage_report *report, swec_damage_range *ranges, int ranges_cap,
                                int *n_ranges, void *stream);
+/* ---- checked rebuild: errors and erasures ---------------------------------------------------------------------------
+ * swec_rebuild_ec_files reads only the first k present shards, so a wrong byte in one of them goes into every shard it
+ * rebuilds.  The checked rebuild reads every present shard.  The first k present shards are the information set; the
+ * other c = m - f present shards (f = missing shards) are its check shards, re-encoded and compared, and the damage the
+ * syndrome locates in the information set is taken out of the rebuilt bytes.  The present shards form a code of
+ * distance c+1, and the radius used is t = min(radius, floor(c/2)); radius may be 0, 1 or 2.  Per column:
+ *   - at most t wrong present shards: exactly those shards are blamed, and the rebuilt bytes are the true ones;
+ *   - t+1 .. c-t wrong present shards: the column is counted as uncorrectable, nothing is blamed, and its rebuilt bytes
+ *     are exactly what swec_rebuild_ec_files writes;
+ *   - more than c-t wrong present shards: the blame and the rebuilt bytes can both be wrong.  That includes a column in
+ *     which only check shards are wrong, which plain rebuild would have rebuilt right;
+ *   - radius 0 (detect only): a column with 1 .. c wrong present shards is always counted as uncorrectable and rebuilt
+ *     exactly as plain rebuild does.  Take it when no guess is wanted, notably when c is 2 or 3.
+ * For RS(10,4) at radius 1: with 1 shard lost (c = 3), 1 wrong present shard is corrected and 2 are reported; with 2
+ * lost (c = 2), 1 is corrected and 2 can be wrong (radius 0 reports them instead); with 3 lost (c = 1), 1 is reported;
+ * with 4 lost nothing can be checked.  With nothing lost (c = m) the report is the one of swec_locate_ec_damage.
+ * Present shards are never written, neither the files nor the device buffers.  To fix them, run swec_repair_ec_damage
+ * (or swec_correct_damage_device) on the completed set afterwards: with every rebuilt column right, a column with one
+ * damaged present shard is within radius 1 of the full code.
+ * The report and ranges are those of the locate calls, over the present shards (a missing shard is never blamed);
+ * with c = 0 the report has columns = 0 and no ranges.  Argument rules: report not NULL, ranges_cap not negative,
+ * ranges not NULL when ranges_cap > 0, radius 0, 1 or 2 (SWEC_ERR_INVALID_ARG otherwise, before anything else).
+ * File level: the arguments, ratio rule, shard lookup, errors and texts of swec_rebuild_ec_files, in its order (too few
+ * shards before any output exists; the outputs created, then the lengths compared; on any failure no ids and no
+ * output file left).  rebuilt[] receives the rebuilt ids (none when nothing is missing; then nothing is written).  The
+ * rebuilt files are written even where uncorrectable columns remain; the ranges say where.  *ok = 1 iff c >= 1 and no
+ * column is uncorrectable.
+ * Device level: the argument rules of swec_reconstruct_device (a shard to rebuild needs a buffer, fewer than k present
+ * is SWEC_ERR_TOO_FEW_SHARDS) plus the ones above.  The check shards are re-encoded into scratch of at most 256 MiB per
+ * shard at a time; synchronises `stream`.                                                                             */
+int swec_rebuild_ec_files_checked(const char *base_file_name, const char *const *additional_dirs, int n_additional_dirs,
+                                  int data_shards, int parity_shards, int device, int radius,
+                                  uint32_t *rebuilt, int *n_rebuilt, swec_damage_report *report,
+                                  swec_damage_range *ranges, int ranges_cap, int *n_ranges, int *ok);
+int swec_reconstruct_checked_device(swec_encoder *enc, void *const *shards, const uint8_t *present, size_t shard_len,
+                                    int radius, swec_damage_report *report, swec_damage_range *ranges, int ranges_cap,
+                                    int *n_ranges, void *stream);
 int swec_write_dat_file(const char *base_file_name, int64_t dat_file_size,
                         const char *const *shard_file_names, int data_shards,
                         int64_t large_block, int64_t small_block);

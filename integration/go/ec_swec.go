@@ -483,6 +483,46 @@ func swecRepairEcDamage(baseFileName string, ctx *ECContext, additionalDirs []st
 	return repaired, details, nil
 }
 
+// swecRebuildEcFilesChecked is RebuildEcFiles reading every present shard (rebuildEcFiles, ec_encoder.go:342-357),
+// which corrects the damage it locates in the shards it rebuilds from instead of copying it into every rebuilt shard:
+// a lost disk plus bit rot on the others is the common case.  Use radius 1 by default.  Use radius 0 when two or more
+// shards are lost and no guess is wanted: with few check shards left, radius 1 can blame the wrong shard, and radius 0
+// only reports the damaged columns, rebuilding them as plain rebuild does.  Present shard files are never written; run
+// swecRepairEcDamage on the completed set afterwards to fix them.  details say where damage was found or left.
+func swecRebuildEcFilesChecked(baseFileName string, ctx *ECContext, additionalDirs []string, radius int) (generated []uint32, details []string, err error) {
+	cs := C.CString(baseFileName)
+	defer C.free(unsafe.Pointer(cs))
+	dirs := make([]*C.char, len(additionalDirs)+1)
+	for i, d := range additionalDirs {
+		dirs[i] = C.CString(d)
+		defer C.free(unsafe.Pointer(dirs[i]))
+	}
+	var ids [C.SWEC_MAX_SHARDS]C.uint32_t
+	var report C.swec_damage_report
+	var nIds, nRanges, ok C.int
+	if err := swecCall(func() C.int {
+		return C.swec_rebuild_ec_files_checked(cs, (**C.char)(unsafe.Pointer(&dirs[0])), C.int(len(additionalDirs)),
+			C.int(ctx.DataShards), C.int(ctx.ParityShards), swecPickDevice(), C.int(radius), &ids[0], &nIds, &report,
+			nil, 0, &nRanges, &ok)
+	}); err != nil {
+		return nil, nil, fmt.Errorf("rebuild ec files checked: %w", err)
+	}
+	for i := 0; i < int(nIds); i++ {
+		generated = append(generated, uint32(ids[i]))
+	}
+	for i := 0; i < ctx.DataShards+ctx.ParityShards; i++ {
+		if n := uint64(report.shard_bytes[i]); n > 0 {
+			details = append(details, fmt.Sprintf("ec shard %d: %d bytes wrong, kept out of the rebuilt shards, offsets %d..%d",
+				i, n, int64(report.shard_first[i]), int64(report.shard_last[i])))
+		}
+	}
+	if report.uncorrectable_columns > 0 {
+		details = append(details, fmt.Sprintf("%d byte columns are damaged in more shards than can be corrected, rebuilt from the shards as found, offsets %d..%d",
+			uint64(report.uncorrectable_columns), int64(report.first_uncorrectable), int64(report.last_uncorrectable)))
+	}
+	return generated, details, nil
+}
+
 // ---- pinned batch buffers ---------------------------------------------------------------------------------
 // runtime.Pinner only stops the Go GC from moving a slice; to CUDA such memory is PAGEABLE, so every Encode /
 // Reconstruct on it bounces through the library's pinned ring (a memcpy per shard each way).  The batch buffers of

@@ -113,6 +113,12 @@ PROTOTYPES = {
                                         C.POINTER(C.c_int)]),
     "swec_correct_damage_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.POINTER(DamageReport),
                                              C.POINTER(DamageRange), C.c_int, C.POINTER(C.c_int), C.c_void_p]),
+    "swec_rebuild_ec_files_checked": (C.c_int, [C.c_char_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                                C.c_void_p, C.POINTER(C.c_int), C.POINTER(DamageReport),
+                                                C.POINTER(DamageRange), C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "swec_reconstruct_checked_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int,
+                                                  C.POINTER(DamageReport), C.POINTER(DamageRange), C.c_int,
+                                                  C.POINTER(C.c_int), C.c_void_p]),
     "swec_write_dat_file": (C.c_int, [C.c_char_p, C.c_int64, C.c_void_p, C.c_int, C.c_int64, C.c_int64]),
     "swec_ec_shards_generate": (C.c_int, [C.c_char_p, C.c_char_p, C.c_uint32, C.c_uint64, C.c_int]),
     "swec_ec_shards_rebuild": (C.c_int, [C.c_char_p, C.c_char_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p,

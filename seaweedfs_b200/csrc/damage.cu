@@ -16,9 +16,16 @@
 //                        Per-lane runs (set, count, first, last) merge the columns a lane blames on one shard, and a
 //                        warp merges equal runs with __match_any_sync / __reduce_*_sync before one set of atomics.
 //                        Bytes after the last whole vector, and unaligned streams, go through a byte loop.
-//                        The correcting instantiation (CORRECT) also XORs each blamed shard's error value into that
+//                        The correcting instantiation (kCorrect) also XORs each blamed shard's error value into that
 //                        shard's byte of the column, which makes the column a codeword again; it reads stored parity
 //                        with coherent loads, because it writes it.
+//                        The rebuilding instantiation (kRebuild) decodes the punctured code of a set with f missing
+//                        shards: positions [0, k) are the first k present shards (the information set I), positions
+//                        [k, k+c) the other present ones, whose rows P' = G[C]·G[I]^-1 take the place of P.  The f
+//                        rebuilt streams were computed from I by the rows R = G[missing]·G[I]^-1, so an error e_j in
+//                        information position j put R[r][j]·e_j into rebuilt byte x of stream r: the kernel XORs it
+//                        back out.  A blamed check position, and every present shard, are left as they are.  Radius 0
+//                        counts every damaged column as uncorrectable and decodes none.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -37,6 +44,9 @@ namespace {
 constexpr int kSets = SWEC_MAX_SHARDS + 1;  // one counter set per shard, and one for uncorrectable columns (set k+m)
 constexpr int kCounters = 3 * kSets + 1;    // bytes[kSets], first[kSets], last[kSets], damaged columns
 constexpr int kPageShift = 12;              // 4 KiB pages
+constexpr u8 kLogZero = 0xff;               // log R entry of a zero coefficient (logs of non-zero bytes are < 255)
+
+enum : int { kLocate = 0, kCorrect = 1, kRebuild = 2 };  // the instantiations of swec_locate_kernel
 
 struct LocateTables {
     u8 log[256];
@@ -47,6 +57,12 @@ struct LocateTables {
 constexpr int kTableWords = int(sizeof(LocateTables) / 4);
 static_assert(sizeof(LocateTables) % 16 == 0, "tables are copied in words");
 
+// kRebuild only, in shared memory of its own so that the other instantiations copy no more than before
+struct RebuildTables {
+    u8 logr[32 * 32];  // log R[r][j] at r*32 + j, kLogZero for a zero entry
+};
+constexpr int kRebuildWords = int(sizeof(RebuildTables) / 4);
+
 struct LocateParams {
     const u8* comp[SWEC_MAX_SHARDS];
     const u8* stored[SWEC_MAX_SHARDS];
@@ -56,7 +72,10 @@ struct LocateParams {
     unsigned long long* ctr;
     u32* pages;
     u64 page_words;
-    u8* fix[SWEC_MAX_SHARDS];  // correcting kernel: the k+m shards' bytes of these columns (fix[k+p] == stored[p])
+    u8* fix[SWEC_MAX_SHARDS];  // kCorrect: the k+m shards' bytes of these columns (fix[k+p] == stored[p]);
+                               // kRebuild: the nout rebuilt streams
+    int nout;                  // kRebuild: rebuilt streams
+    const u32* rtables;        // kRebuild: RebuildTables
 };
 
 struct Run {  // columns one lane blamed on one set, in increasing offset order
@@ -130,8 +149,8 @@ __device__ __forceinline__ bool multiple_of_column(const LocateTables& t, const 
 }
 
 // Shards that explain the non-zero syndrome s within the radius, ascending in *a, *b; returns how many (0: none does).
-// CORRECT: also their error values in *ea, *eb, the bytes that XORed into the shards turn the column into a codeword.
-template <bool CORRECT>
+// VALUES: also their error values in *ea, *eb, the bytes that XORed into the shards turn the column into a codeword.
+template <bool VALUES>
 __device__ int decode_column(const LocateTables& t, const u8* s, int k, int m, int radius, int* a, int* b, u8* ea, u8* eb) {
     u8 L[SWEC_MAX_SHARDS];
     u32 nz = 0;
@@ -142,7 +161,7 @@ __device__ int decode_column(const LocateTables& t, const u8* s, int k, int m, i
     const int w = __popc(nz);
     if (w == 1) {
         *a = k + __ffs(nz) - 1;
-        if (CORRECT) *ea = s[*a - k];
+        if (VALUES) *ea = s[*a - k];
         return 1;
     }
     if (w == m)  // every entry of an MDS P is non-zero
@@ -150,7 +169,7 @@ __device__ int decode_column(const LocateTables& t, const u8* s, int k, int m, i
             int r;
             if (multiple_of_column(t, L, m, j, -1, r)) {
                 *a = j;
-                if (CORRECT) *ea = t.exp[r];
+                if (VALUES) *ea = t.exp[r];
                 return 1;
             }
         }
@@ -158,7 +177,7 @@ __device__ int decode_column(const LocateTables& t, const u8* s, int k, int m, i
     if (w == 2) {
         *a = k + __ffs(nz) - 1;
         *b = k + __ffs(nz & (nz - 1)) - 1;
-        if (CORRECT) {
+        if (VALUES) {
             *ea = s[*a - k];
             *eb = s[*b - k];
         }
@@ -172,7 +191,7 @@ __device__ int decode_column(const LocateTables& t, const u8* s, int k, int m, i
             if (multiple_of_column(t, L, m, j, q, r)) {
                 *a = j;
                 *b = k + q;
-                if (CORRECT) {  // s_q = P[q][j]·e_j ^ e_q
+                if (VALUES) {  // s_q = P[q][j]·e_j ^ e_q
                     *ea = t.exp[r];
                     *eb = s[q] ^ t.exp[r + t.logp[q * 32 + j]];
                 }
@@ -195,7 +214,7 @@ __device__ int decode_column(const LocateTables& t, const u8* s, int k, int m, i
             if (ok) {
                 *a = x;
                 *b = y;
-                if (CORRECT) {
+                if (VALUES) {
                     *ea = t.exp[lx];
                     *eb = t.exp[ly];
                 }
@@ -205,26 +224,42 @@ __device__ int decode_column(const LocateTables& t, const u8* s, int k, int m, i
     return 0;
 }
 
-// column x of the launch (shard offset p.base + x); the correcting kernel XORs the error values into the shards
-template <bool CORRECT>
-__device__ __forceinline__ void blame(const LocateParams& p, const LocateTables& t, const u8* s, int m, u64 x, Run* run) {
+// kRebuild: the error value e of position j carried into byte x of every rebuilt stream (nothing for a check position)
+__device__ __forceinline__ void propagate(const LocateParams& p, const LocateTables& t, const u8* logr, int j, u8 e, u64 x) {
+    if (j >= p.k) return;
+    const int le = t.log[e];
+    for (int r = 0; r < p.nout; r++) {
+        const u8 lr = logr[r * 32 + j];
+        if (lr != kLogZero) p.fix[r][x] ^= t.exp[lr + le];
+    }
+}
+
+// column x of the launch (shard offset p.base + x); the correcting kernel XORs the error values into the shards, the
+// rebuilding kernel their images into the rebuilt streams
+template <int MODE>
+__device__ __forceinline__ void blame(const LocateParams& p, const LocateTables& t, const u8* logr, const u8* s, int m,
+                                      u64 x, Run* run) {
     int a = -1, b = -1;
     u8 ea = 0, eb = 0;
     const u64 off = p.base + x;
-    const int found = decode_column<CORRECT>(t, s, p.k, m, p.radius, &a, &b, &ea, &eb);
+    const int found = (MODE == kRebuild && p.radius == 0)
+                          ? 0
+                          : decode_column<MODE != kLocate>(t, s, p.k, m, p.radius, &a, &b, &ea, &eb);
     if (!found) {
         record(p, run, p.k + m, off);
         return;
     }
     record(p, run, a, off);
-    if (CORRECT) p.fix[a][x] ^= ea;
+    if (MODE == kCorrect) p.fix[a][x] ^= ea;
+    if (MODE == kRebuild) propagate(p, t, logr, a, ea, x);
     if (found == 2) {
         record(p, run, b, off);
-        if (CORRECT) p.fix[b][x] ^= eb;
+        if (MODE == kCorrect) p.fix[b][x] ^= eb;
+        if (MODE == kRebuild) propagate(p, t, logr, b, eb, x);
     }
 }
 
-// Stored parity is read through the non-coherent path only by the kernel that does not write it.
+// Stored parity is read through the non-coherent path only by the kernels that do not write it.
 template <bool CORRECT>
 __device__ __forceinline__ uint4 load_stored(const u8* p) {
     if (CORRECT) return *reinterpret_cast<const uint4*>(p);
@@ -240,12 +275,20 @@ __device__ __forceinline__ uint4 xor4(const uint4& a, const uint4& b) {
     return make_uint4(a.x ^ b.x, a.y ^ b.y, a.z ^ b.z, a.w ^ b.w);
 }
 
-// MT > 0: m known at compile time; 0: run-time m.  CORRECT: fix every column decoded within the radius in place.  A
-// column's bytes are read and written only by the thread that owns its vector (or its byte in the tail loop).
-template <int MT, bool CORRECT>
+// MT > 0: m known at compile time; 0: run-time m.  MODE: kLocate, kCorrect (fix every column decoded within the radius
+// in place) or kRebuild (take the errors of the information positions out of the rebuilt streams).  A column's bytes
+// are read and written only by the thread that owns its vector (or its byte in the tail loop).
+template <int MT, int MODE>
 __global__ void __launch_bounds__(256) swec_locate_kernel(const __grid_constant__ LocateParams p) {
+    constexpr bool CORRECT = MODE == kCorrect;
     __shared__ __align__(16) u32 words[kTableWords];
     for (int i = threadIdx.x; i < kTableWords; i += blockDim.x) words[i] = p.tables[i];
+    const u8* logr = nullptr;
+    if constexpr (MODE == kRebuild) {
+        __shared__ __align__(16) u32 rwords[kRebuildWords];
+        for (int i = threadIdx.x; i < kRebuildWords; i += blockDim.x) rwords[i] = p.rtables[i];
+        logr = reinterpret_cast<const u8*>(rwords);
+    }
     __syncthreads();
     const LocateTables& t = *reinterpret_cast<const LocateTables*>(words);
     constexpr int kMaxM = MT > 0 ? MT : SWEC_MAX_SHARDS;
@@ -287,7 +330,7 @@ __global__ void __launch_bounds__(256) swec_locate_kernel(const __grid_constant_
                 }
                 if (!any) continue;
                 damaged++;
-                blame<CORRECT>(p, t, s, m, (v << 4) + u64(c), run);
+                blame<MODE>(p, t, logr, s, m, (v << 4) + u64(c), run);
             }
         }
         const u64 wbase = p.base + (vb << 4);
@@ -306,17 +349,17 @@ __global__ void __launch_bounds__(256) swec_locate_kernel(const __grid_constant_
         }
         if (!any) continue;
         atomicAdd(p.ctr + 3 * kSets, 1ull);
-        blame<CORRECT>(p, t, s, m, x, run);
+        blame<MODE>(p, t, logr, s, m, x, run);
         flush_plain(p, run[0]);
         flush_plain(p, run[1]);
     }
 }
 
-template <int MT, bool CORRECT>
+template <int MT, int MODE>
 unsigned locate_grid(u64 n) {
     static int per_sm = 0;  // resident CTAs per SM, the same on every device of this architecture
     if (!per_sm &&
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, swec_locate_kernel<MT, CORRECT>, 256, 0) != cudaSuccess) {
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, swec_locate_kernel<MT, MODE>, 256, 0) != cudaSuccess) {
         cudaGetLastError();
         per_sm = 4;
     }
@@ -325,6 +368,18 @@ unsigned locate_grid(u64 n) {
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const u64 need = (n / 16 + 255) / 256 + 1;
     return unsigned(std::min<u64>(need, u64(sms) * u64(std::max(1, per_sm))));
+}
+
+// logs of the field's non-zero bytes (to base 2), and two periods of powers of 2
+void log_exp_tables(u8* log, u8* exp) {
+    unsigned x = 1;
+    for (int i = 0; i < 255; i++) {
+        exp[i] = u8(x);
+        log[x] = u8(i);
+        x <<= 1;
+        if (x & 0x100) x ^= kFieldPoly;
+    }
+    for (int i = 255; i < 512; i++) exp[i] = exp[i - 255];
 }
 
 }  // namespace
@@ -341,7 +396,23 @@ int check_locate_args(int m, int radius, const swec_damage_report* report, const
     return SWEC_OK;
 }
 
+int check_rebuild_args(int radius, const swec_damage_report* report, const swec_damage_range* ranges, int ranges_cap) {
+    if (!report) return fail(SWEC_ERR_INVALID_ARG, "report is NULL");
+    if (ranges_cap < 0 || (ranges_cap > 0 && !ranges))
+        return fail(SWEC_ERR_INVALID_ARG, "ranges_cap must be >= 0, and ranges non-NULL when it is > 0");
+    if (radius < 0 || radius > 2) return fail(SWEC_ERR_INVALID_ARG, "radius must be 0, 1 or 2");
+    return SWEC_OK;
+}
+
+void unchecked_report(swec_damage_report* report, int* n_ranges) {
+    memset(report, 0, sizeof *report);
+    report->first_uncorrectable = report->last_uncorrectable = -1;
+    for (int i = 0; i < SWEC_MAX_SHARDS; i++) report->shard_first[i] = report->shard_last[i] = -1;
+    if (n_ranges) *n_ranges = 0;
+}
+
 DamageLocator::~DamageLocator() {
+    if (rtables_) cudaFree(rtables_);
     if (tables_) cudaFree(tables_);
     if (counters_) cudaFree(counters_);
     if (pages_) cudaFree(pages_);
@@ -353,16 +424,11 @@ int DamageLocator::init(const Matrix& parity, int64_t shard_len, int radius, cud
     radius_ = radius;
     correct_ = correct;
     shard_len_ = shard_len;
+    ids_.resize(size_t(k_ + m_));
+    for (int i = 0; i < k_ + m_; i++) ids_[size_t(i)] = i;
     LocateTables t;
     memset(&t, 0, sizeof t);
-    unsigned x = 1;
-    for (int i = 0; i < 255; i++) {
-        t.exp[i] = u8(x);
-        t.log[x] = u8(i);
-        x <<= 1;
-        if (x & 0x100) x ^= kFieldPoly;
-    }
-    for (int i = 255; i < 512; i++) t.exp[i] = t.exp[i - 255];
+    log_exp_tables(t.log, t.exp);
     const GF& gf = GF::get();
     for (int i = 0; i < m_; i++)
         for (int j = 0; j < k_; j++) t.logp[i * 32 + j] = t.log[parity.at(i, j)];
@@ -384,17 +450,49 @@ int DamageLocator::init(const Matrix& parity, int64_t shard_len, int radius, cud
     return SWEC_OK;
 }
 
-int DamageLocator::launch(const uint8_t* const* computed, uint8_t* const* shards, size_t n, int64_t base,
-                          cudaStream_t s) {
+int DamageLocator::init_rebuild(const Matrix& fused, const std::vector<int>& info, const std::vector<int>& outs,
+                                const uint8_t* present, int64_t shard_len, int radius, cudaStream_t s) {
+    const int k = fused.cols;
+    std::vector<int> check;  // rows of `fused`
+    out_rows_.clear();
+    for (size_t o = 0; o < outs.size(); o++) (present[outs[o]] ? check : out_rows_).push_back(int(o));
+    const int c = int(check.size());
+    Matrix pc(c, k);
+    for (int i = 0; i < c; i++)
+        for (int j = 0; j < k; j++) pc.at(i, j) = fused.at(check[size_t(i)], j);
+    // the punctured code has distance c+1: radius t needs 2t <= c
+    if (int rc = init(pc, shard_len, std::min(radius, c / 2), s)) return rc;
+    rebuild_ = true;
+    check_rows_ = check;
+    for (int j = 0; j < k; j++) ids_[size_t(j)] = info[size_t(j)];
+    for (int i = 0; i < c; i++) ids_[size_t(k + i)] = outs[size_t(check[size_t(i)])];
+    u8 log[256], exp[512];
+    log_exp_tables(log, exp);
+    RebuildTables rt;
+    memset(&rt, kLogZero, sizeof rt);
+    for (size_t r = 0; r < out_rows_.size(); r++)
+        for (int j = 0; j < k; j++)
+            if (const u8 v = fused.at(out_rows_[r], j)) rt.logr[r * 32 + size_t(j)] = log[v];
+    SWEC_CUDA(cudaMalloc(reinterpret_cast<void**>(&rtables_), sizeof rt));
+    SWEC_CUDA(cudaMemcpy(rtables_, &rt, sizeof rt, cudaMemcpyHostToDevice));
+    return SWEC_OK;
+}
+
+int DamageLocator::launch(uint8_t* const* computed, uint8_t* const* shards, size_t n, int64_t base, cudaStream_t s) {
     if (n == 0) return SWEC_OK;
     LocateParams p;
     memset(&p, 0, sizeof p);
     for (int i = 0; i < m_; i++) {
-        p.comp[i] = computed[i];
+        p.comp[i] = computed[rebuild_ ? check_rows_[size_t(i)] : i];
         p.stored[i] = shards[k_ + i];
     }
     if (correct_)
         for (int i = 0; i < k_ + m_; i++) p.fix[i] = shards[i];
+    if (rebuild_) {
+        for (size_t r = 0; r < out_rows_.size(); r++) p.fix[r] = computed[out_rows_[r]];
+        p.nout = int(out_rows_.size());
+        p.rtables = rtables_;
+    }
     p.n = n;
     p.base = u64(base);
     p.k = k_;
@@ -404,12 +502,15 @@ int DamageLocator::launch(const uint8_t* const* computed, uint8_t* const* shards
     p.ctr = counters_;
     p.pages = pages_;
     p.page_words = page_words_;
-    if (correct_) {
-        if (m_ == 4) swec_locate_kernel<4, true><<<locate_grid<4, true>(n), 256, 0, s>>>(p);
-        else swec_locate_kernel<0, true><<<locate_grid<0, true>(n), 256, 0, s>>>(p);
+    if (rebuild_) {
+        if (m_ == 3) swec_locate_kernel<3, kRebuild><<<locate_grid<3, kRebuild>(n), 256, 0, s>>>(p);
+        else swec_locate_kernel<0, kRebuild><<<locate_grid<0, kRebuild>(n), 256, 0, s>>>(p);
+    } else if (correct_) {
+        if (m_ == 4) swec_locate_kernel<4, kCorrect><<<locate_grid<4, kCorrect>(n), 256, 0, s>>>(p);
+        else swec_locate_kernel<0, kCorrect><<<locate_grid<0, kCorrect>(n), 256, 0, s>>>(p);
     } else {
-        if (m_ == 4) swec_locate_kernel<4, false><<<locate_grid<4, false>(n), 256, 0, s>>>(p);
-        else swec_locate_kernel<0, false><<<locate_grid<0, false>(n), 256, 0, s>>>(p);
+        if (m_ == 4) swec_locate_kernel<4, kLocate><<<locate_grid<4, kLocate>(n), 256, 0, s>>>(p);
+        else swec_locate_kernel<0, kLocate><<<locate_grid<0, kLocate>(n), 256, 0, s>>>(p);
     }
     g_kernel_launches++;
     SWEC_CUDA(cudaGetLastError());
@@ -423,19 +524,20 @@ int DamageLocator::collect(swec_damage_report* report, swec_damage_range* ranges
     std::vector<uint32_t> bits(size_t(n + 1) * page_words_);
     SWEC_CUDA(cudaMemcpy(c.data(), counters_, c.size() * sizeof c[0], cudaMemcpyDeviceToHost));
     SWEC_CUDA(cudaMemcpy(bits.data(), pages_, bits.size() * 4, cudaMemcpyDeviceToHost));
-    memset(report, 0, sizeof *report);
+    unchecked_report(report, nullptr);
     report->columns = uint64_t(shard_len_);
     report->damaged_columns = c[3 * kSets];
     report->uncorrectable_columns = c[size_t(n)];
     report->first_uncorrectable = c[size_t(n)] ? int64_t(c[size_t(kSets + n)]) : -1;
     report->last_uncorrectable = c[size_t(n)] ? int64_t(c[size_t(2 * kSets + n)]) : -1;
-    for (int i = 0; i < SWEC_MAX_SHARDS; i++) {
-        const bool hit = i < n && c[size_t(i)];
-        report->shard_bytes[i] = hit ? c[size_t(i)] : 0;
-        report->shard_first[i] = hit ? int64_t(c[size_t(kSets + i)]) : -1;
-        report->shard_last[i] = hit ? int64_t(c[size_t(2 * kSets + i)]) : -1;
+    for (int i = 0; i < n; i++) {  // kernel position i is shard ids_[i]
+        if (!c[size_t(i)]) continue;
+        const int id = ids_[size_t(i)];
+        report->shard_bytes[id] = c[size_t(i)];
+        report->shard_first[id] = int64_t(c[size_t(kSets + i)]);
+        report->shard_last[id] = int64_t(c[size_t(2 * kSets + i)]);
     }
-    // maximal runs of flagged pages: shards in ascending id, then the uncorrectable columns
+    // maximal runs of flagged pages: shards in ascending id (ids_ ascends), then the uncorrectable columns
     const int64_t pages = (shard_len_ + (int64_t(1) << kPageShift) - 1) >> kPageShift;
     int total = 0;
     if (all) all->clear();
@@ -454,7 +556,7 @@ int DamageLocator::collect(swec_damage_report* report, swec_damage_range* ranges
             int64_t end = pg + 1;
             while (end < pages && flagged(end)) end++;
             swec_damage_range r;
-            r.shard_id = set < n ? set : -1;
+            r.shard_id = set < n ? ids_[size_t(set)] : -1;
             r.reserved = 0;
             r.offset = pg << kPageShift;
             r.length = std::min(end << kPageShift, shard_len_) - r.offset;

@@ -199,12 +199,14 @@ double reserve_extents(const std::vector<int>& outs, int64_t size) {
 class FilePipeline {
   public:
     PipeStats stats;
-    // verify = true: streams [K, K+R) are the parity bytes read from disk; the computed parity goes to
-    // streams [K+R, K+2R) and is only compared on the device (no D2H, no writes) — counted per parity stream, or,
-    // with a locator, decoded into the shards it blames.  A correcting locator also fixes those shards in the slot,
-    // and the streams the item writes come back to be written.
-    FilePipeline(swec_encoder* enc, const Matrix& rows, size_t chunk, bool verify = false, DamageLocator* locator = nullptr)
-        : enc_(enc), rows_(rows), chunk_(chunk), verify_(verify), locator_(locator) {}
+    // verify = true: streams [K, K+S) are stored bytes read from disk (S = `stored`, R when negative); the R computed
+    // rows go to streams [K+S, K+S+R) and are only compared on the device (no D2H, no writes) — counted per parity
+    // stream, or, with a locator, decoded into the shards it blames.  A correcting locator also fixes those shards in
+    // the slot, a rebuilding one the rebuilt rows, and the streams the item writes come back to be written.
+    FilePipeline(swec_encoder* enc, const Matrix& rows, size_t chunk, bool verify = false, DamageLocator* locator = nullptr,
+                 int stored = -1)
+        : enc_(enc), rows_(rows), chunk_(chunk), verify_(verify), stored_(verify ? (stored < 0 ? rows.rows : stored) : 0),
+          locator_(locator) {}
     ~FilePipeline() { shutdown(); }
 
     int start() {
@@ -213,13 +215,13 @@ class FilePipeline {
         int rc = enc_->ensure_device();
         if (rc) return rc;
         const size_t nslots = stage_slots();
-        const size_t streams = size_t(rows_.cols + rows_.rows * (verify_ ? 2 : 1));
+        const size_t streams = size_t(rows_.cols + stored_ + rows_.rows);
         if (verify_ && !locator_) {
             SWEC_CUDA(cudaMalloc(reinterpret_cast<void**>(&dev_bad_), sizeof(unsigned long long) * size_t(rows_.rows)));
             SWEC_CUDA(cudaMemset(dev_bad_, 0, sizeof(unsigned long long) * size_t(rows_.rows)));
         }
         // one size for every kind of pipeline of this code on this device (generate: k+m streams, rebuild: k + missing,
-        // verify: k+2m), so that a parked ring fits whichever call comes next
+        // verify: k+2m, checked rebuild: k + c + m <= k+2m), so that a parked ring fits whichever call comes next
         const size_t slot_bytes = std::max(streams, size_t(enc_->k + 2 * enc_->m)) * chunk_;
         {
             std::lock_guard<std::mutex> lk(parked_mu());
@@ -296,7 +298,7 @@ class FilePipeline {
         const uint8_t* din[SWEC_MAX_SHARDS];
         uint8_t* dout[SWEC_MAX_SHARDS];
         for (int i = 0; i < K; i++) din[i] = b.dev + size_t(i) * chunk_;
-        const int nin = K + (verify_ ? R : 0);
+        const int nin = K + stored_;
         if (len == chunk_) {  // full slot: the input streams are contiguous — one DMA
             e = cudaMemcpyAsync(b.dev, b.host, size_t(nin) * chunk_, cudaMemcpyHostToDevice, b.stream);
         } else {
@@ -304,7 +306,7 @@ class FilePipeline {
                 e = cudaMemcpyAsync(b.dev + size_t(i) * chunk_, b.host + size_t(i) * chunk_, len, cudaMemcpyHostToDevice, b.stream);
         }
         if (e != cudaSuccess) return set_error(cuda_fail(e, "H2D"), s);
-        for (int r = 0; r < R; r++) dout[r] = b.dev + size_t(K + (verify_ ? R : 0) + r) * chunk_;
+        for (int r = 0; r < R; r++) dout[r] = b.dev + size_t(K + stored_ + r) * chunk_;
         int rc;
         {
             std::lock_guard<std::mutex> lk(enc_->mu);
@@ -313,15 +315,16 @@ class FilePipeline {
         if (rc) return set_error(rc, s);
         if (locator_) {
             uint8_t* shards[SWEC_MAX_SHARDS];
-            for (int i = 0; i < K + R; i++) shards[i] = b.dev + size_t(i) * chunk_;
+            for (int i = 0; i < K + stored_; i++) shards[i] = b.dev + size_t(i) * chunk_;
             if ((rc = locator_->launch(dout, shards, len, item.shard_off, b.stream))) return set_error(rc, s);
-            // corrected shards that are written back: their streams come back whole, once each
+            // corrected or rebuilt streams that are written: they come back whole, once each
             uint64_t back = 0;
             for (const WriteOp& w : item.writes) {
                 if ((back >> w.stream) & 1) continue;
                 back |= uint64_t(1) << w.stream;
                 if (e == cudaSuccess)
-                    e = cudaMemcpyAsync(b.host + size_t(w.stream) * chunk_, shards[w.stream], len, cudaMemcpyDeviceToHost, b.stream);
+                    e = cudaMemcpyAsync(b.host + size_t(w.stream) * chunk_, b.dev + size_t(w.stream) * chunk_, len,
+                                        cudaMemcpyDeviceToHost, b.stream);
             }
         } else if (verify_) {
             for (int r = 0; r < R && e == cudaSuccess; r++)
@@ -474,6 +477,7 @@ class FilePipeline {
     const size_t io_piece_ = std::max<size_t>(4096, env_size("SWEC_FILE_IO_PIECE", size_t(2) << 20) & ~size_t(4095));
     double t_begin_ = 0;
     bool verify_ = false;
+    int stored_ = 0;                    // streams read after the K inputs
     DamageLocator* locator_ = nullptr;  // not owned
     unsigned long long* dev_bad_ = nullptr;
     StagingRing ring_;
@@ -669,6 +673,156 @@ int damage_files(const char* base, const char* const* dirs, int ndirs, int k, in
     return SWEC_OK;
 }
 
+// What the checked rebuild adds to swec_rebuild_ec_files: the radius and where the report goes.
+struct Checked {
+    int radius;
+    swec_damage_report* report;
+    swec_damage_range* ranges;
+    int ranges_cap;
+    int* n_ranges;
+    bool checked = false;  // set once the report comes from a locator (c >= 1)
+};
+
+// The checked rebuild's pipeline.  The first k present shards are the information set I; the other c present shards
+// are read too, as the check shards of the punctured code.  Per slot: one apply of the m x k rows of every shard outside
+// I (its c check shards re-encoded, its f missing shards rebuilt), then the rebuilding locator, which compares the c
+// check rows with the stored ones and takes the errors it locates in I out of the f rebuilt rows.  Only those come back
+// and are written.
+int rebuild_checked(swec_encoder* enc, const std::vector<int>& in, const std::vector<int>& in_d,
+                    const std::vector<uint8_t>& present, const std::vector<int>& out, const std::vector<int>& out_d,
+                    int64_t todo, Checked* chk) {
+    const int k = enc->k, total = enc->k + enc->m;
+    std::vector<uint8_t> info(static_cast<size_t>(total), 0);
+    for (int i = 0, n = 0; i < total && n < k; i++)
+        if (present[size_t(i)]) info[size_t(i)] = 1, n++;
+    std::vector<int> ins, outs;  // outs: every shard outside I, ascending, one row of `fused` each
+    Matrix fused;
+    if (!rs_reconstruct_plan(enc->gen, k, info.data(), false, &ins, &outs, &fused))
+        return fail(SWEC_ERR_TOO_FEW_SHARDS, "not enough shards");
+    std::vector<int> checks;     // check shard ids, ascending: streams k .. k+c of a slot
+    std::vector<int> out_rows;   // the fused row of out[r]
+    for (size_t o = 0; o < outs.size(); o++) {
+        if (present[size_t(outs[o])]) checks.push_back(outs[o]);
+        else out_rows.push_back(int(o));
+    }
+    const int c = int(checks.size());
+    const size_t chunk = file_chunk(todo);
+    DamageLocator locator;
+    FilePipeline pipe(enc, fused, chunk, /*verify=*/true, &locator, /*stored=*/c);
+    int rc = pipe.start();
+    if (rc) return rc;
+    if ((rc = locator.init_rebuild(fused, ins, outs, present.data(), todo, chk->radius, enc->stream))) return rc;
+    if (!out.empty()) reserve_extents(out, todo);
+    for (int64_t o = 0; rc == SWEC_OK && o < todo; o += int64_t(chunk)) {
+        Item it;
+        it.len = size_t(std::min<int64_t>(int64_t(chunk), todo - o));
+        it.shard_off = o;
+        for (int i = 0; i < k; i++) it.reads.push_back({i, in[size_t(ins[size_t(i)])], o, 0, it.len, in_d[size_t(ins[size_t(i)])]});
+        for (int i = 0; i < c; i++)
+            it.reads.push_back({k + i, in[size_t(checks[size_t(i)])], o, 0, it.len, in_d[size_t(checks[size_t(i)])]});
+        for (size_t r = 0; r < out.size(); r++) it.writes.push_back({k + c + out_rows[r], out[r], o, 0, it.len, out_d[r]});
+        rc = pipe.submit(std::move(it));
+    }
+    if ((rc = pipe.finish())) return rc;
+    if ((rc = locator.collect(chk->report, chk->ranges, chk->ranges_cap, chk->n_ranges))) return rc;
+    chk->checked = true;
+    return SWEC_OK;
+}
+
+// swec_rebuild_ec_files, and with `chk` swec_rebuild_ec_files_checked: the same files, checks, errors and order.  The
+// checked rebuild reads every present shard, not only the first k, and corrects the damage it locates in the first k
+// before it reaches the rebuilt shards.
+int rebuild_files(const char* base, const char* const* dirs, int ndirs, int k, int m, int device, uint32_t* rebuilt,
+                  int* n_rebuilt, Checked* chk) {
+    if (!base || !rebuilt || !n_rebuilt || (ndirs > 0 && !dirs)) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
+    *n_rebuilt = 0;
+    const std::string b(base);
+    if (k == 0) ec_ratio(b, &k, &m);  // RebuildEcFiles (ec_encoder.go:76-95)
+    CallEncoder enc;
+    int rc = new_call_encoder(k, m, device, &enc);
+    if (rc) return rc;
+    const int total = k + m;
+
+    // pass 1: which shards exist
+    FdSet fds;
+    const long direct = g_opt_file_direct_io.load();
+    std::vector<int> in(static_cast<size_t>(total), -1), in_d(static_cast<size_t>(total), -1);
+    std::vector<uint8_t> present(static_cast<size_t>(total), 0);
+    std::vector<uint32_t> missing;
+    for (int i = 0; i < total; i++) {
+        if ((rc = open_shard(b, dirs, ndirs, i, &fds, &in[size_t(i)], &in_d[size_t(i)], direct & 1))) return rc;
+        present[size_t(i)] = in[size_t(i)] >= 0;
+        if (!present[size_t(i)]) missing.push_back(uint32_t(i));
+    }
+    const int npresent = total - int(missing.size());
+    if (npresent < k)  // before any output file exists — ec_encoder.go:172-175
+        return fail(SWEC_ERR_TOO_FEW_SHARDS, "not enough shards to rebuild " + b + ": found " + std::to_string(npresent) +
+                                                 " shards, need at least " + std::to_string(k));
+    for (uint32_t id : missing) rebuilt[(*n_rebuilt)++] = id;
+    if (missing.empty() && !chk) return SWEC_OK;  // the checked call still checks the set
+
+    // pass 2: create the outputs — ec_encoder.go:182-193.  Whatever goes wrong from here on, the caller gets no
+    // shard ids (the reference returns nil ids with the error) and no half-written output survives: a shard file
+    // that exists is taken for a present input by the next rebuild (findShardFile), so a partial one must not stay.
+    std::vector<int> out, out_d;  // in the order of `missing`
+    struct Undo {
+        const std::string& b;
+        const std::vector<uint32_t>& ids;
+        int* n_rebuilt;
+        size_t created = 0;
+        bool armed = true;
+        ~Undo() {
+            if (!armed) return;
+            for (size_t i = 0; i < created; i++) unlink((b + shard_ext(int(ids[i]))).c_str());
+            *n_rebuilt = 0;
+        }
+    } undo{b, missing, n_rebuilt};
+    for (uint32_t id : missing) {
+        const int fd = fds.keep(open((b + shard_ext(int(id))).c_str(), O_TRUNC | O_WRONLY | O_CREAT, 0644));
+        if (fd < 0) return io_fail("create " + b + shard_ext(int(id)));
+        undo.created++;
+        out.push_back(fd);
+        out_d.push_back(fds.keep(open_direct(b + shard_ext(int(id)), O_WRONLY, direct & 2)));
+    }
+
+    // every present shard must have the same length; the reference steps in 1 MiB reads and fails at the first
+    // short, unequal one
+    int64_t size = -1;
+    for (int fd : in)
+        if (fd >= 0 && (rc = check_length(fd, &size))) return rc;
+    // quirk kept: the reference reads in small-block buffers, and a length above 1 MiB that is not a multiple of
+    // 1 MiB errors on the last read
+    const int64_t mib = kSmallBlockSize;
+    const bool ragged = !missing.empty() && size > mib && size % mib != 0;
+    const int64_t todo = ragged ? size / mib * mib : size;
+
+    const int checks = m - int(missing.size());  // present shards beyond the first k
+    if (chk && checks > 0) {
+        if ((rc = rebuild_checked(enc.get(), in, in_d, present, out, out_d, todo, chk))) return rc;
+    } else {
+        std::vector<int> ins, outs_idx;  // outs_idx == missing: fused row r rebuilds the shard of out[r]
+        Matrix fused;
+        if (!rs_reconstruct_plan(enc->gen, k, present.data(), false, &ins, &outs_idx, &fused))
+            return fail(SWEC_ERR_TOO_FEW_SHARDS, "not enough shards");
+        const size_t chunk = file_chunk(todo);
+        FilePipeline pipe(enc.get(), fused, chunk);
+        if ((rc = pipe.start())) return rc;
+        reserve_extents(out, todo);
+        for (int64_t o = 0; rc == SWEC_OK && o < todo; o += int64_t(chunk)) {
+            Item it;
+            it.len = size_t(std::min<int64_t>(int64_t(chunk), todo - o));
+            for (int i = 0; i < k; i++) it.reads.push_back({i, in[size_t(ins[size_t(i)])], o, 0, it.len, in_d[size_t(ins[size_t(i)])]});
+            for (size_t r = 0; r < out.size(); r++) it.writes.push_back({k + int(r), out[r], o, 0, it.len, out_d[r]});
+            rc = pipe.submit(std::move(it));
+        }
+        if ((rc = pipe.finish())) return rc;
+        if (chk) unchecked_report(chk->report, chk->n_ranges);  // no present shard beyond the first k: nothing to check
+    }
+    if (ragged) return shard_size_error(mib, size % mib);
+    undo.armed = false;
+    return SWEC_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -781,87 +935,20 @@ int swec_write_ec_files(const char* base, int device) {
 
 int swec_rebuild_ec_files(const char* base, const char* const* dirs, int ndirs, int k, int m, int device,
                           uint32_t* rebuilt, int* n_rebuilt) {
-    if (!base || !rebuilt || !n_rebuilt || (ndirs > 0 && !dirs)) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
+    return rebuild_files(base, dirs, ndirs, k, m, device, rebuilt, n_rebuilt, nullptr);
+}
+
+int swec_rebuild_ec_files_checked(const char* base, const char* const* dirs, int ndirs, int k, int m, int device,
+                                  int radius, uint32_t* rebuilt, int* n_rebuilt, swec_damage_report* report,
+                                  swec_damage_range* ranges, int ranges_cap, int* n_ranges, int* ok) {
+    if (!base || !rebuilt || !n_rebuilt || !ok || (ndirs > 0 && !dirs)) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
+    *ok = 0;
     *n_rebuilt = 0;
-    const std::string b(base);
-    if (k == 0) ec_ratio(b, &k, &m);  // RebuildEcFiles (ec_encoder.go:76-95)
-    CallEncoder enc;
-    int rc = new_call_encoder(k, m, device, &enc);
-    if (rc) return rc;
-    const int total = k + m;
-
-    // pass 1: which shards exist
-    FdSet fds;
-    const long direct = g_opt_file_direct_io.load();
-    std::vector<int> in(static_cast<size_t>(total), -1), in_d(static_cast<size_t>(total), -1);
-    std::vector<uint8_t> present(static_cast<size_t>(total), 0);
-    std::vector<uint32_t> missing;
-    for (int i = 0; i < total; i++) {
-        if ((rc = open_shard(b, dirs, ndirs, i, &fds, &in[size_t(i)], &in_d[size_t(i)], direct & 1))) return rc;
-        present[size_t(i)] = in[size_t(i)] >= 0;
-        if (!present[size_t(i)]) missing.push_back(uint32_t(i));
-    }
-    const int npresent = total - int(missing.size());
-    if (npresent < k)  // before any output file exists — ec_encoder.go:172-175
-        return fail(SWEC_ERR_TOO_FEW_SHARDS, "not enough shards to rebuild " + b + ": found " + std::to_string(npresent) +
-                                                 " shards, need at least " + std::to_string(k));
-    for (uint32_t id : missing) rebuilt[(*n_rebuilt)++] = id;
-    if (missing.empty()) return SWEC_OK;
-
-    // pass 2: create the outputs — ec_encoder.go:182-193.  Whatever goes wrong from here on, the caller gets no
-    // shard ids (the reference returns nil ids with the error) and no half-written output survives: a shard file
-    // that exists is taken for a present input by the next rebuild (findShardFile), so a partial one must not stay.
-    std::vector<int> out, out_d;  // in the order of `missing`
-    struct Undo {
-        const std::string& b;
-        const std::vector<uint32_t>& ids;
-        int* n_rebuilt;
-        size_t created = 0;
-        bool armed = true;
-        ~Undo() {
-            if (!armed) return;
-            for (size_t i = 0; i < created; i++) unlink((b + shard_ext(int(ids[i]))).c_str());
-            *n_rebuilt = 0;
-        }
-    } undo{b, missing, n_rebuilt};
-    for (uint32_t id : missing) {
-        const int fd = fds.keep(open((b + shard_ext(int(id))).c_str(), O_TRUNC | O_WRONLY | O_CREAT, 0644));
-        if (fd < 0) return io_fail("create " + b + shard_ext(int(id)));
-        undo.created++;
-        out.push_back(fd);
-        out_d.push_back(fds.keep(open_direct(b + shard_ext(int(id)), O_WRONLY, direct & 2)));
-    }
-
-    // every present shard must have the same length; the reference steps in 1 MiB reads and fails at the first
-    // short, unequal one
-    int64_t size = -1;
-    for (int fd : in)
-        if (fd >= 0 && (rc = check_length(fd, &size))) return rc;
-    // quirk kept: the reference reads in small-block buffers, and a length above 1 MiB that is not a multiple of
-    // 1 MiB errors on the last read
-    const int64_t mib = kSmallBlockSize;
-    const bool ragged = size > mib && size % mib != 0;
-    const int64_t todo = ragged ? size / mib * mib : size;
-
-    std::vector<int> ins, outs_idx;  // outs_idx == missing: fused row r rebuilds the shard of out[r]
-    Matrix fused;
-    if (!rs_reconstruct_plan(enc->gen, k, present.data(), false, &ins, &outs_idx, &fused))
-        return fail(SWEC_ERR_TOO_FEW_SHARDS, "not enough shards");
-    const size_t chunk = file_chunk(todo);
-    FilePipeline pipe(enc.get(), fused, chunk);
-    if ((rc = pipe.start())) return rc;
-    reserve_extents(out, todo);
-    for (int64_t o = 0; rc == SWEC_OK && o < todo; o += int64_t(chunk)) {
-        Item it;
-        it.len = size_t(std::min<int64_t>(int64_t(chunk), todo - o));
-        for (int i = 0; i < k; i++) it.reads.push_back({i, in[size_t(ins[size_t(i)])], o, 0, it.len, in_d[size_t(ins[size_t(i)])]});
-        for (size_t r = 0; r < out.size(); r++) it.writes.push_back({k + int(r), out[r], o, 0, it.len, out_d[r]});
-        rc = pipe.submit(std::move(it));
-    }
-    if ((rc = pipe.finish())) return rc;
-    if (ragged) return shard_size_error(mib, size % mib);
-    undo.armed = false;
-    return SWEC_OK;
+    if (const int rc = check_rebuild_args(radius, report, ranges, ranges_cap)) return rc;
+    Checked chk{radius, report, ranges, ranges_cap, n_ranges};
+    const int rc = rebuild_files(base, dirs, ndirs, k, m, device, rebuilt, n_rebuilt, &chk);
+    *ok = rc == SWEC_OK && chk.checked && report->uncorrectable_columns == 0 ? 1 : 0;
+    return rc;
 }
 
 int swec_verify_ec_files(const char* base, const char* const* dirs, int ndirs, int k, int m, int device,

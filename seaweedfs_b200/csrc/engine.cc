@@ -826,6 +826,61 @@ int swec_correct_damage_device(swec_encoder* e, void* const* shards, size_t n, i
     return damage_device(e, shards, n, radius, true, report, ranges, ranges_cap, n_ranges, stream);
 }
 
+// The first k present shards are the information set; the other c present shards are re-encoded from it into scratch
+// and checked, and the missing shards are rebuilt into the caller's buffers by the same apply, then cleared of the
+// errors the locator finds in the information set.  Present shards are only read.
+int swec_reconstruct_checked_device(swec_encoder* e, void* const* shards, const uint8_t* present, size_t n, int radius,
+                                    swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges,
+                                    void* stream) {
+    if (!e || !shards || !present) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
+    int rc = check_rebuild_args(radius, report, ranges, ranges_cap);
+    if (rc) return rc;
+    const int k = e->k, total = e->k + e->m;
+    std::vector<uint8_t> info(static_cast<size_t>(total), 0);
+    int npresent = 0;
+    for (int i = 0; i < total; i++)
+        if (present[i] && npresent++ < k) info[size_t(i)] = 1;
+    if (npresent < k) return fail(SWEC_ERR_TOO_FEW_SHARDS, "fewer than data_shards shards present");
+    for (int i = 0; i < total; i++)
+        if (!shards[i]) return fail(SWEC_ERR_INVALID_ARG, present[i] ? "NULL shard" : "missing shard has no buffer");
+    std::vector<int> ins, outs;  // outs: every shard outside the information set, ascending, one row of `fused` each
+    Matrix fused;
+    if (!rs_reconstruct_plan(e->gen, k, info.data(), false, &ins, &outs, &fused))
+        return fail(SWEC_ERR_TOO_FEW_SHARDS, "fewer than data_shards shards present");
+    std::vector<int> checks;
+    for (int id : outs)
+        if (present[id]) checks.push_back(id);
+    const int c = int(checks.size());
+    uint8_t* const* sh = reinterpret_cast<uint8_t* const*>(shards);
+    std::lock_guard<std::mutex> lock(e->mu);
+    if ((rc = e->ensure_device())) return rc;
+    cudaStream_t s = pick_stream(e, stream);
+    DamageLocator locator;
+    if (c > 0 && (rc = locator.init_rebuild(fused, ins, outs, present, int64_t(n), radius, s))) return rc;
+    // the computed check rows go to scratch a piece at a time, as in damage_device
+    const size_t piece = std::min(n, size_t(256) << 20);
+    StreamScratch scratch(s);
+    if (piece && c > 0) SWEC_CUDA(scratch.alloc(size_t(c) * piece));
+    for (size_t off = 0; off < n; off += piece) {
+        const size_t len = std::min(piece, n - off);
+        const uint8_t* in[SWEC_MAX_SHARDS];
+        uint8_t* at[SWEC_MAX_SHARDS];  // information shards, then stored check shards
+        uint8_t* comp[SWEC_MAX_SHARDS];
+        for (int i = 0; i < k; i++) in[i] = at[i] = sh[ins[size_t(i)]] + off;
+        for (int i = 0; i < c; i++) at[k + i] = sh[checks[size_t(i)]] + off;
+        for (size_t o = 0, ci = 0; o < outs.size(); o++)
+            comp[o] = present[outs[o]] ? scratch.as<uint8_t>() + (ci++) * piece : sh[outs[o]] + off;
+        if ((rc = e->apply(fused, in, comp, len, Layout{}, s))) return rc;
+        if (c > 0 && (rc = locator.launch(comp, at, len, int64_t(off), s))) return rc;
+    }
+    SWEC_CUDA(cudaStreamSynchronize(s));
+    if (c == 0) {  // every present shard is an information shard: nothing to check
+        unchecked_report(report, n_ranges);
+        return SWEC_OK;
+    }
+    return locator.collect(report, ranges, ranges_cap, n_ranges);
+}
+
 int swec_stream_synchronize(swec_encoder* e, void* stream) {
     if (!e) return fail(SWEC_ERR_INVALID_ARG, "NULL encoder");
     int rc = e->ensure_device();

@@ -195,6 +195,17 @@ class Encoder:
                                                max_ranges, C.byref(n), stream))
         return _damage_result(report, ranges, n.value, max_ranges)
 
+    def reconstruct_checked_device(self, shard_ptrs, present, shard_len: int, radius: int = 1, max_ranges: int = 4096,
+                                   stream: int = 0) -> dict:
+        """reconstruct_device that reads every present shard and corrects the damage it locates in the first k present
+        before it reaches the rebuilt shards (swec_reconstruct_checked_device).  Present shards are only read.  Returns
+        the report of locate_damage_device over the present shards; radius 0 only detects (include/swec.h)."""
+        pres = np.ascontiguousarray(np.asarray(present, dtype=np.uint8))
+        report, ranges, n = DamageReport(), (DamageRange * max(1, max_ranges))(), C.c_int(0)
+        check(lib().swec_reconstruct_checked_device(self._h, _ptrs(shard_ptrs), pres.ctypes.data, shard_len, radius,
+                                                    C.byref(report), ranges, max_ranges, C.byref(n), stream))
+        return _damage_result(report, ranges, n.value, max_ranges)
+
     def synchronize(self, stream: int = 0) -> None:
         check(lib().swec_stream_synchronize(self._h, stream))
 
@@ -335,6 +346,22 @@ def repair_ec_damage(base_file_name: str, additional_dirs: list[str] | None = No
     check(lib().swec_repair_ec_damage(base_file_name.encode(), arr, nd, k, m, dev, radius, C.byref(report), ranges,
                                       max_ranges, C.byref(n), C.byref(ok)))
     return {"ok": bool(ok.value), **_damage_result(report, ranges, n.value, max_ranges)}
+
+
+def rebuild_ec_files_checked(base_file_name: str, additional_dirs: list[str] | None = None,
+                             ctx: ECContext | None = None, device: int = 0, radius: int = 1,
+                             max_ranges: int = 4096) -> dict:
+    """rebuild_ec_files that reads every present shard and corrects the damage it locates in the shards it rebuilds
+    from (swec_rebuild_ec_files_checked).  Returns "rebuilt" (the ids), "ok" (True iff something could be checked and
+    no column is uncorrectable) and the report of locate_ec_damage over the present shards.  Radius 0 only detects;
+    run repair_ec_damage afterwards to fix the present shards (include/swec.h)."""
+    arr, nd = _dirs(additional_dirs)
+    k, m, dev = (ctx.DataShards, ctx.ParityShards, ctx.device) if ctx else (0, 0, device)
+    ids, n_ids = (C.c_uint32 * MaxShardCount)(), C.c_int(0)
+    report, ranges, n, ok = DamageReport(), (DamageRange * max(1, max_ranges))(), C.c_int(0), C.c_int(0)
+    check(lib().swec_rebuild_ec_files_checked(base_file_name.encode(), arr, nd, k, m, dev, radius, ids, C.byref(n_ids),
+                                              C.byref(report), ranges, max_ranges, C.byref(n), C.byref(ok)))
+    return {"rebuilt": list(ids[: n_ids.value]), "ok": bool(ok.value), **_damage_result(report, ranges, n.value, max_ranges)}
 
 
 def write_dat_file(base_file_name: str, dat_file_size: int, shard_file_names: list[str],
