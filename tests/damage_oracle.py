@@ -117,3 +117,126 @@ def report(length: int, n: int, cols: np.ndarray, a: np.ndarray, b: np.ndarray) 
 
 def locate(shards: list[np.ndarray], k: int, m: int, radius: int = 1) -> dict:
     return report(len(shards[0]), k + m, *locate_columns(shards, k, m, radius))
+
+
+# ---------------------------------------------------------------------------------------------- any m (up to 31)
+# The functions above pack a syndrome into one uint64 and so stop at m = 8.  These key a syndrome by its m bytes,
+# compared as a fixed-width string, decode the punctured code of a presence mask as well as the full code, and build the
+# report from per-column blame with whole-array operations, so that it also serves 2^28-column shard sets on the GPU.
+
+
+def byte_keys(s: np.ndarray) -> np.ndarray:
+    """One key per row of s (..., c) uint8: its c bytes as a fixed-width string (any c)."""
+    s = np.ascontiguousarray(s, dtype=np.uint8).reshape(-1, s.shape[-1])
+    return s.view(np.dtype((np.void, s.shape[-1]))).ravel()
+
+
+@functools.lru_cache(maxsize=None)
+def punctured_rows(k: int, m: int, present: tuple | None = None):
+    """(info ids, check ids, lost ids, P' = G[C]·G[I]^-1, R = G[lost]·G[I]^-1) for a presence mask: I the first k present
+    shards, C the other present ones.  present None: the full code, P' = P."""
+    g = rn.build_matrix(k, k + m)
+    present = present or (True,) * (k + m)
+    ids = [i for i in range(k + m) if present[i]]
+    info, checks = ids[:k], ids[k:]
+    lost = [i for i in range(k + m) if not present[i]]
+    ginv = rn.mat_inv(g[info])
+    pc = rn.mat_mul(g[checks], ginv) if checks else np.zeros((0, k), dtype=np.uint8)
+    r = rn.mat_mul(g[lost], ginv) if lost else np.zeros((0, k), dtype=np.uint8)
+    return info, checks, lost, pc, r
+
+
+@functools.lru_cache(maxsize=None)
+def error_table(k: int, m: int, radius: int, present: tuple | None = None):
+    """Every pattern of 1..radius wrong positions of the (punctured) code with every non-zero value, sorted by byte key:
+    (keys, syndromes (N, c), positions a < b (-1: none), values va, vb).  Positions [0, k) are the information set,
+    [k, k+c) the check shards.  Asserts that no two patterns share a syndrome (the code is MDS within the radius)."""
+    pc = punctured_rows(k, m, present)[3]
+    c = pc.shape[0]
+    h = np.concatenate([pc, np.eye(c, dtype=np.uint8)], axis=1)
+    n = k + c
+    e = np.arange(1, 256, dtype=np.uint8)
+    cols = [rn.MUL[e[:, None], h[:, j][None, :]] for j in range(n)]  # (255, c): e·h_j
+    syn, a, b, va, vb = [np.zeros((0, c), dtype=np.uint8)], [], [], [], []
+    if radius >= 1:
+        for j in range(n):
+            syn.append(cols[j])
+            a.append(np.full(255, j, dtype=np.int16))
+            b.append(np.full(255, -1, dtype=np.int16))
+            va.append(e)
+            vb.append(np.zeros(255, dtype=np.uint8))
+    if radius >= 2:
+        for x in range(n):
+            for y in range(x + 1, n):
+                syn.append((cols[x][:, None, :] ^ cols[y][None, :, :]).reshape(-1, c))
+                a.append(np.full(255 * 255, x, dtype=np.int16))
+                b.append(np.full(255 * 255, y, dtype=np.int16))
+                va.append(np.repeat(e, 255))
+                vb.append(np.tile(e, 255))
+    syn = np.concatenate(syn)
+    a, b, va, vb = (np.concatenate(v) if v else np.zeros(0, dtype=t) for v, t in
+                    ((a, np.int16), (b, np.int16), (va, np.uint8), (vb, np.uint8)))
+    keys = byte_keys(syn)
+    order = np.argsort(keys, kind="stable")
+    keys, syn = keys[order], syn[order]
+    assert not (keys[1:] == keys[:-1]).any(), "two patterns within the radius share a syndrome: the code is not MDS"
+    return keys, syn, a[order], b[order], va[order], vb[order]
+
+
+def decode_columns(shards: list, k: int, m: int, radius: int, present: tuple | None = None):
+    """Damaged columns of a shard set (lost shards may be None) and what decoding within the radius finds in each:
+    (cols, positions a, b (-1: none; both -1: uncorrectable), values va, vb, position -> shard id)."""
+    info, checks, _, pc, _ = punctured_rows(k, m, present)
+    comp = rn.apply_rows(pc, [shards[i] for i in info])
+    s = np.stack([x ^ shards[i] for x, i in zip(comp, checks)], axis=1)
+    cols = np.flatnonzero(s.any(axis=1))
+    keys, _, a, b, va, vb = error_table(k, m, radius, present)
+    q = byte_keys(s[cols])
+    pos = np.minimum(np.searchsorted(keys, q), max(len(keys) - 1, 0))
+    found = (keys[pos] == q) if len(keys) else np.zeros(len(cols), dtype=bool)
+    pick = [np.where(found, v[pos] if len(v) else fill, fill) for v, fill in ((a, -1), (b, -1), (va, 0), (vb, 0))]
+    return cols, pick[0].astype(np.int64), pick[1].astype(np.int64), pick[2].astype(np.uint8), \
+        pick[3].astype(np.uint8), np.array(info + checks, dtype=np.int64)
+
+
+def _runs(flags: np.ndarray, length: int, shard_id: int) -> list[tuple[int, int, int]]:
+    """(shard id, offset, length) of every maximal run of flagged pages."""
+    pages = np.flatnonzero(flags)
+    if not len(pages):
+        return []
+    cut = np.flatnonzero(np.diff(pages) != 1) + 1
+    starts, ends = pages[np.r_[0, cut]], pages[np.r_[cut - 1, len(pages) - 1]] + 1
+    return [(shard_id, int(s) * PAGE, min(int(e) * PAGE, length) - int(s) * PAGE) for s, e in zip(starts, ends)]
+
+
+def dense_report(a, b, damaged, n: int) -> dict:
+    """damage_oracle.report from per-column blame: torch tensors over every column (on any device) of the shard ids a
+    and b each column is blamed on (-1: none) and whether it is damaged.  One pass over the columns per shard, no Python
+    loop per column, so it takes the 2^28 columns of a device call."""
+    import torch
+    length = damaged.numel()
+    whole = length // PAGE * PAGE
+
+    def summary(mask):
+        cnt = int(mask.sum())
+        if not cnt:
+            return 0, -1, -1, np.zeros(0, dtype=bool)
+        first = int(mask.to(torch.uint8).argmax())
+        last = length - 1 - int(mask.flip(0).to(torch.uint8).argmax())
+        flags = mask[:whole].view(-1, PAGE).any(1)
+        if whole < length:
+            flags = torch.cat([flags, mask[whole:].any().view(1)])
+        return cnt, first, last, flags.cpu().numpy()
+
+    shards, ranges = {}, []
+    for sid in range(n):
+        cnt, first, last, flags = summary((a == sid) | (b == sid))
+        if cnt:
+            shards[sid] = (cnt, first, last)
+            ranges += _runs(flags, length, sid)
+    unc, first_u, last_u, flags = summary(damaged & (a < 0) & (b < 0))
+    ranges += _runs(flags, length, -1)
+    n_damaged = int(damaged.sum())
+    return {"ok": n_damaged == 0, "columns": length, "damaged_columns": n_damaged, "uncorrectable_columns": unc,
+            "first_uncorrectable": first_u, "last_uncorrectable": last_u, "shards": shards, "ranges": ranges,
+            "n_ranges": len(ranges)}
