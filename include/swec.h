@@ -27,6 +27,8 @@
  *   swec_ec_shards_generate     VolumeEcShardsGenerate (file work)   weed/server/volume_grpc_erasure_coding.go:43-146
  *   swec_ec_shards_rebuild      VolumeEcShardsRebuild  (file work)   weed/server/volume_grpc_erasure_coding.go:149-225
  *   swec_ec_shards_to_volume    VolumeEcShardsToVolume (file work)   weed/server/volume_grpc_erasure_coding.go:578-668
+ *   swec_ec_shards_to_volume_checked  the same from any k shards, correcting damaged data shards before the .dat is
+ *                               written (swec_write_dat_file_checked, swec_decode_data_checked_device)
  *   swec_read_ec_needles        Store.ReadEcShardNeedle (local shards, batched)   weed/storage/store_ec.go:252-355,482-560
  *   swec_check_index_file       idx.CheckIndexFile / EcVolume.ScrubIndex   weed/storage/idx/check.go:36-111
  *   swec_check_needles_device   Needle.ReadBytes on records in HBM   weed/storage/needle/needle_read.go:59-190,
@@ -66,7 +68,8 @@ typedef enum swec_status {
     SWEC_ERR_JIT = -8,             /* run-time kernel specialisation failed                     */
     SWEC_ERR_NO_LIVE_NEEDLES = -9, /* ec.decode of a volume whose index has no live entries      */
     SWEC_ERR_NOT_FOUND = -10,      /* needle id not in .ecx (erasure_coding.NotFoundError)       */
-    SWEC_ERR_DELETED = -11         /* needle is tombstoned or journalled (storage.ErrorDeleted)  */
+    SWEC_ERR_DELETED = -11,        /* needle is tombstoned or journalled (storage.ErrorDeleted)  */
+    SWEC_ERR_UNCORRECTABLE = -12   /* checked decode: damage left that cannot be corrected       */
 } swec_status;
 
 typedef struct swec_encoder swec_encoder;
@@ -327,6 +330,48 @@ int swec_reconstruct_checked_device(swec_encoder *enc, void *const *shards, cons
 int swec_write_dat_file(const char *base_file_name, int64_t dat_file_size,
                         const char *const *shard_file_names, int data_shards,
                         int64_t large_block, int64_t small_block);
+/* ---- checked decode: errors and erasures before the parity is dropped -----------------------------------------------
+ * ec.decode deletes every shard, parity included, once the .dat is written (weed/shell/command_ec_decode.go:156-181),
+ * so it is the last point at which damage in the data shards can be corrected.  swec_write_dat_file copies the data
+ * shards byte for byte and needs all of them.  The checked decode needs any k of the k+m shards.  It decodes like the
+ * checked rebuild above: the first k present shards are the information set, the other c = (present shards) - k are
+ * its check shards (always parity shards), and the radius used is t = min(radius, floor(c/2)), radius 0, 1 or 2.
+ * Unlike the checked rebuild, it also corrects the damage located in present data shards, so per column:
+ *   - at most t wrong present shards: every data byte of the column is the true one, present or rebuilt;
+ *   - t+1 .. c-t wrong present shards: the column is counted as uncorrectable, and its data bytes are exactly what
+ *     swec_reconstruct_device(data_only = 1) gives from the shards as found;
+ *   - more than c-t wrong present shards: the data bytes can be wrong (the limit of the code);
+ *   - radius 0: every damaged column is uncorrectable.
+ * Only missing data shards are rebuilt; a missing parity shard is neither computed nor needed.  Present parity is only
+ * read.  The report and ranges are those of the checked rebuild for the same shards; with c = 0 the report has
+ * columns = 0 and no ranges.  Argument rules: those of swec_reconstruct_checked_device (SWEC_ERR_INVALID_ARG first).
+ * Device level: shards[k+m] in HBM, shard_len bytes each.  Every data shard needs a buffer: present ones are corrected in
+ * place, missing ones rebuilt.  A missing parity shard may be NULL.  Fewer than k present is SWEC_ERR_TOO_FEW_SHARDS.
+ * The check shards are re-encoded into scratch of at most 256 MiB per shard at a time; synchronises `stream`.  With
+ * c = 0 it is swec_reconstruct_device(data_only = 1).
+ * File level: swec_write_dat_file_checked is swec_write_dat_file from shard_file_names[k+m] (NULL = missing): the same
+ * copy plan and the same .dat bytes, as if written from the corrected data shards.  The columns decoded are those the
+ * plan reads from shard 0, [0, columns).  Before any device work and before the .dat is created, in this order: fewer
+ * than k shards present is SWEC_ERR_TOO_FEW_SHARDS, present shards of unequal length SWEC_ERR_SHARD_SIZE, and shards
+ * shorter than the plan needs SWEC_ERR_IO (the short read of the plain call).  Shard files are never opened for writing.
+ * If any column is left uncorrectable the call fails with SWEC_ERR_UNCORRECTABLE and removes the .dat, with the report
+ * and ranges filled in: a caller that then keeps the EC shards loses nothing.  Radius 0 therefore decodes only a set
+ * in which every checked column is clean.  On any other failure no .dat is left either.  *ok = 1 iff c >= 1 and no
+ * column is uncorrectable.  With every data shard present and no parity shard (c = 0, nothing missing) there is
+ * nothing to check or rebuild: the call is swec_write_dat_file, with no GPU work, columns = 0 and *ok = 0.
+ * swec_ec_shards_to_volume_checked is swec_ec_shards_to_volume with this call in place of swec_write_dat_file, and any k
+ * shards instead of all k data shards: the ratio from .vif, the shards looked up in data_base's directory then in
+ * additional_dirs (fewer than k found: SWEC_ERR_TOO_FEW_SHARDS), the .ecj folded into .ecx, SWEC_ERR_NO_LIVE_NEEDLES,
+ * FindDatFileSize, the .dat, the .idx.  FindDatFileSize takes the needle version from the .ec00 superblock, or from
+ * .vif's version when .ec00 is missing; with neither the call fails with SWEC_ERR_TOO_FEW_SHARDS before anything is
+ * written.  On SWEC_ERR_UNCORRECTABLE neither .dat nor .idx is left.                                                */
+int swec_decode_data_checked_device(swec_encoder *enc, void *const *shards, const uint8_t *present, size_t shard_len,
+                                    int radius, swec_damage_report *report, swec_damage_range *ranges, int ranges_cap,
+                                    int *n_ranges, void *stream);
+int swec_write_dat_file_checked(const char *base_file_name, int64_t dat_file_size, const char *const *shard_file_names,
+                                int data_shards, int parity_shards, int64_t large_block, int64_t small_block,
+                                int device, int radius, swec_damage_report *report, swec_damage_range *ranges,
+                                int ranges_cap, int *n_ranges, int *ok);
 
 /* ---- whole-volume operations: what the three EC gRPC handlers do to files, in their order --------- */
 /* VolumeEcShardsGenerate: ratio from data_base.vif when valid else 10+4; index_base.idx → .ecx FIRST;
@@ -347,6 +392,12 @@ int swec_ec_shards_rebuild(const char *data_base_file_name, const char *index_ba
 int swec_ec_shards_to_volume(const char *data_base_file_name, const char *index_base_file_name,
                              const char *const *additional_dirs, int n_additional_dirs,
                              int64_t *dat_file_size);
+/* The same from any k of the k+m shards, correcting damaged data shards on the GPU first (see the checked decode
+ * above).  *dat_file_size may be NULL.                                                                              */
+int swec_ec_shards_to_volume_checked(const char *data_base_file_name, const char *index_base_file_name,
+                                     const char *const *additional_dirs, int n_additional_dirs, int device,
+                                     int radius, int64_t *dat_file_size, swec_damage_report *report,
+                                     swec_damage_range *ranges, int ranges_cap, int *n_ranges, int *ok);
 
 /* Store.ReadEcShardNeedle for MANY needles of one EC volume whose shard files are local (data_base's
  * directory, then additional_dirs) — weed/storage/store_ec.go:252-355,482-560: find each needle in .ecx

@@ -317,6 +317,54 @@ func ecShardsToVolumeSwec(dataBaseFileName, indexBaseFileName string, additional
 	return int64(size), swecErr(rc)
 }
 
+// ecShardsToVolumeCheckedSwec is ecShardsToVolumeSwec from any k of the k+m shards, with the damage the present parity
+// locates in the data shards corrected on the GPU before the .dat is written.  ec.decode deletes every shard once the
+// handler succeeds, so this is the last point at which such damage can be fixed.  Columns that cannot be corrected fail
+// the call (no .dat, no .idx) with the damaged page ranges in the error, and the shell keeps the EC shards.  Radius 1
+// by default; radius 0 decodes only a set whose checked columns are all clean.  The check needs parity shards next to
+// the data shards: collectEcShards copies only data shards today, and without parity the call decodes unchecked
+// (checked = false), exactly as ecShardsToVolumeSwec.
+func ecShardsToVolumeCheckedSwec(dataBaseFileName, indexBaseFileName string, additionalDirs []string, radius int) (datFileSize int64, checked bool, err error) {
+	cd, ci := C.CString(dataBaseFileName), C.CString(indexBaseFileName)
+	defer C.free(unsafe.Pointer(cd))
+	defer C.free(unsafe.Pointer(ci))
+	dirs := make([]*C.char, len(additionalDirs)+1)
+	for i, d := range additionalDirs {
+		dirs[i] = C.CString(d)
+		defer C.free(unsafe.Pointer(dirs[i]))
+	}
+	var size C.int64_t
+	var report C.swec_damage_report
+	var ranges [64]C.swec_damage_range
+	var nRanges, ok C.int
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	rc := C.swec_ec_shards_to_volume_checked(cd, ci, (**C.char)(unsafe.Pointer(&dirs[0])), C.int(len(additionalDirs)),
+		swecPickDevice(), C.int(radius), &size, &report, &ranges[0], C.int(len(ranges)), &nRanges, &ok)
+	switch rc {
+	case C.SWEC_OK:
+		return int64(size), ok != 0, nil
+	case C.SWEC_ERR_NO_LIVE_NEEDLES:
+		return 0, false, errNoLiveEntries
+	case C.SWEC_ERR_UNCORRECTABLE:
+		var where []string
+		for i := 0; i < int(nRanges) && i < len(ranges); i++ {
+			r := ranges[i]
+			who := fmt.Sprintf("ec shard %d", int(r.shard_id))
+			if r.shard_id < 0 {
+				who = "uncorrectable"
+			}
+			where = append(where, fmt.Sprintf("%s [%d, %d)", who, int64(r.offset), int64(r.offset)+int64(r.length)))
+		}
+		if int(nRanges) > len(ranges) {
+			where = append(where, fmt.Sprintf("and %d more ranges", int(nRanges)-len(ranges)))
+		}
+		return 0, false, fmt.Errorf("%w; %d byte columns cannot be corrected, damaged pages: %s", swecErr(rc),
+			uint64(report.uncorrectable_columns), strings.Join(where, ", "))
+	}
+	return 0, false, swecErr(rc)
+}
+
 // ---- the read path of a mounted EC volume whose shards are local files ----------------------------------------
 
 // swecEcVolume is the twin of the long-lived EcVolume (ec_volume.go:36-160) for Store.ReadEcShardNeedle

@@ -14,7 +14,7 @@ STATUS = {
     0: "SWEC_OK", -1: "SWEC_ERR_INVALID_ARG", -2: "SWEC_ERR_TOO_FEW_SHARDS", -3: "SWEC_ERR_CUDA",
     -4: "SWEC_ERR_IO", -5: "SWEC_ERR_NOMEM", -6: "SWEC_ERR_SHARD_SIZE", -7: "SWEC_ERR_NO_DEVICE",
     -8: "SWEC_ERR_JIT", -9: "SWEC_ERR_NO_LIVE_NEEDLES",
-    -10: "SWEC_ERR_NOT_FOUND", -11: "SWEC_ERR_DELETED",
+    -10: "SWEC_ERR_NOT_FOUND", -11: "SWEC_ERR_DELETED", -12: "SWEC_ERR_UNCORRECTABLE",
 }
 
 
@@ -119,11 +119,20 @@ PROTOTYPES = {
     "swec_reconstruct_checked_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int,
                                                   C.POINTER(DamageReport), C.POINTER(DamageRange), C.c_int,
                                                   C.POINTER(C.c_int), C.c_void_p]),
+    "swec_decode_data_checked_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int,
+                                                  C.POINTER(DamageReport), C.POINTER(DamageRange), C.c_int,
+                                                  C.POINTER(C.c_int), C.c_void_p]),
     "swec_write_dat_file": (C.c_int, [C.c_char_p, C.c_int64, C.c_void_p, C.c_int, C.c_int64, C.c_int64]),
+    "swec_write_dat_file_checked": (C.c_int, [C.c_char_p, C.c_int64, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_int64,
+                                              C.c_int, C.c_int, C.POINTER(DamageReport), C.POINTER(DamageRange), C.c_int,
+                                              C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "swec_ec_shards_generate": (C.c_int, [C.c_char_p, C.c_char_p, C.c_uint32, C.c_uint64, C.c_int]),
     "swec_ec_shards_rebuild": (C.c_int, [C.c_char_p, C.c_char_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
                                          C.POINTER(C.c_int)]),
     "swec_ec_shards_to_volume": (C.c_int, [C.c_char_p, C.c_char_p, C.c_void_p, C.c_int, C.POINTER(C.c_int64)]),
+    "swec_ec_shards_to_volume_checked": (C.c_int, [C.c_char_p, C.c_char_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                                   C.POINTER(C.c_int64), C.POINTER(DamageReport), C.POINTER(DamageRange),
+                                                   C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "swec_read_ec_needles": (C.c_int, [C.c_char_p, C.c_char_p, C.c_void_p, C.c_int, C.POINTER(NeedleRead), C.c_int, C.c_int]),
     "swec_ec_volume_open": (C.c_int, [C.c_char_p, C.c_char_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     "swec_ec_volume_read_needles": (C.c_int, [C.c_void_p, C.POINTER(NeedleRead), C.c_int]),

@@ -26,6 +26,10 @@
 //                        information position j put R[r][j]·e_j into rebuilt byte x of stream r: the kernel XORs it
 //                        back out.  A blamed check position, and every present shard, are left as they are.  Radius 0
 //                        counts every damaged column as uncorrectable and decodes none.
+//                        The decoding instantiation (kDecode) is kRebuild for ec.decode: its rows are those of the
+//                        missing data shards and the check shards only, and it also XORs each located error value of an
+//                        information position that holds a data shard into that shard's own byte, so every data byte of
+//                        a column decoded within the radius is the true one.  Present parity shards are never written.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -46,7 +50,7 @@ constexpr int kCounters = 3 * kSets + 1;    // bytes[kSets], first[kSets], last[
 constexpr int kPageShift = 12;              // 4 KiB pages
 constexpr u8 kLogZero = 0xff;               // log R entry of a zero coefficient (logs of non-zero bytes are < 255)
 
-enum : int { kLocate = 0, kCorrect = 1, kRebuild = 2 };  // the instantiations of swec_locate_kernel
+enum : int { kLocate = 0, kCorrect = 1, kRebuild = 2, kDecode = 3 };  // the instantiations of swec_locate_kernel
 
 struct LocateTables {
     u8 log[256];
@@ -57,7 +61,7 @@ struct LocateTables {
 constexpr int kTableWords = int(sizeof(LocateTables) / 4);
 static_assert(sizeof(LocateTables) % 16 == 0, "tables are copied in words");
 
-// kRebuild only, in shared memory of its own so that the other instantiations copy no more than before
+// kRebuild and kDecode only, in shared memory of its own so that the other instantiations copy no more than before
 struct RebuildTables {
     u8 logr[32 * 32];  // log R[r][j] at r*32 + j, kLogZero for a zero entry
 };
@@ -73,9 +77,10 @@ struct LocateParams {
     u32* pages;
     u64 page_words;
     u8* fix[SWEC_MAX_SHARDS];  // kCorrect: the k+m shards' bytes of these columns (fix[k+p] == stored[p]);
-                               // kRebuild: the nout rebuilt streams
-    int nout;                  // kRebuild: rebuilt streams
-    const u32* rtables;        // kRebuild: RebuildTables
+                               // kRebuild: the nout rebuilt streams; kDecode: those, then at fix[nout + j] the bytes of
+                               // information position j when it holds a data shard (NULL for a parity shard)
+    int nout;                  // kRebuild, kDecode: rebuilt streams
+    const u32* rtables;        // kRebuild, kDecode: RebuildTables
 };
 
 struct Run {  // columns one lane blamed on one set, in increasing offset order
@@ -234,15 +239,21 @@ __device__ __forceinline__ void propagate(const LocateParams& p, const LocateTab
     }
 }
 
+// kDecode: the error value e of information position j XORed into its own byte, when it holds a data shard
+__device__ __forceinline__ void restore(const LocateParams& p, int j, u8 e, u64 x) {
+    if (j >= p.k) return;
+    if (u8* d = p.fix[p.nout + j]) d[x] ^= e;
+}
+
 // column x of the launch (shard offset p.base + x); the correcting kernel XORs the error values into the shards, the
-// rebuilding kernel their images into the rebuilt streams
+// rebuilding kernel their images into the rebuilt streams, the decoding kernel both into the data shards
 template <int MODE>
 __device__ __forceinline__ void blame(const LocateParams& p, const LocateTables& t, const u8* logr, const u8* s, int m,
                                       u64 x, Run* run) {
     int a = -1, b = -1;
     u8 ea = 0, eb = 0;
     const u64 off = p.base + x;
-    const int found = (MODE == kRebuild && p.radius == 0)
+    const int found = ((MODE == kRebuild || MODE == kDecode) && p.radius == 0)
                           ? 0
                           : decode_column<MODE != kLocate>(t, s, p.k, m, p.radius, &a, &b, &ea, &eb);
     if (!found) {
@@ -251,11 +262,13 @@ __device__ __forceinline__ void blame(const LocateParams& p, const LocateTables&
     }
     record(p, run, a, off);
     if (MODE == kCorrect) p.fix[a][x] ^= ea;
-    if (MODE == kRebuild) propagate(p, t, logr, a, ea, x);
+    if (MODE == kRebuild || MODE == kDecode) propagate(p, t, logr, a, ea, x);
+    if (MODE == kDecode) restore(p, a, ea, x);
     if (found == 2) {
         record(p, run, b, off);
         if (MODE == kCorrect) p.fix[b][x] ^= eb;
-        if (MODE == kRebuild) propagate(p, t, logr, b, eb, x);
+        if (MODE == kRebuild || MODE == kDecode) propagate(p, t, logr, b, eb, x);
+        if (MODE == kDecode) restore(p, b, eb, x);
     }
 }
 
@@ -276,7 +289,8 @@ __device__ __forceinline__ uint4 xor4(const uint4& a, const uint4& b) {
 }
 
 // MT > 0: m known at compile time; 0: run-time m.  MODE: kLocate, kCorrect (fix every column decoded within the radius
-// in place) or kRebuild (take the errors of the information positions out of the rebuilt streams).  A column's bytes
+// in place), kRebuild (take the errors of the information positions out of the rebuilt streams) or kDecode (kRebuild,
+// and the errors of the information positions that hold data shards corrected in place too).  A column's bytes
 // are read and written only by the thread that owns its vector (or its byte in the tail loop).
 template <int MT, int MODE>
 __global__ void __launch_bounds__(256) swec_locate_kernel(const __grid_constant__ LocateParams p) {
@@ -284,7 +298,7 @@ __global__ void __launch_bounds__(256) swec_locate_kernel(const __grid_constant_
     __shared__ __align__(16) u32 words[kTableWords];
     for (int i = threadIdx.x; i < kTableWords; i += blockDim.x) words[i] = p.tables[i];
     const u8* logr = nullptr;
-    if constexpr (MODE == kRebuild) {
+    if constexpr (MODE == kRebuild || MODE == kDecode) {
         __shared__ __align__(16) u32 rwords[kRebuildWords];
         for (int i = threadIdx.x; i < kRebuildWords; i += blockDim.x) rwords[i] = p.rtables[i];
         logr = reinterpret_cast<const u8*>(rwords);
@@ -411,6 +425,20 @@ void unchecked_report(swec_damage_report* report, int* n_ranges) {
     if (n_ranges) *n_ranges = 0;
 }
 
+void drop_missing_parity(const uint8_t* present, int k, std::vector<int>* outs, Matrix* fused) {
+    std::vector<int> kept;
+    Matrix rows(0, fused->cols);
+    for (size_t o = 0; o < outs->size(); o++) {
+        const int id = (*outs)[o];
+        if (id >= k && !present[id]) continue;
+        kept.push_back(id);
+        rows.v.insert(rows.v.end(), fused->row(int(o)), fused->row(int(o)) + fused->cols);
+        rows.rows++;
+    }
+    *outs = kept;
+    *fused = rows;
+}
+
 DamageLocator::~DamageLocator() {
     if (rtables_) cudaFree(rtables_);
     if (tables_) cudaFree(tables_);
@@ -451,7 +479,7 @@ int DamageLocator::init(const Matrix& parity, int64_t shard_len, int radius, cud
 }
 
 int DamageLocator::init_rebuild(const Matrix& fused, const std::vector<int>& info, const std::vector<int>& outs,
-                                const uint8_t* present, int64_t shard_len, int radius, cudaStream_t s) {
+                                const uint8_t* present, int64_t shard_len, int radius, cudaStream_t s, bool decode) {
     const int k = fused.cols;
     std::vector<int> check;  // rows of `fused`
     out_rows_.clear();
@@ -463,6 +491,7 @@ int DamageLocator::init_rebuild(const Matrix& fused, const std::vector<int>& inf
     // the punctured code has distance c+1: radius t needs 2t <= c
     if (int rc = init(pc, shard_len, std::min(radius, c / 2), s)) return rc;
     rebuild_ = true;
+    decode_ = decode;
     check_rows_ = check;
     for (int j = 0; j < k; j++) ids_[size_t(j)] = info[size_t(j)];
     for (int i = 0; i < c; i++) ids_[size_t(k + i)] = outs[size_t(check[size_t(i)])];
@@ -493,6 +522,8 @@ int DamageLocator::launch(uint8_t* const* computed, uint8_t* const* shards, size
         p.nout = int(out_rows_.size());
         p.rtables = rtables_;
     }
+    if (decode_)  // nout + k <= k + m slots: the rebuilt streams are missing data shards
+        for (int j = 0; j < k_; j++) p.fix[p.nout + j] = ids_[size_t(j)] < k_ ? shards[j] : nullptr;
     p.n = n;
     p.base = u64(base);
     p.k = k_;
@@ -502,7 +533,11 @@ int DamageLocator::launch(uint8_t* const* computed, uint8_t* const* shards, size
     p.ctr = counters_;
     p.pages = pages_;
     p.page_words = page_words_;
-    if (rebuild_) {
+    if (decode_) {
+        if (m_ == 4) swec_locate_kernel<4, kDecode><<<locate_grid<4, kDecode>(n), 256, 0, s>>>(p);
+        else if (m_ == 3) swec_locate_kernel<3, kDecode><<<locate_grid<3, kDecode>(n), 256, 0, s>>>(p);
+        else swec_locate_kernel<0, kDecode><<<locate_grid<0, kDecode>(n), 256, 0, s>>>(p);
+    } else if (rebuild_) {
         if (m_ == 3) swec_locate_kernel<3, kRebuild><<<locate_grid<3, kRebuild>(n), 256, 0, s>>>(p);
         else swec_locate_kernel<0, kRebuild><<<locate_grid<0, kRebuild>(n), 256, 0, s>>>(p);
     } else if (correct_) {

@@ -22,6 +22,9 @@ int check_locate_args(int m, int radius, const swec_damage_report* report, const
 int check_rebuild_args(int radius, const swec_damage_report* report, const swec_damage_range* ranges, int ranges_cap);
 // The report of a set where nothing could be checked: no columns, no shards, no ranges (n_ranges may be NULL).
 void unchecked_report(swec_damage_report* report, int* n_ranges);
+// ec.decode's plan from rs_reconstruct_plan's: the entries of `outs` that are missing parity shards, and their rows of
+// `fused`, removed, so that one apply rebuilds only the missing data shards and re-encodes the present check shards.
+void drop_missing_parity(const uint8_t* present, int k, std::vector<int>* outs, Matrix* fused);
 
 // Accumulates, over any number of launches, the shards blamed for every byte column of a shard set whose syndrome
 // (computed parity XOR stored parity) is not zero.  Device memory lives on the device current at init().
@@ -41,14 +44,17 @@ class DamageLocator {
     // check shards; the code punctured to info + check has distance c+1, so the radius is clamped to c/2, and 0
     // decodes nothing.  Launches also take the errors of the information shards they locate out of the missing shards'
     // rows.  The report and ranges name shard ids; check ids exceed information ids, so ranges stay in ascending id.
+    // decode: `outs` holds only missing data shards and check shards (every check shard is then a parity shard), and
+    // launches also correct the errors they locate in information shards that are data shards, in place.
     int init_rebuild(const Matrix& fused, const std::vector<int>& info, const std::vector<int>& outs,
-                     const uint8_t* present, int64_t shard_len, int radius, cudaStream_t s);
+                     const uint8_t* present, int64_t shard_len, int radius, cudaStream_t s, bool decode = false);
     bool correcting() const { return correct_; }
     // Columns [base, base + n) of the set: computed[p] is the parity re-encoded from the data shards, shards[0..k+m) the
     // shards as found (stored parity at shards[k+p]).  The shards are only read unless correcting; a correcting launch
     // must come after the encode that read the data shards, in stream order.  Asynchronous on `s`.
     // Rebuild mode: computed[o] is row o of `fused`, shards[0..k) the information shards and shards[k..k+c) the check
     // shards in ascending id; only the rows of missing shards in `computed` are written, after the apply that made them.
+    // Decode mode also writes shards[j] of the information shards that are data shards.
     int launch(uint8_t* const* computed, uint8_t* const* shards, size_t n, int64_t base, cudaStream_t s);
     // After every launch has completed: the report, the page ranges (first ranges_cap of them) and their total; `all`
     // (may be NULL) receives every range.
@@ -57,7 +63,7 @@ class DamageLocator {
 
   private:
     int k_ = 0, m_ = 0, radius_ = 1;  // m_: check positions (c in rebuild mode)
-    bool correct_ = false, rebuild_ = false;
+    bool correct_ = false, rebuild_ = false, decode_ = false;
     std::vector<int> ids_;                   // shard id of every kernel position, ascending
     std::vector<int> check_rows_, out_rows_;  // rebuild mode: rows of `computed` that are check shards / rebuilt shards
     int64_t shard_len_ = 0;

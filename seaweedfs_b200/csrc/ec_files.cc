@@ -823,6 +823,96 @@ int rebuild_files(const char* base, const char* const* dirs, int ndirs, int k, i
     return SWEC_OK;
 }
 
+// The checked decode's pipeline over columns [0, cols) of the shards.  Its items follow swec_write_dat_file's copy
+// plan: rows of large blocks cut at the slot size, then the small rows, several to a slot as in swec_generate_ec_files,
+// the ragged tail row last; no item straddles a row boundary.  Each item reads the k information and c check streams.
+// One apply of the rows of the missing data shards and of the check shards, then the decoding locator (c >= 1), which
+// corrects the information streams that are data shards in the slot and the rebuilt rows.  The item's writes un-stripe
+// the k data streams into the .dat at the plan's offsets.
+int decode_dat(swec_encoder* enc, const std::vector<int>& in, const std::vector<int>& in_d,
+               const std::vector<uint8_t>& present, int dat, int dat_d, const StripeGeometry& g, int64_t dat_size,
+               int64_t cols, Checked* chk) {
+    const int k = enc->k, total = enc->k + enc->m;
+    std::vector<uint8_t> info(static_cast<size_t>(total), 0);
+    for (int i = 0, n = 0; i < total && n < k; i++)
+        if (present[size_t(i)]) info[size_t(i)] = 1, n++;
+    std::vector<int> ins, outs;  // outs: the missing data shards and the check shards, ascending, one row of `fused` each
+    Matrix fused;
+    if (!rs_reconstruct_plan(enc->gen, k, info.data(), false, &ins, &outs, &fused))
+        return fail(SWEC_ERR_TOO_FEW_SHARDS, "not enough shards");
+    drop_missing_parity(present.data(), k, &outs, &fused);
+    std::vector<int> checks;                           // check shard ids, ascending: streams k .. k+c of a slot
+    std::vector<int> stream(static_cast<size_t>(k));   // the slot stream that holds data shard s
+    for (int j = 0; j < k; j++)
+        if (ins[size_t(j)] < k) stream[size_t(ins[size_t(j)])] = j;
+    for (int id : outs)
+        if (present[size_t(id)]) checks.push_back(id);
+    const int c = int(checks.size());
+    for (size_t o = 0; o < outs.size(); o++)  // computed row o is stream k + c + o
+        if (!present[size_t(outs[o])]) stream[size_t(outs[o])] = k + c + int(o);
+    const size_t chunk = file_chunk(cols);
+    DamageLocator locator;
+    FilePipeline pipe(enc, fused, chunk, /*verify=*/c > 0, c > 0 ? &locator : nullptr, /*stored=*/c);
+    int rc = pipe.start();
+    if (rc) return rc;
+    if (c > 0 && (rc = locator.init_rebuild(fused, ins, outs, present.data(), cols, chk->radius, enc->stream, /*decode=*/true)))
+        return rc;
+    reserve_extents(std::vector<int>{dat}, dat_size);
+    // columns [o, o + len) of a row whose blocks start at .dat offset row_dat, `block` bytes apart, taken from offset
+    // src of the item's streams; shard s holds tail_bytes(s) of the tail row
+    auto unstripe = [&](Item& it, int64_t row_dat, int64_t block, bool tail, int64_t o, int64_t len, size_t src) {
+        for (int s = 0; s < k; s++) {
+            const int64_t n = std::min(len, (tail ? g.tail_bytes(s) : block) - o);
+            if (n > 0) it.writes.push_back({stream[size_t(s)], dat, row_dat + int64_t(s) * block + o, src, size_t(n), dat_d});
+        }
+    };
+    auto submit = [&](Item&& it, int64_t col) -> int {
+        it.shard_off = col;
+        for (int i = 0; i < k; i++)
+            it.reads.push_back({i, in[size_t(ins[size_t(i)])], col, 0, it.len, in_d[size_t(ins[size_t(i)])]});
+        for (int i = 0; i < c; i++)
+            it.reads.push_back({k + i, in[size_t(checks[size_t(i)])], col, 0, it.len, in_d[size_t(checks[size_t(i)])]});
+        return pipe.submit(std::move(it));
+    };
+    for (int64_t r = 0; rc == SWEC_OK && r < g.large_rows; r++)
+        for (int64_t o = 0; rc == SWEC_OK && o < g.large; o += int64_t(chunk)) {
+            Item it;
+            it.len = size_t(std::min<int64_t>(int64_t(chunk), g.large - o));
+            unstripe(it, r * g.large_row(), g.large, false, o, int64_t(it.len), 0);
+            rc = submit(std::move(it), r * g.large + o);
+        }
+    // the small rows, then the tail row, whose columns are the ones shard 0 gives it
+    const int64_t nrows = g.small_rows + (g.tail > 0 ? 1 : 0);
+    auto width = [&](int64_t j) { return j < g.small_rows ? g.small : g.tail_bytes(0); };
+    auto row_dat = [&](int64_t j) { return g.small_dat_offset() + j * g.small_row(); };
+    int64_t j = 0;
+    for (; rc == SWEC_OK && j < nrows && g.small > int64_t(chunk); j++)  // small blocks bigger than a slot: row by row
+        for (int64_t o = 0; rc == SWEC_OK && o < width(j); o += int64_t(chunk)) {
+            Item it;
+            it.len = size_t(std::min<int64_t>(int64_t(chunk), width(j) - o));
+            unstripe(it, row_dat(j), g.small, j == g.small_rows, o, int64_t(it.len), 0);
+            rc = submit(std::move(it), g.small_shard_offset() + j * g.small + o);
+        }
+    const int64_t rows_per_item = std::max<int64_t>(1, int64_t(chunk) / g.small);
+    while (rc == SWEC_OK && j < nrows) {
+        Item it;
+        const int64_t first = j;
+        for (; j < nrows && j - first < rows_per_item; j++) {
+            unstripe(it, row_dat(j), g.small, j == g.small_rows, 0, width(j), it.len);
+            it.len += size_t(width(j));
+        }
+        rc = submit(std::move(it), g.small_shard_offset() + first * g.small);
+    }
+    if ((rc = pipe.finish())) return rc;
+    if (c == 0) {  // exactly k shards present: rebuilt, not checked
+        unchecked_report(chk->report, chk->n_ranges);
+        return SWEC_OK;
+    }
+    if ((rc = locator.collect(chk->report, chk->ranges, chk->ranges_cap, chk->n_ranges))) return rc;
+    chk->checked = true;
+    return SWEC_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1060,6 +1150,70 @@ int swec_write_dat_file(const char* base, int64_t dat_size, const char* const* s
         return SWEC_OK;
     };
     return file_io_pool().parallel_for(int(pieces.size()), copy_piece) ? first.get() : SWEC_OK;
+}
+
+
+int swec_write_dat_file_checked(const char* base, int64_t dat_size, const char* const* names, int k, int m, int64_t large,
+                                int64_t small, int device, int radius, swec_damage_report* report,
+                                swec_damage_range* ranges, int ranges_cap, int* n_ranges, int* ok) {
+    if (!base || !names || !ok || k <= 0 || m <= 0 || k + m > SWEC_MAX_SHARDS || large <= 0 || small <= 0 || dat_size < 0)
+        return fail(SWEC_ERR_INVALID_ARG, "bad argument");
+    *ok = 0;
+    int rc = check_rebuild_args(radius, report, ranges, ranges_cap);
+    if (rc) return rc;
+    const int total = k + m;
+    FdSet fds;
+    const long direct = g_opt_file_direct_io.load();
+    std::vector<int> in(static_cast<size_t>(total), -1), in_d(static_cast<size_t>(total), -1);
+    std::vector<uint8_t> present(static_cast<size_t>(total), 0);
+    int npresent = 0;
+    for (int i = 0; i < total; i++) {
+        if (!names[i]) continue;
+        if ((in[size_t(i)] = fds.keep(open(names[i], O_RDONLY))) < 0) return io_fail(std::string("open ") + names[i]);
+        in_d[size_t(i)] = fds.keep(open_direct(names[i], O_RDONLY, direct & 1));
+        present[size_t(i)] = 1;
+        npresent++;
+    }
+    // every check before the .dat exists: enough shards, of one length, long enough for the copy plan
+    if (npresent < k)
+        return fail(SWEC_ERR_TOO_FEW_SHARDS, "not enough shards to decode " + std::string(base) + ": found " +
+                                                 std::to_string(npresent) + " shards, need at least " + std::to_string(k));
+    int64_t size = -1;
+    for (int fd : in)
+        if (fd >= 0 && (rc = check_length(fd, &size))) return rc;
+    const StripeGeometry g(dat_size, k, large, small);
+    for (int s = 0; s < k; s++)  // what the plan reads from shard s (ec_decoder.go:200-219); shard 0 reads the most
+        if (size < g.tail_shard_offset() + g.tail_bytes(s)) return fail(SWEC_ERR_IO, "short read copying shard " + std::to_string(s));
+    bool all_data = true;
+    for (int s = 0; s < k; s++) all_data = all_data && present[size_t(s)];
+    if (all_data && npresent == k) {  // the data shards alone: nothing to check, nothing to rebuild
+        unchecked_report(report, n_ranges);
+        return swec_write_dat_file(base, dat_size, names, k, large, small);
+    }
+    CallEncoder enc;
+    if ((rc = new_call_encoder(k, m, device, &enc))) return rc;
+    const std::string path = std::string(base) + ".dat";
+    const int dat = fds.keep(open(path.c_str(), O_WRONLY | O_CREAT | O_TRUNC, 0644));
+    if (dat < 0) return io_fail("cannot write volume .dat");
+    struct Undo {  // only a .dat decoded without uncorrectable columns stays
+        const std::string& path;
+        bool armed = true;
+        ~Undo() {
+            if (armed) unlink(path.c_str());
+        }
+    } undo{path};
+    const int dat_d = fds.keep(open_direct(path, O_WRONLY, direct & 2));
+    if (ftruncate(dat, off_t(dat_size)) != 0) return io_fail("size .dat");
+    Checked chk{radius, report, ranges, ranges_cap, n_ranges};
+    if ((rc = decode_dat(enc.get(), in, in_d, present, dat, dat_d, g, dat_size, g.tail_shard_offset() + g.tail_bytes(0), &chk)))
+        return rc;
+    if (chk.checked && report->uncorrectable_columns)
+        return fail(SWEC_ERR_UNCORRECTABLE, std::to_string(report->uncorrectable_columns) + " byte columns of " + std::string(base) +
+                                                " cannot be corrected, shard offsets " + std::to_string(report->first_uncorrectable) +
+                                                ".." + std::to_string(report->last_uncorrectable) + ": no .dat written");
+    undo.armed = false;
+    *ok = chk.checked ? 1 : 0;
+    return SWEC_OK;
 }
 
 }  // extern "C"

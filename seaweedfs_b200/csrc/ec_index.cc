@@ -236,9 +236,16 @@ int swec_find_dat_file_size(const char* data_base, const char* index_base, int64
     const ssize_t got = pread(fd, sb, sizeof sb, 0);
     close(fd);
     if (got != ssize_t(sizeof sb)) return fail(SWEC_ERR_IO, "cannot read the superblock from .ec00");
-    const int version = sb[0];
+    return swec::dat_file_size_from_ecx(index_base, sb[0], dat_size);
+}
+
+}  // extern "C"
+
+namespace swec {
+
+int dat_file_size_from_ecx(const std::string& index_base, int version, int64_t* dat_size) {
     std::vector<uint8_t> ecx;
-    if (!read_file(std::string(index_base) + ".ecx", &ecx)) return io_err(std::string("cannot open ec index ") + index_base + ".ecx");
+    if (!read_file(index_base + ".ecx", &ecx)) return io_err("cannot open ec index " + index_base + ".ecx");
     int64_t size = kSuperBlockSize;
     for (size_t off = 0; off + kIndexEntrySize <= ecx.size(); off += kIndexEntrySize) {
         const IndexEntry e = index_entry(&ecx[off]);
@@ -250,4 +257,4 @@ int swec_find_dat_file_size(const char* data_base, const char* index_base, int64
     return SWEC_OK;
 }
 
-}  // extern "C"
+}  // namespace swec

@@ -3,6 +3,7 @@
 //   swec_ec_shards_generate    VolumeEcShardsGenerate   weed/server/volume_grpc_erasure_coding.go:43-146
 //   swec_ec_shards_rebuild     VolumeEcShardsRebuild    weed/server/volume_grpc_erasure_coding.go:149-225
 //   swec_ec_shards_to_volume   VolumeEcShardsToVolume   weed/server/volume_grpc_erasure_coding.go:578-668
+//   swec_ec_shards_to_volume_checked   the same from any k shards, damaged data shards corrected on the GPU first
 //   swec_read_ec_needles       Store.ReadEcShardNeedle + readEcShardIntervals + readOneEcShardInterval +
 //                              recoverOneRemoteEcShardInterval, on local shard files, batched
 //                                                       weed/storage/store_ec.go:252-355,482-560
@@ -28,6 +29,7 @@
 #include <string>
 #include <vector>
 
+#include "damage.h"
 #include "engine.h"
 #include "mini_json.h"
 #include "needles.h"
@@ -178,6 +180,64 @@ int swec_ec_shards_to_volume(const char* data_base, const char* index_base, cons
     for (const auto& s : names) cnames.push_back(s.c_str());
     if ((rc = swec_write_dat_file(db.c_str(), size, cnames.data(), k, kLargeBlockSize, kSmallBlockSize))) return rc;
     if ((rc = swec_write_idx_file_from_ec_index(ib.c_str()))) return rc;
+    if (dat_file_size) *dat_file_size = size;
+    return SWEC_OK;
+}
+
+// swec_ec_shards_to_volume from any k of the k+m shards, through swec_write_dat_file_checked: the data shards are
+// corrected (or rebuilt) on the GPU before the .dat is written, and a volume left with uncorrectable columns gets
+// neither .dat nor .idx, so the caller keeps its EC shards.
+int swec_ec_shards_to_volume_checked(const char* data_base, const char* index_base, const char* const* additional_dirs,
+                                     int n_additional_dirs, int device, int radius, int64_t* dat_file_size,
+                                     swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges,
+                                     int* ok) {
+    if (!data_base || !ok || (n_additional_dirs > 0 && !additional_dirs)) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
+    *ok = 0;
+    if (const int rc = check_rebuild_args(radius, report, ranges, ranges_cap)) return rc;
+    const std::string db(data_base);
+    int k, m;
+    ec_ratio(db, &k, &m);
+    std::vector<std::string> names(size_t(k + m));
+    int found = 0;
+    for (int i = 0; i < k + m; i++) {
+        names[size_t(i)] = find_shard_file(db, additional_dirs, n_additional_dirs, i);
+        found += names[size_t(i)].empty() ? 0 : 1;
+    }
+    if (found < k)
+        return fail(SWEC_ERR_TOO_FEW_SHARDS, "ec volume " + db + " has " + std::to_string(found) + " of its " +
+                                                 std::to_string(k + m) + " shards, needs at least " + std::to_string(k));
+    std::string ib(index_base && *index_base ? index_base : data_base);
+    if (!is_file(ib + ".ecx")) ib = db;
+    // FindDatFileSize reads the needle version from .ec00's superblock; without .ec00, .vif keeps it.  Known before
+    // anything is written.
+    int64_t vif_version = 0;
+    if (names[0].empty()) {
+        std::vector<uint8_t> raw;
+        if (read_file(db + ".vif", &raw) || read_file(ib + ".vif", &raw))
+            if (!vif_number(std::string(raw.begin(), raw.end()), "version", &vif_version)) vif_version = 0;
+        if (vif_version <= 0)
+            return fail(SWEC_ERR_TOO_FEW_SHARDS, "ec volume " + db + " has no .ec00 and no needle version in its .vif");
+    }
+    int rc = swec_rebuild_ecx_file(ib.c_str());  // fold .ecj first so deleted needles are not counted live
+    if (rc) return rc;
+    int live = 0;
+    if ((rc = swec_has_live_needles(ib.c_str(), &live))) return rc;
+    if (!live) return fail(SWEC_ERR_NO_LIVE_NEEDLES, "ec volume has no live entries");  // EcNoLiveEntriesSubstring
+    int64_t size = 0;
+    if (names[0].empty()) rc = dat_file_size_from_ecx(ib, int(vif_version), &size);
+    else rc = swec_find_dat_file_size(names[0].substr(0, names[0].size() - 5).c_str(), ib.c_str(), &size);
+    if (rc) return rc;
+    std::vector<const char*> cnames;
+    for (const auto& s : names) cnames.push_back(s.empty() ? nullptr : s.c_str());
+    if ((rc = swec_write_dat_file_checked(db.c_str(), size, cnames.data(), k, m, kLargeBlockSize, kSmallBlockSize, device,
+                                          radius, report, ranges, ranges_cap, n_ranges, ok)))
+        return rc;
+    if ((rc = swec_write_idx_file_from_ec_index(ib.c_str()))) {
+        *ok = 0;
+        unlink((db + ".dat").c_str());
+        unlink((ib + ".idx").c_str());
+        return rc;
+    }
     if (dat_file_size) *dat_file_size = size;
     return SWEC_OK;
 }

@@ -300,6 +300,7 @@ const char* swec_strerror(int status) {
         case SWEC_ERR_NO_LIVE_NEEDLES: return "ec volume has no live entries";
         case SWEC_ERR_NOT_FOUND: return "needle not found";
         case SWEC_ERR_DELETED: return "needle already deleted";
+        case SWEC_ERR_UNCORRECTABLE: return "damage that cannot be corrected remains";
         default: return "unknown error";
     }
 }
@@ -826,12 +827,18 @@ int swec_correct_damage_device(swec_encoder* e, void* const* shards, size_t n, i
     return damage_device(e, shards, n, radius, true, report, ranges, ranges_cap, n_ranges, stream);
 }
 
-// The first k present shards are the information set; the other c present shards are re-encoded from it into scratch
-// and checked, and the missing shards are rebuilt into the caller's buffers by the same apply, then cleared of the
-// errors the locator finds in the information set.  Present shards are only read.
-int swec_reconstruct_checked_device(swec_encoder* e, void* const* shards, const uint8_t* present, size_t n, int radius,
-                                    swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges,
-                                    void* stream) {
+}  // extern "C"
+
+namespace {
+
+// swec_reconstruct_checked_device, and with `decode` swec_decode_data_checked_device.  The first k present shards are
+// the information set; the other c present shards are re-encoded from it into scratch and checked, and the missing
+// shards are rebuilt into the caller's buffers by the same apply, then cleared of the errors the locator finds in the
+// information set.  The rebuild reads every present shard and rebuilds every missing one.  The decode rebuilds only the
+// missing data shards and also corrects the present data shards in place; parity shards are only read, and a missing
+// one needs no buffer.
+int checked_device(swec_encoder* e, void* const* shards, const uint8_t* present, size_t n, int radius, bool decode,
+                   swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges, void* stream) {
     if (!e || !shards || !present) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
     int rc = check_rebuild_args(radius, report, ranges, ranges_cap);
     if (rc) return rc;
@@ -842,11 +849,13 @@ int swec_reconstruct_checked_device(swec_encoder* e, void* const* shards, const 
         if (present[i] && npresent++ < k) info[size_t(i)] = 1;
     if (npresent < k) return fail(SWEC_ERR_TOO_FEW_SHARDS, "fewer than data_shards shards present");
     for (int i = 0; i < total; i++)
-        if (!shards[i]) return fail(SWEC_ERR_INVALID_ARG, present[i] ? "NULL shard" : "missing shard has no buffer");
-    std::vector<int> ins, outs;  // outs: every shard outside the information set, ascending, one row of `fused` each
+        if (!shards[i] && (present[i] || i < k || !decode))
+            return fail(SWEC_ERR_INVALID_ARG, present[i] ? "NULL shard" : "missing shard has no buffer");
+    std::vector<int> ins, outs;  // outs: the shards outside the information set, ascending, one row of `fused` each
     Matrix fused;
     if (!rs_reconstruct_plan(e->gen, k, info.data(), false, &ins, &outs, &fused))
         return fail(SWEC_ERR_TOO_FEW_SHARDS, "fewer than data_shards shards present");
+    if (decode) drop_missing_parity(present, k, &outs, &fused);
     std::vector<int> checks;
     for (int id : outs)
         if (present[id]) checks.push_back(id);
@@ -856,12 +865,12 @@ int swec_reconstruct_checked_device(swec_encoder* e, void* const* shards, const 
     if ((rc = e->ensure_device())) return rc;
     cudaStream_t s = pick_stream(e, stream);
     DamageLocator locator;
-    if (c > 0 && (rc = locator.init_rebuild(fused, ins, outs, present, int64_t(n), radius, s))) return rc;
+    if (c > 0 && (rc = locator.init_rebuild(fused, ins, outs, present, int64_t(n), radius, s, decode))) return rc;
     // the computed check rows go to scratch a piece at a time, as in damage_device
     const size_t piece = std::min(n, size_t(256) << 20);
     StreamScratch scratch(s);
     if (piece && c > 0) SWEC_CUDA(scratch.alloc(size_t(c) * piece));
-    for (size_t off = 0; off < n; off += piece) {
+    for (size_t off = 0; off < n && !outs.empty(); off += piece) {
         const size_t len = std::min(piece, n - off);
         const uint8_t* in[SWEC_MAX_SHARDS];
         uint8_t* at[SWEC_MAX_SHARDS];  // information shards, then stored check shards
@@ -879,6 +888,22 @@ int swec_reconstruct_checked_device(swec_encoder* e, void* const* shards, const 
         return SWEC_OK;
     }
     return locator.collect(report, ranges, ranges_cap, n_ranges);
+}
+
+}  // namespace
+
+extern "C" {
+
+int swec_reconstruct_checked_device(swec_encoder* e, void* const* shards, const uint8_t* present, size_t n, int radius,
+                                    swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges,
+                                    void* stream) {
+    return checked_device(e, shards, present, n, radius, false, report, ranges, ranges_cap, n_ranges, stream);
+}
+
+int swec_decode_data_checked_device(swec_encoder* e, void* const* shards, const uint8_t* present, size_t n, int radius,
+                                    swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges,
+                                    void* stream) {
+    return checked_device(e, shards, present, n, radius, true, report, ranges, ranges_cap, n_ranges, stream);
 }
 
 int swec_stream_synchronize(swec_encoder* e, void* stream) {

@@ -100,4 +100,8 @@ std::vector<uint64_t> ecj_ids(const std::vector<uint8_t>& ecj);
 
 bool read_file(const std::string& path, std::vector<uint8_t>* out);  // the whole file; false when it cannot be opened
 
+// FindDatFileSize (ec_decoder.go:113-135) with the needle version given: the end of the furthest live needle of
+// <index_base>.ecx, at least the superblock
+int dat_file_size_from_ecx(const std::string& index_base, int version, int64_t* dat_size);
+
 }  // namespace swec

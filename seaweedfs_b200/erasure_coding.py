@@ -206,6 +206,18 @@ class Encoder:
                                                     C.byref(report), ranges, max_ranges, C.byref(n), stream))
         return _damage_result(report, ranges, n.value, max_ranges)
 
+    def decode_data_checked_device(self, shard_ptrs, present, shard_len: int, radius: int = 1, max_ranges: int = 4096,
+                                   stream: int = 0) -> dict:
+        """reconstruct_checked_device for ec.decode (swec_decode_data_checked_device): the present data shards are
+        corrected in place and the missing data shards rebuilt, from any k present shards; parity shards are only read
+        and a missing one may be None.  Returns the report of reconstruct_checked_device for the same shards; radius 0
+        only detects (include/swec.h)."""
+        pres = np.ascontiguousarray(np.asarray(present, dtype=np.uint8))
+        report, ranges, n = DamageReport(), (DamageRange * max(1, max_ranges))(), C.c_int(0)
+        check(lib().swec_decode_data_checked_device(self._h, _ptrs(shard_ptrs), pres.ctypes.data, shard_len, radius,
+                                                    C.byref(report), ranges, max_ranges, C.byref(n), stream))
+        return _damage_result(report, ranges, n.value, max_ranges)
+
     def synchronize(self, stream: int = 0) -> None:
         check(lib().swec_stream_synchronize(self._h, stream))
 
@@ -364,6 +376,32 @@ def rebuild_ec_files_checked(base_file_name: str, additional_dirs: list[str] | N
     return {"rebuilt": list(ids[: n_ids.value]), "ok": bool(ok.value), **_damage_result(report, ranges, n.value, max_ranges)}
 
 
+def _check_decoded(status: int, report, ranges, n_ranges: int, max_ranges: int) -> None:
+    """check(), but a SWEC_ERR_UNCORRECTABLE error carries the report as .report"""
+    if STATUS.get(status) == "SWEC_ERR_UNCORRECTABLE":
+        err = SwecError(status, lib().swec_last_error().decode(errors="replace"))
+        err.report = _damage_result(report, ranges, n_ranges, max_ranges)
+        raise err
+    check(status)
+
+
+def write_dat_file_checked(base_file_name: str, dat_file_size: int, shard_file_names: list, data_shards: int = DataShardsCount,
+                           parity_shards: int = ParityShardsCount, large_block: int = ErasureCodingLargeBlockSize,
+                           small_block: int = ErasureCodingSmallBlockSize, device: int = 0, radius: int = 1,
+                           max_ranges: int = 4096) -> dict:
+    """write_dat_file from any k of the k+m shards (swec_write_dat_file_checked): shard_file_names has k+m entries, None
+    for a missing shard.  Damaged data shards are corrected, and missing ones rebuilt, on the GPU before the .dat is
+    written.  Returns "dat_file_size", "ok" (True iff something could be checked and nothing is uncorrectable) and the
+    report of rebuild_ec_files_checked.  Uncorrectable columns raise SwecError(SWEC_ERR_UNCORRECTABLE), with the report
+    in its .report, and leave no .dat (include/swec.h)."""
+    names = (C.c_char_p * len(shard_file_names))(*[s.encode() if s else None for s in shard_file_names])
+    report, ranges, n, ok = DamageReport(), (DamageRange * max(1, max_ranges))(), C.c_int(0), C.c_int(0)
+    _check_decoded(lib().swec_write_dat_file_checked(base_file_name.encode(), dat_file_size, names, data_shards, parity_shards,
+                                                     large_block, small_block, device, radius, C.byref(report), ranges,
+                                                     max_ranges, C.byref(n), C.byref(ok)), report, ranges, n.value, max_ranges)
+    return {"dat_file_size": dat_file_size, "ok": bool(ok.value), **_damage_result(report, ranges, n.value, max_ranges)}
+
+
 def write_dat_file(base_file_name: str, dat_file_size: int, shard_file_names: list[str],
                    data_shards: int = DataShardsCount, large_block: int = ErasureCodingLargeBlockSize,
                    small_block: int = ErasureCodingSmallBlockSize) -> None:
@@ -405,6 +443,23 @@ def volume_ec_shards_to_volume(data_base_file_name: str, index_base_file_name: s
     check(lib().swec_ec_shards_to_volume(data_base_file_name.encode(), (index_base_file_name or "").encode(),
                                          arr, n, C.byref(size)))
     return int(size.value)
+
+
+def ec_shards_to_volume_checked(data_base_file_name: str, index_base_file_name: str | None = None,
+                                additional_dirs: list[str] | None = None, device: int = 0, radius: int = 1,
+                                max_ranges: int = 4096) -> dict:
+    """volume_ec_shards_to_volume from any k of the k+m shards, correcting damaged data shards on the GPU before the
+    .dat is written (swec_ec_shards_to_volume_checked).  Returns "dat_file_size", "ok" and the report, as
+    write_dat_file_checked does; uncorrectable columns raise SwecError(SWEC_ERR_UNCORRECTABLE) with .report and leave
+    neither .dat nor .idx, so the EC shards should be kept."""
+    arr, nd = _dirs(additional_dirs)
+    size = C.c_int64(0)
+    report, ranges, n, ok = DamageReport(), (DamageRange * max(1, max_ranges))(), C.c_int(0), C.c_int(0)
+    _check_decoded(lib().swec_ec_shards_to_volume_checked(data_base_file_name.encode(), (index_base_file_name or "").encode(),
+                                                          arr, nd, device, radius, C.byref(size), C.byref(report), ranges,
+                                                          max_ranges, C.byref(n), C.byref(ok)), report, ranges, n.value,
+                   max_ranges)
+    return {"dat_file_size": int(size.value), "ok": bool(ok.value), **_damage_result(report, ranges, n.value, max_ranges)}
 
 
 def _needle_reads(needle_ids, capacity, sizes=None):
