@@ -102,8 +102,9 @@ uint64_t swec_kernel_launches(void);          /* kernels this process has launch
  * memory over PCIe instead of staging through HBM}, "file_direct_io" {bit 0: O_DIRECT reads, bit 1: O_DIRECT writes in
  * the file-level entry points}.  Measurement knobs: "xt_variant" {0..3} (instruction mix of run-time specialised kernels,
  * device_common.cuh), "use_aot" {0,1} (0: RS(10,4) encode is specialised at run time like any matrix), "jit_share_powers"
- * {0,1} (1: run-time specialised kernels are generated with shared power chains — fewer multiply-by-2 steps; CPU-verified,
- * not yet measured on a GPU, hence off).                                                                           */
+ * {0,1} (1: run-time specialised kernels are generated with shared power chains — fewer multiply-by-2 steps; bytes
+ * checked on the GPU, speed not yet measured, hence off).  Changing any of enc_threads, enc_unroll, xt_variant,
+ * power_mode or jit_share_powers makes later calls use (and if needed compile) the kernel of the new setting. */
 int swec_set_option(const char *name, long value);
 /* Diagnostics: generate and NVRTC-compile (sm_90a) the specialised kernel for an r×k matrix without
  * loading it — needs no GPU.  Reports the cubin size and the generator's instruction statistics.  */
@@ -215,7 +216,8 @@ int swec_rebuild_ec_files(const char *base_file_name, const char *const *additio
 /* Scrub: re-encode .ec00–.ec(k-1) on the GPU and compare with the parity shards on disk (the Rust
  * twin's verify_ec_shards, seaweed-volume/src/storage/erasure_coding/ec_encoder.rs:177-278; the Go
  * scrub never checks parity, ec_volume_scrub.go:27-118).  mismatched_vectors[p] (m entries, may be
- * NULL) = number of differing 16-byte vectors in parity shard p; *ok = 1 iff all are zero.       */
+ * NULL) = number of differing 16-byte vectors in parity shard p, the partial last vector of a length
+ * that is not a multiple of 16 counting as one; *ok = 1 iff all are zero.                          */
 int swec_verify_ec_files(const char *base_file_name, const char *const *additional_dirs,
                          int n_additional_dirs, int data_shards, int parity_shards, int device,
                          uint64_t *mismatched_vectors, int *ok);

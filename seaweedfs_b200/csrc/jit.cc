@@ -97,6 +97,7 @@ struct JitRequest {
     Matrix rows;
     std::vector<uint8_t> key;
     int threads, unroll, device, variant;
+    bool share_powers;
 };
 // Process-wide state.  Deliberately leaked (never destroyed): the compiler thread may still be
 // finishing when static destructors run at process exit and must find the map and mutex alive.
@@ -115,7 +116,7 @@ JitGlobal& G() {
 constexpr int kHotUses = 1;        // a matrix is worth a background compile from its first short use
 constexpr size_t kMaxQueued = 16;  // beyond that the table kernel keeps serving
 
-std::shared_ptr<JitKernel> build_kernel(const Matrix& rows, int threads, int unroll, int variant);
+std::shared_ptr<JitKernel> build_kernel(const Matrix& rows, int threads, int unroll, int variant, bool share_powers);
 
 void jit_worker_loop() {
     JitGlobal& g = G();
@@ -128,7 +129,7 @@ void jit_worker_loop() {
         g.cache[rq.key].state = JitEntry::kCompiling;
         lock.unlock();
         cudaSetDevice(rq.device);
-        auto k = build_kernel(rq.rows, rq.threads, rq.unroll, rq.variant);
+        auto k = build_kernel(rq.rows, rq.threads, rq.unroll, rq.variant, rq.share_powers);
         lock.lock();
         g.cache[rq.key].kernel = k;
         g.cache[rq.key].state = k ? JitEntry::kReady : JitEntry::kFailed;
@@ -152,14 +153,17 @@ void jit_stop_at_exit() {
 
 void jit_shutdown() { jit_stop_at_exit(); }
 
-static std::vector<uint8_t> jit_key(const Matrix& rows, int threads, int unroll, int variant) {
-    std::vector<uint8_t> key{uint8_t(rows.rows), uint8_t(rows.cols), uint8_t(threads / 64), uint8_t(unroll), uint8_t(variant)};
+// everything the generated source depends on besides the matrix: a kernel cached under one key is the kernel of those options
+static std::vector<uint8_t> jit_key(const Matrix& rows, int threads, int unroll, int variant, bool share_powers) {
+    std::vector<uint8_t> key{uint8_t(rows.rows), uint8_t(rows.cols), uint8_t(threads / 64), uint8_t(unroll), uint8_t(variant),
+                             uint8_t(share_powers)};
     key.insert(key.end(), rows.v.begin(), rows.v.end());
     return key;
 }
 
 bool jit_cached(swec_encoder_impl* enc, const Matrix& rows) {
-    return enc->jit.count(jit_key(rows, int(g_opt_enc_threads.load()), int(g_opt_enc_unroll.load()), effective_xt_variant())) != 0;
+    return enc->jit.count(jit_key(rows, int(g_opt_enc_threads.load()), int(g_opt_enc_unroll.load()), effective_xt_variant(),
+                                  g_opt_jit_share_powers.load() != 0)) != 0;
 }
 
 // ---- on-disk cubin cache -------------------------------------------------------------------------------------
@@ -235,12 +239,12 @@ unsigned long long jit_disk_hit_count() { return g_jit_disk_hits.load(); }
 bool jit_available() { return nvrtc().ok || !disk_cache_dir().empty(); }
 
 // the complete source of the two specialised kernels for `rows` (also the identity of the cached cubin)
-static std::string jit_source(const Matrix& rows, int threads, int unroll, int variant, CodegenStats* stats) {
+static std::string jit_source(const Matrix& rows, int threads, int unroll, int variant, bool share_powers, CodegenStats* stats) {
     const std::string T = std::to_string(threads), U = std::to_string(unroll);
     std::string src = "#define SWEC_XT_VARIANT " + std::to_string(variant) + "\n";
     src += kDeviceCommonSrc;
     CodegenOptions copt;
-    copt.share_powers = g_opt_jit_share_powers.load() != 0;  // off by default (kernels.h); the source text keys the cubin cache
+    copt.share_powers = share_powers;  // off by default (kernels.h); the source text keys the cubin cache
     src += generate_combine(rows, "SwecJit", copt, stats);
     src +=
         "extern \"C\" __global__ void __launch_bounds__(" + T + ") swec_jit_flat(const __grid_constant__ SwecApplyParams p) {\n"
@@ -252,10 +256,11 @@ static std::string jit_source(const Matrix& rows, int threads, int unroll, int v
 
 // cubin for `rows`: from the disk cache when this exact source was compiled before (by any process), else NVRTC
 // (and into the cache).  No CUDA context needed.  *from_disk tells which.
-static int compile_cubin(const Matrix& rows, int threads, int unroll, int variant, std::vector<char>* cubin, CodegenStats* stats,
+static int compile_cubin(const Matrix& rows, int threads, int unroll, int variant, bool share_powers, std::vector<char>* cubin,
+                         CodegenStats* stats,
                          bool* from_disk = nullptr, std::string* disk_path = nullptr) {
     if (rows.rows > SWEC_MAX_OUTPUTS) return fail(SWEC_ERR_JIT, "too many output rows for one specialised kernel");
-    const std::string src = jit_source(rows, threads, unroll, variant, stats);
+    const std::string src = jit_source(rows, threads, unroll, variant, share_powers, stats);
     const std::string dir = disk_cache_dir(), name = dir.empty() ? "" : cache_name(src);
     if (from_disk) *from_disk = false;
     if (!dir.empty() && read_file(dir + "/" + name, cubin)) {
@@ -292,7 +297,7 @@ static int compile_cubin(const Matrix& rows, int threads, int unroll, int varian
 }
 
 namespace {
-std::shared_ptr<JitKernel> build_kernel(const Matrix& rows, int threads, int unroll, int variant) {
+std::shared_ptr<JitKernel> build_kernel(const Matrix& rows, int threads, int unroll, int variant, bool share_powers) {
     for (int attempt = 0; attempt < 2; attempt++) {
         auto kernel = std::make_shared<JitKernel>();
         kernel->threads = threads;
@@ -300,7 +305,8 @@ std::shared_ptr<JitKernel> build_kernel(const Matrix& rows, int threads, int unr
         std::vector<char> cubin;
         bool from_disk = false;
         std::string disk_path;
-        if (compile_cubin(rows, threads, unroll, variant, &cubin, &kernel->stats, &from_disk, &disk_path) != SWEC_OK) return nullptr;
+        if (compile_cubin(rows, threads, unroll, variant, share_powers, &cubin, &kernel->stats, &from_disk, &disk_path) != SWEC_OK)
+            return nullptr;
         cudaError_t e = cudaLibraryLoadData(&kernel->lib, cubin.data(), nullptr, nullptr, 0, nullptr, nullptr, 0);
         if (e == cudaSuccess) e = cudaLibraryGetKernel(&kernel->flat, kernel->lib, "swec_jit_flat");
         if (e == cudaSuccess) e = cudaLibraryGetKernel(&kernel->blocked, kernel->lib, "swec_jit_blocked");
@@ -324,7 +330,8 @@ std::shared_ptr<JitKernel> build_kernel(const Matrix& rows, int threads, int unr
 int jit_get(swec_encoder_impl* enc, const Matrix& rows, std::shared_ptr<JitKernel>* out, bool wait, bool hot) {
     const int threads = int(g_opt_enc_threads.load()), unroll = int(g_opt_enc_unroll.load());
     const int variant = effective_xt_variant();  // boost-clock or low-power step, by the device's recent load
-    const std::vector<uint8_t> key = jit_key(rows, threads, unroll, variant);
+    const bool share_powers = g_opt_jit_share_powers.load() != 0;  // read once: the key and a queued compile must agree
+    const std::vector<uint8_t> key = jit_key(rows, threads, unroll, variant, share_powers);
     *out = nullptr;
     auto local = enc->jit.find(key);
     if (local != enc->jit.end()) {
@@ -346,7 +353,7 @@ int jit_get(swec_encoder_impl* enc, const Matrix& rows, std::shared_ptr<JitKerne
                 int dev = 0;
                 cudaGetDevice(&dev);
                 e.state = JitEntry::kQueued;
-                g.queue.push_back({rows, key, threads, unroll, dev, variant});
+                g.queue.push_back({rows, key, threads, unroll, dev, variant, share_powers});
                 if (!g.worker_started) {
                     g.worker_started = true;
                     g.worker = std::thread(jit_worker_loop);
@@ -369,7 +376,7 @@ int jit_get(swec_encoder_impl* enc, const Matrix& rows, std::shared_ptr<JitKerne
         }
         e.state = JitEntry::kCompiling;
         lock.unlock();
-        auto k = build_kernel(rows, threads, unroll, variant);
+        auto k = build_kernel(rows, threads, unroll, variant, share_powers);
         lock.lock();
         JitEntry& e2 = g.cache[key];
         e2.kernel = k;
@@ -384,7 +391,8 @@ int jit_get(swec_encoder_impl* enc, const Matrix& rows, std::shared_ptr<JitKerne
 int jit_debug_compile(const Matrix& rows, size_t* cubin_bytes, int* xtime_steps, int* xor_ops) {
     std::vector<char> cubin;
     CodegenStats st;
-    const int rc = compile_cubin(rows, int(g_opt_enc_threads.load()), int(g_opt_enc_unroll.load()), effective_xt_variant(), &cubin, &st);
+    const int rc = compile_cubin(rows, int(g_opt_enc_threads.load()), int(g_opt_enc_unroll.load()), effective_xt_variant(),
+                                 g_opt_jit_share_powers.load() != 0, &cubin, &st);
     if (cubin_bytes) *cubin_bytes = cubin.size();
     if (xtime_steps) *xtime_steps = st.xtime_steps;
     if (xor_ops) *xor_ops = st.xor_ops;

@@ -199,18 +199,25 @@ __global__ void __launch_bounds__(256) swec_digest_kernel(const u8* __restrict__
     if ((threadIdx.x & 31) == 0) atomicAdd(reinterpret_cast<unsigned long long*>(out), sum);
 }
 
-// counts 16-byte vectors (and tail bytes) where a != b
+// counts 16-byte vectors where a != b; a partial last vector (nbytes % 16 bytes) is one vector, as is every vector of
+// an unaligned pair, which is compared byte by byte
 __global__ void __launch_bounds__(256) swec_compare_kernel(const u8* __restrict__ a, const u8* __restrict__ b,
                                                             u64 nbytes, unsigned long long* __restrict__ mismatches) {
     const u64 stride = (u64)gridDim.x * blockDim.x;
     const bool aligned = ((reinterpret_cast<unsigned long long>(a) | reinterpret_cast<unsigned long long>(b)) & 15) == 0;
-    const u64 nvec = aligned ? nbytes >> 4 : 0;
+    const u64 nvec = (nbytes + 15) >> 4;
     unsigned long long bad = 0;
     for (u64 v = (u64)blockIdx.x * blockDim.x + threadIdx.x; v < nvec; v += stride) {
-        const uint4 x = swec_ldg_stream(a + (v << 4)), y = swec_ldg_stream(b + (v << 4));
-        bad += ((x.x ^ y.x) | (x.y ^ y.y) | (x.z ^ y.z) | (x.w ^ y.w)) != 0;
+        const u64 off = v << 4;
+        if (aligned && off + 16 <= nbytes) {
+            const uint4 x = swec_ldg_stream(a + off), y = swec_ldg_stream(b + off);
+            bad += ((x.x ^ y.x) | (x.y ^ y.y) | (x.z ^ y.z) | (x.w ^ y.w)) != 0;
+        } else {
+            bool diff = false;
+            for (u64 x = off; x < nbytes && x < off + 16; x++) diff |= a[x] != b[x];
+            bad += diff;
+        }
     }
-    for (u64 x = (nvec << 4) + (u64)blockIdx.x * blockDim.x + threadIdx.x; x < nbytes; x += stride) bad += a[x] != b[x];
     if (bad) atomicAdd(mismatches, bad);
 }
 
@@ -395,7 +402,7 @@ cudaError_t launch_digest(const void* src, u64 nbytes, u64* out_dev, cudaStream_
 
 cudaError_t launch_compare(const void* a, const void* b, u64 nbytes, unsigned long long* out_dev, cudaStream_t s) {
     if (nbytes == 0) return cudaSuccess;
-    swec_compare_kernel<<<grid_for(nbytes / 16 + 1, 256, 8), 256, 0, s>>>(static_cast<const u8*>(a), static_cast<const u8*>(b), nbytes, out_dev);
+    swec_compare_kernel<<<grid_for((nbytes + 15) / 16, 256, 8), 256, 0, s>>>(static_cast<const u8*>(a), static_cast<const u8*>(b), nbytes, out_dev);
     g_kernel_launches++;
     return cudaGetLastError();
 }

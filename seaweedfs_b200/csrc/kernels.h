@@ -17,7 +17,8 @@ extern std::atomic<long> g_opt_enc_threads, g_opt_enc_unroll, g_opt_ctas_per_sm;
 // whether RS(10,4) encode takes the ahead-of-time kernel (1) or is specialised at run time like any matrix (0)
 extern std::atomic<long> g_opt_xt_variant, g_opt_use_aot;
 // measurement knob: run-time specialised kernels are generated with shared power chains (codegen.h share_powers): fewer
-// multiply-by-2 steps (RS(10,4) encode 24 -> 20, worst-case decode 27 -> 21); verified on the CPU, not yet measured on a GPU
+// multiply-by-2 steps (RS(10,4) encode 24 -> 20, worst-case decode 27 -> 21); bytes checked on the GPU
+// (tests/test_kernel_variants.py), speed not yet measured.  Part of the specialised kernel's cache key (jit.cc)
 extern std::atomic<long> g_opt_jit_share_powers;
 // Power policy (kernels.cu).  A GPU that encodes back to back for more than a few hundred ms can run into its power
 // cap and lower the SM clock; from then on the 4-instruction multiply-by-2 step (variant 2: fewer instructions, far
