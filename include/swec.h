@@ -73,6 +73,7 @@ typedef enum swec_status {
 } swec_status;
 
 typedef struct swec_encoder swec_encoder;
+typedef struct swec_ec_volume swec_ec_volume; /* a mounted EC volume (swec_ec_volume_open, below) */
 
 /* ---- library ------------------------------------------------------------------------------ */
 const char *swec_version(void);
@@ -292,6 +293,53 @@ int swec_repair_ec_damage(const char *base_file_name, const char *const *additio
 int swec_correct_damage_device(swec_encoder *enc, void *const *shards, size_t shard_len, int radius,
                                swec_damage_report *report, swec_damage_range *ranges, int ranges_cap,
                                int *n_ranges, void *stream);
+/* ---- which needles the located damage hits ---------------------------------------------------------------------------
+ * The locate calls, and per live record of the volume the bytes the damage hits.  Report, ranges and ok are byte for byte
+ * those of swec_locate_ec_damage / swec_locate_damage_device for the same shards and radius, with their argument rules.
+ * New rules, checked before any other (SWEC_ERR_INVALID_ARG): needles_cap not negative, needles NULL only when
+ * needles_cap is 0, unowned not NULL, records NULL only when n_records is 0.
+ * Every byte of a data shard is one .dat byte through the two-tier striping.  A live record owns the bytes [offset,
+ * offset + GetActualSize(size, version)); where records overlap (a corrupt .ecx), a byte belongs to the record with the
+ * greatest offset not above it (the later entry on a tie) if it lies inside that record, so every byte counts once.
+ *   - damaged: the locate decode blamed the byte's shard in its column.  A repair restores these bytes, within the
+ *     guarantee of the locate calls.
+ *   - uncorrectable: the byte's column is uncorrectable; each such column puts its k data bytes at risk.  A repair
+ *     leaves them as they are: the record has to come from another copy.
+ *   - Parity bytes are never attributed (they stay in report.shard_bytes).  Bytes no live record owns (superblock,
+ *     deleted records, gaps, the zero padding of the last row) go to unowned[0] (damaged) and unowned[1]
+ *     (uncorrectable).  So sum(damaged_bytes) + unowned[0] = sum over data shards of report.shard_bytes, and
+ *     sum(uncorrectable_bytes) + unowned[1] = k * report.uncorrectable_columns.
+ *   - The limit of the locate calls carries over: in a column with more than m-t wrong shards the blame, and with it
+ *     the attribution, can be wrong.
+ * Nothing is written: this only reports. */
+typedef struct swec_needle_damage {
+    uint64_t needle_id;            /* in (device call) / out (handle call)                                          */
+    int64_t offset;                /* byte offset of the record in the .dat                                         */
+    int32_t size;                  /* Size of the index entry                                                       */
+    uint32_t shard_mask;           /* out: bit i = data shard i holds a byte counted below                          */
+    uint64_t damaged_bytes;        /* out: record bytes located as wrong in their data shard (repair restores them,
+                                      within the guarantee of the locate calls)                                     */
+    uint64_t uncorrectable_bytes;  /* out: record bytes in uncorrectable columns (repair cannot restore them)        */
+} swec_needle_damage;
+/* Mounted volume: all k+m shards must be local.  Live records are the .ecx entries that are not deleted, minus the
+ * .ecj ids as the handle's reads see them (.ecj re-read when it moved), striped by the LocateData geometry of the reads
+ * (shard_dat_size, 1 GiB / 1 MiB).  needles[] receives the records with a non-zero count in ascending needle id, the
+ * first needles_cap of them; *n_needles is how many there are.  A clean set gives *n_needles = 0 after the locate pass
+ * alone.  Errors before any device work, in this order: the arguments; a shard that is not local
+ * SWEC_ERR_TOO_FEW_SHARDS; unequal shard lengths SWEC_ERR_SHARD_SIZE; a handle opened with device < 0
+ * SWEC_ERR_NO_DEVICE.  The shard files are only read.  Calls on one handle serialise.                              */
+int swec_ec_volume_locate_needle_damage(swec_ec_volume *vol, int radius, swec_damage_report *report,
+                                        swec_damage_range *ranges, int ranges_cap, int *n_ranges,
+                                        swec_needle_damage *needles, int needles_cap, int *n_needles,
+                                        uint64_t unowned[2], int *ok);
+/* Device level: shards[k+m] in HBM (only read), the image of a .dat of dat_size bytes striped as
+ * swec_encode_volume_device does with large_block / small_block.  records[n_records] holds needle_id, offset and size
+ * of every live record, sized as needle version 3; its out fields are filled for every entry, zero counts included
+ * (a negative size owns no bytes).  Scratch of (k+2m) x 256 MiB at most; synchronises `stream`.                     */
+int swec_locate_needle_damage_device(swec_encoder *enc, const void *const *shards, size_t shard_len, int64_t dat_size,
+                                     int64_t large_block, int64_t small_block, int radius, swec_needle_damage *records,
+                                     int n_records, swec_damage_report *report, swec_damage_range *ranges,
+                                     int ranges_cap, int *n_ranges, uint64_t unowned[2], void *stream);
 /* ---- checked rebuild: errors and erasures ---------------------------------------------------------------------------
  * swec_rebuild_ec_files reads only the first k present shards, so a wrong byte in one of them goes into every shard it
  * rebuilds.  The checked rebuild reads every present shard.  The first k present shards are the information set; the
@@ -429,7 +477,6 @@ int swec_read_ec_needles(const char *data_base_file_name, const char *index_base
  * (ratio / needle version / datFileSize from .vif, shard files opened, .ecx loaded, .ecj re-read when it
  * grows), read many times; the encoder behind the recoveries, its staging ring and its specialised kernels
  * live as long as the handle.  Calls on one handle serialise.  swec_read_ec_needles = open + read + close. */
-typedef struct swec_ec_volume swec_ec_volume;
 int swec_ec_volume_open(const char *data_base_file_name, const char *index_base_file_name,
                         const char *const *additional_dirs, int n_additional_dirs, int device,
                         swec_ec_volume **out);

@@ -459,6 +459,43 @@ func (v *swecEcVolume) ScrubLocal(volumeId uint32) (int64, []uint32, []error, er
 	return int64(entries), shards, errs, nil
 }
 
+// swecNeedleDamage is one needle that located damage hits: DamagedBytes a repair restores, UncorrectableBytes it
+// cannot (restore that needle from a replica or a backup).  ShardMask has bit i set for each data shard i holding a
+// counted byte.
+type swecNeedleDamage struct {
+	NeedleId           uint64
+	Offset             int64
+	Size               int32
+	ShardMask          uint32
+	DamagedBytes       uint64
+	UncorrectableBytes uint64
+}
+
+// LocateNeedleDamage runs in the scrub of a volume whose shards are all local, next to swecLocateEcDamage: it names the
+// live needles the located damage hits (ascending id, at most maxNeedles of them; total is how many there are), and
+// the damaged / uncorrectable bytes no live needle owns.  It only reads the shard files.  After swecRepairEcDamage, the
+// needles with UncorrectableBytes > 0 are the ones to restore from another copy.
+func (v *swecEcVolume) LocateNeedleDamage(radius int, maxNeedles int) (needles []swecNeedleDamage, total int, unowned [2]uint64, err error) {
+	var report C.swec_damage_report
+	var nRanges, nNeedles, ok C.int
+	var cUnowned [2]C.uint64_t
+	buf := make([]C.swec_needle_damage, maxNeedles+1)
+	if err := swecCall(func() C.int {
+		return C.swec_ec_volume_locate_needle_damage(v.h, C.int(radius), &report, nil, 0, &nRanges, &buf[0],
+			C.int(maxNeedles), &nNeedles, &cUnowned[0], &ok)
+	}); err != nil {
+		return nil, 0, unowned, fmt.Errorf("locate needle damage: %w", err)
+	}
+	total = int(nNeedles)
+	for i := 0; i < total && i < maxNeedles; i++ {
+		d := buf[i]
+		needles = append(needles, swecNeedleDamage{uint64(d.needle_id), int64(d.offset), int32(d.size), uint32(d.shard_mask),
+			uint64(d.damaged_bytes), uint64(d.uncorrectable_bytes)})
+	}
+	unowned = [2]uint64{uint64(cUnowned[0]), uint64(cUnowned[1])}
+	return needles, total, unowned, nil
+}
+
 // swecLocateEcDamage is the parity side of a scrub of a volume whose shards are all local, run before ec.rebuild: it
 // names the shard FILES that are wrong, where verify_ec_shards (seaweed-volume/src/storage/erasure_coding/
 // ec_encoder.rs:240-258) can only name the parity shards that disagree.  broken is ready to become EcShardInfos (delete

@@ -59,6 +59,11 @@ class DamageRange(C.Structure):
     _fields_ = [("shard_id", C.c_int32), ("reserved", C.c_int32), ("offset", C.c_int64), ("length", C.c_int64)]
 
 
+class NeedleDamage(C.Structure):
+    _fields_ = [("needle_id", C.c_uint64), ("offset", C.c_int64), ("size", C.c_int32), ("shard_mask", C.c_uint32),
+                ("damaged_bytes", C.c_uint64), ("uncorrectable_bytes", C.c_uint64)]
+
+
 NEEDLE_STATUS = {0: "ok", 1: "size mismatch", 2: "out of range", 3: "bad crc", 4: "outside image"}
 
 
@@ -113,6 +118,13 @@ PROTOTYPES = {
                                         C.POINTER(C.c_int)]),
     "swec_correct_damage_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.POINTER(DamageReport),
                                              C.POINTER(DamageRange), C.c_int, C.POINTER(C.c_int), C.c_void_p]),
+    "swec_ec_volume_locate_needle_damage": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(DamageReport), C.POINTER(DamageRange),
+                                                      C.c_int, C.POINTER(C.c_int), C.POINTER(NeedleDamage), C.c_int,
+                                                      C.POINTER(C.c_int), C.POINTER(C.c_uint64), C.POINTER(C.c_int)]),
+    "swec_locate_needle_damage_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int64, C.c_int64, C.c_int64,
+                                                   C.c_int, C.POINTER(NeedleDamage), C.c_int, C.POINTER(DamageReport),
+                                                   C.POINTER(DamageRange), C.c_int, C.POINTER(C.c_int),
+                                                   C.POINTER(C.c_uint64), C.c_void_p]),
     "swec_rebuild_ec_files_checked": (C.c_int, [C.c_char_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                                 C.c_void_p, C.POINTER(C.c_int), C.POINTER(DamageReport),
                                                 C.POINTER(DamageRange), C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),

@@ -30,6 +30,7 @@
 #include "damage.h"
 #include "engine.h"
 #include "io_pool.h"
+#include "needle_damage.h"
 #include "volume_format.h"
 
 namespace swec {
@@ -199,6 +200,10 @@ double reserve_extents(const std::vector<int>& outs, int64_t size) {
 class FilePipeline {
   public:
     PipeStats stats;
+    // With a locator: when set, called on each item in place of the locator's launch, with the computed rows, the
+    // slot's streams, the item's columns and the index of its slot, in the slot's stream order.
+    std::function<int(uint8_t* const* computed, uint8_t* const* shards, size_t len, int64_t base, int slot, cudaStream_t s)>
+        piece_fn;
     // verify = true: streams [K, K+S) are stored bytes read from disk (S = `stored`, R when negative); the R computed
     // rows go to streams [K+S, K+S+R) and are only compared on the device (no D2H, no writes) — counted per parity
     // stream, or, with a locator, decoded into the shards it blames.  A correcting locator also fixes those shards in
@@ -316,7 +321,9 @@ class FilePipeline {
         if (locator_) {
             uint8_t* shards[SWEC_MAX_SHARDS];
             for (int i = 0; i < K + stored_; i++) shards[i] = b.dev + size_t(i) * chunk_;
-            if ((rc = locator_->launch(dout, shards, len, item.shard_off, b.stream))) return set_error(rc, s);
+            rc = piece_fn ? piece_fn(dout, shards, len, item.shard_off, int(s - slots_.data()), b.stream)
+                          : locator_->launch(dout, shards, len, item.shard_off, b.stream);
+            if (rc) return set_error(rc, s);
             // corrected or rebuilt streams that are written: they come back whole, once each
             uint64_t back = 0;
             for (const WriteOp& w : item.writes) {
@@ -397,6 +404,8 @@ class FilePipeline {
         dev_bad_ = nullptr;
         started_ = false;
     }
+
+    size_t slot_count() const { return slots_.size(); }  // after start()
 
     // verify mode, after finish(): mismatching 16-byte vectors per parity row
     int mismatches(unsigned long long* out) {
@@ -571,6 +580,33 @@ int scrub_columns(FilePipeline& pipe, const std::vector<int>& in, int64_t size, 
     return pipe.finish();
 }
 
+// Pass 2 of the damage calls, through a started pipeline: the union of pass 1's page `runs` as maximal spans, cut into
+// items of at most `chunk` columns, each reading its columns from every shard (in_d: O_DIRECT twins, -1 = none).
+// `add` adds what else an item needs (the repair: its writes) before it is submitted.  Returns pipe.finish().
+int submit_flagged(FilePipeline& pipe, const std::vector<swec_damage_range>& runs, size_t chunk, const std::vector<int>& in,
+                   const std::vector<int>& in_d, const std::function<void(Item&)>& add) {
+    std::vector<std::pair<int64_t, int64_t>> spans;
+    for (const swec_damage_range& r : runs) spans.push_back({r.offset, r.offset + r.length});
+    std::sort(spans.begin(), spans.end());
+    size_t nspans = 0;
+    for (const auto& sp : spans) {
+        if (nspans && sp.first <= spans[nspans - 1].second) spans[nspans - 1].second = std::max(spans[nspans - 1].second, sp.second);
+        else spans[nspans++] = sp;
+    }
+    spans.resize(nspans);
+    int rc = SWEC_OK;
+    for (size_t sp = 0; rc == SWEC_OK && sp < spans.size(); sp++)
+        for (int64_t o = spans[sp].first; rc == SWEC_OK && o < spans[sp].second; o += int64_t(chunk)) {
+            Item it;
+            it.len = size_t(std::min<int64_t>(int64_t(chunk), spans[sp].second - o));
+            it.shard_off = o;
+            for (size_t i = 0; i < in.size(); i++) it.reads.push_back({int(i), in[i], o, 0, it.len, in_d[i]});
+            if (add) add(it);
+            rc = pipe.submit(std::move(it));
+        }
+    return pipe.finish();
+}
+
 // Pass 2 of swec_repair_ec_damage.  `runs` are every page run pass 1 found, of the blamed shards and of the
 // uncorrectable columns.  Only the columns of those pages go through the pipeline again, with a correcting locator, and
 // the report and ranges are collected from that.  Each blamed shard gets back only its own pages, in the file where it
@@ -598,45 +634,43 @@ int repair_pages(swec_encoder* enc, const Matrix& rows, const std::string& b, co
         if ((out[size_t(i)] = fds.keep(open(path.c_str(), O_RDWR))) < 0) return io_fail("open " + path);
         out_d[size_t(i)] = fds.keep(open_direct(path, O_RDWR, direct & 2));
     }
-    // the union of the runs, as maximal spans [begin, end)
-    std::vector<std::pair<int64_t, int64_t>> spans;
-    for (const swec_damage_range& r : runs) spans.push_back({r.offset, r.offset + r.length});
-    std::sort(spans.begin(), spans.end());
-    size_t nspans = 0;
-    for (const auto& sp : spans) {
-        if (nspans && sp.first <= spans[nspans - 1].second) spans[nspans - 1].second = std::max(spans[nspans - 1].second, sp.second);
-        else spans[nspans++] = sp;
-    }
-    spans.resize(nspans);
-
     const size_t chunk = file_chunk(size);
     DamageLocator locator;
     FilePipeline pipe(enc, rows, chunk, /*verify=*/true, &locator);
     int rc = pipe.start();
     if (rc) return rc;
     if ((rc = locator.init(rows, size, radius, enc->stream, /*correct=*/true))) return rc;
-    for (size_t sp = 0; rc == SWEC_OK && sp < spans.size(); sp++)
-        for (int64_t o = spans[sp].first; rc == SWEC_OK && o < spans[sp].second; o += int64_t(chunk)) {
-            Item it;
-            it.len = size_t(std::min<int64_t>(int64_t(chunk), spans[sp].second - o));
-            it.shard_off = o;
-            const int64_t end = o + int64_t(it.len);
-            for (int i = 0; i < total; i++) {
-                it.reads.push_back({i, in[size_t(i)], o, 0, it.len, in_d[size_t(i)]});
-                for (size_t& r = next[size_t(i)]; r < stop[size_t(i)]; r++) {  // shard i's own pages in the item
-                    const int64_t lo = std::max(runs[r].offset, o), hi = std::min(runs[r].offset + runs[r].length, end);
-                    if (lo >= end) break;
-                    it.writes.push_back({i, out[size_t(i)], lo, size_t(lo - o), size_t(hi - lo), out_d[size_t(i)]});
-                    if (hi < runs[r].offset + runs[r].length) break;  // the run goes on in the next item
-                }
+    const auto writes = [&](Item& it) {
+        const int64_t o = it.shard_off, end = o + int64_t(it.len);
+        for (int i = 0; i < total; i++)
+            for (size_t& r = next[size_t(i)]; r < stop[size_t(i)]; r++) {  // shard i's own pages in the item
+                const int64_t lo = std::max(runs[r].offset, o), hi = std::min(runs[r].offset + runs[r].length, end);
+                if (lo >= end) break;
+                it.writes.push_back({i, out[size_t(i)], lo, size_t(lo - o), size_t(hi - lo), out_d[size_t(i)]});
+                if (hi < runs[r].offset + runs[r].length) break;  // the run goes on in the next item
             }
-            rc = pipe.submit(std::move(it));
-        }
-    if ((rc = pipe.finish())) return rc;
+    };
+    if ((rc = submit_flagged(pipe, runs, chunk, in, in_d, writes))) return rc;
     for (int i = 0; i < total; i++)
         if (out[size_t(i)] >= 0 && fdatasync(out[size_t(i)]) != 0) return io_fail("fdatasync " + b + shard_ext(i));
     return locator.collect(report, ranges, ranges_cap, n_ranges);
 }
+
+// Pass 1 of the damage calls, swec_locate_ec_damage itself: every column of the k+m shard files `in`, all `size` bytes,
+// through a verify pipeline with a locator.  `runs` (may be NULL) receives every page run, for pass 2.
+int locate_pass(swec_encoder* enc, const Matrix& rows, const std::vector<int>& in, int64_t size, int radius,
+                swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges,
+                std::vector<swec_damage_range>* runs) {
+    const size_t chunk = file_chunk(size);
+    DamageLocator locator;
+    FilePipeline pipe(enc, rows, chunk, /*verify=*/true, &locator);
+    int rc = pipe.start();
+    if (rc) return rc;
+    rc = locator.init(rows, size, radius, enc->stream);
+    if (rc == SWEC_OK) rc = scrub_columns(pipe, in, size, chunk);
+    if (rc == SWEC_OK) rc = locator.collect(report, ranges, ranges_cap, n_ranges, runs);
+    return rc;
+}  // the pipeline parks its staging ring for pass 2
 
 // swec_locate_ec_damage, and with `repair` swec_repair_ec_damage, whose pass 1 is the locate call itself: a set without
 // damage is never opened for writing.
@@ -656,16 +690,8 @@ int damage_files(const char* base, const char* const* dirs, int ndirs, int k, in
     if ((rc = open_all_shards(b, dirs, ndirs, k + m, &fds, &in, &size))) return rc;
     const Matrix rows = parity_rows(enc.get());
     std::vector<swec_damage_range> runs;
-    {
-        const size_t chunk = file_chunk(size);
-        DamageLocator locator;
-        FilePipeline pipe(enc.get(), rows, chunk, /*verify=*/true, &locator);
-        if ((rc = pipe.start())) return rc;
-        rc = locator.init(rows, size, radius, enc->stream);
-        if (rc == SWEC_OK) rc = scrub_columns(pipe, in, size, chunk);
-        if (rc == SWEC_OK) rc = locator.collect(report, ranges, ranges_cap, n_ranges, repair ? &runs : nullptr);
-        if (rc) return rc;
-    }  // the pipeline parks its staging ring for pass 2
+    if ((rc = locate_pass(enc.get(), rows, in, size, radius, report, ranges, ranges_cap, n_ranges, repair ? &runs : nullptr)))
+        return rc;
     if (repair && report->damaged_columns &&
         (rc = repair_pages(enc.get(), rows, b, dirs, ndirs, in, size, radius, runs, report, ranges, ranges_cap, n_ranges)))
         return rc;
@@ -914,6 +940,45 @@ int decode_dat(swec_encoder* enc, const std::vector<int>& in, const std::vector<
 }
 
 }  // namespace
+
+namespace swec {
+
+// Pass 2 per item: the slot's data shards saved, the correcting locate, the corrected data re-encoded into the computed
+// rows (the locate is done with them), then the attribution.  Nothing comes back to the host and nothing is written.
+int needle_damage_files(swec_encoder* enc, const std::vector<int>& in, int64_t size, int radius, const StripeMap& map,
+                        int version, std::vector<swec_needle_damage>* recs, swec_damage_report* report,
+                        swec_damage_range* ranges, int ranges_cap, int* n_ranges, uint64_t unowned[2]) {
+    const Matrix rows = parity_rows(enc);
+    std::vector<swec_damage_range> runs;
+    int rc = locate_pass(enc, rows, in, size, radius, report, ranges, ranges_cap, n_ranges, &runs);
+    if (rc || report->damaged_columns == 0) return rc;
+    const int k = enc->k;
+    const size_t chunk = file_chunk(size);
+    DamageLocator locator;
+    NeedleDamage nd;
+    FilePipeline pipe(enc, rows, chunk, /*verify=*/true, &locator);
+    pipe.piece_fn = [&](uint8_t* const* computed, uint8_t* const* shards, size_t len, int64_t base, int slot,
+                        cudaStream_t s) -> int {
+        int r = nd.save(shards, len, slot, s);
+        if (r == SWEC_OK) r = locator.launch(computed, shards, len, base, s);
+        if (r == SWEC_OK) {
+            const uint8_t* data[SWEC_MAX_SHARDS];
+            for (int i = 0; i < k; i++) data[i] = shards[i];
+            std::lock_guard<std::mutex> lk(enc->mu);
+            r = enc->apply(rows, data, computed, len, Layout{}, s);
+        }
+        if (r == SWEC_OK) r = nd.launch(nullptr, shards, computed, len, base, slot, s);
+        return r;
+    };
+    if ((rc = pipe.start())) return rc;
+    if ((rc = locator.init(rows, size, radius, enc->stream, /*correct=*/true))) return rc;
+    if ((rc = nd.init(k, enc->m, map, recs->data(), int(recs->size()), version, int(pipe.slot_count()), chunk, enc->stream)))
+        return rc;
+    if ((rc = submit_flagged(pipe, runs, chunk, in, std::vector<int>(in.size(), -1), nullptr))) return rc;
+    return nd.collect(recs->data(), unowned);
+}
+
+}  // namespace swec
 
 extern "C" {
 

@@ -32,6 +32,7 @@
 #include "damage.h"
 #include "engine.h"
 #include "mini_json.h"
+#include "needle_damage.h"
 #include "needles.h"
 #include "volume_format.h"
 
@@ -791,6 +792,63 @@ int swec_ec_volume_info(swec_ec_volume* v, int* data_shards, int* parity_shards,
             if (v->shard_fd[i] >= 0) bits |= 1u << i;
         *local_shard_bits = bits;
     }
+    return SWEC_OK;
+}
+
+// Which needles the located damage hits, on the handle's own descriptors (include/swec.h): every check before any
+// device work, the live records as the reads see them, then pass 1 and, with damage, pass 2 (needle_damage_files).
+int swec_ec_volume_locate_needle_damage(swec_ec_volume* v, int radius, swec_damage_report* report, swec_damage_range* ranges,
+                                        int ranges_cap, int* n_ranges, swec_needle_damage* needles, int needles_cap,
+                                        int* n_needles, uint64_t unowned[2], int* ok) {
+    int rc = check_needle_damage_args(needles_cap, needles, unowned, 0, nullptr);
+    if (rc) return rc;
+    if (!v || !n_needles || !ok) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
+    std::lock_guard<std::mutex> lock(v->mu);
+    if ((rc = check_locate_args(v->m, radius, report, ranges, ranges_cap))) return rc;
+    *ok = 0;
+    *n_needles = 0;
+    unowned[0] = unowned[1] = 0;
+    const int total = v->k + v->m;
+    for (int i = 0; i < total; i++)
+        if (v->shard_fd[size_t(i)] < 0)
+            return fail(SWEC_ERR_TOO_FEW_SHARDS, "locating needle damage needs all shards; missing " + shard_ext(i));
+    int64_t size = -1;
+    for (int i = 0; i < total; i++) {
+        struct stat st;
+        if (fstat(v->shard_fd[size_t(i)], &st) != 0) return fail(SWEC_ERR_IO, std::string("fstat shard: ") + strerror(errno));
+        if (size < 0) size = st.st_size;
+        if (st.st_size != size)
+            return fail(SWEC_ERR_SHARD_SIZE, "ec shard size expected " + std::to_string(size) + " actual " + std::to_string(st.st_size));
+    }
+    if (v->device < 0) return fail(SWEC_ERR_NO_DEVICE, "no CUDA device: the volume was opened with device < 0");
+    // live records: .ecx entries that are not deleted, minus the journalled ids (FindNeedleFromEcx, ec_volume.go:419-429)
+    v->refresh_journal();
+    std::vector<swec_needle_damage> recs;
+    const int64_t entries = int64_t(v->ecx_bytes) / kIndexEntrySize;
+    for (int64_t e = 0; e < entries; e++) {
+        const IndexEntry x = index_entry(v->ecx_map + e * kIndexEntrySize);
+        if (size_deleted(x.size) || std::binary_search(v->deleted.begin(), v->deleted.end(), x.key)) continue;
+        swec_needle_damage r{};
+        r.needle_id = x.key;
+        r.offset = x.offset;
+        r.size = x.size;
+        recs.push_back(r);
+    }
+    if (!v->enc && (rc = swec_encoder_new(v->k, v->m, v->device, &v->enc))) return rc;
+    const StripeMap map = StripeMap::locate(v->shard_dat_size, v->k, kLargeBlockSize, kSmallBlockSize);
+    if ((rc = needle_damage_files(v->enc, v->shard_fd, size, radius, map, v->version, &recs, report, ranges, ranges_cap,
+                                  n_ranges, unowned)))
+        return rc;
+    std::stable_sort(recs.begin(), recs.end(),
+                     [](const swec_needle_damage& a, const swec_needle_damage& b) { return a.needle_id < b.needle_id; });
+    int hit = 0;
+    for (const swec_needle_damage& r : recs) {
+        if (!r.damaged_bytes && !r.uncorrectable_bytes) continue;
+        if (hit < needles_cap) needles[hit] = r;
+        hit++;
+    }
+    *n_needles = hit;
+    *ok = report->damaged_columns == 0 ? 1 : 0;
     return SWEC_OK;
 }
 

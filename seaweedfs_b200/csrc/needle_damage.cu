@@ -1,0 +1,239 @@
+// seaweedfs_b200/csrc/needle_damage.cu — which needles the located damage hits (needle_damage.h), and the device call.
+//
+//   nd_attribute_kernel   grid-stride, one thread per byte column of a piece.  The column is uncorrectable when its
+//                         residual syndrome (parity re-encoded from the corrected data XOR the corrected parity) is not
+//                         zero: every column the correcting locate decoded within the radius is a codeword again.  A
+//                         data byte is damaged when the correcting locate changed it: a blamed byte always changes,
+//                         because its error value is not zero.  Each such byte of data shard i is mapped to its .dat
+//                         offset (stripe_map.h), the live records (sorted by offset) are binary-searched for its owner,
+//                         and the owner's counters and shard mask, or the unowned counters, take it with atomics.
+// The locate kernel itself (damage.cu) is not changed: pass 2 runs its correcting instantiation on a copy.
+#include <cuda_runtime.h>
+
+#include <algorithm>
+#include <cstring>
+#include <numeric>
+
+#include "damage.h"
+#include "device_common.cuh"
+#include "engine.h"
+#include "needle_damage.h"
+#include "needle_format.h"
+
+namespace swec {
+
+namespace {
+
+struct AttributeParams {
+    const u8* orig[SWEC_MAX_SHARDS];    // data shards as found
+    const u8* fixed[SWEC_MAX_SHARDS];   // data shards after the correcting locate
+    const u8* comp[SWEC_MAX_SHARDS];    // parity re-encoded from fixed
+    const u8* stored[SWEC_MAX_SHARDS];  // parity after the correcting locate
+    u64 n;
+    int64_t base;
+    int k, m, nrec;
+    StripeMap map;
+    const int64_t* off;  // record offsets, ascending
+    const int64_t* end;
+    unsigned long long* damaged;        // [nrec]
+    unsigned long long* uncorrectable;  // [nrec]
+    unsigned long long* unowned;        // [2]
+    unsigned* mask;                     // [nrec]
+};
+
+__global__ void __launch_bounds__(256) nd_attribute_kernel(const __grid_constant__ AttributeParams p) {
+    const u64 stride = u64(gridDim.x) * blockDim.x;
+    for (u64 x = u64(blockIdx.x) * blockDim.x + threadIdx.x; x < p.n; x += stride) {
+        u8 residual = 0;
+        for (int q = 0; q < p.m; q++) residual |= p.comp[q][x] ^ p.stored[q][x];
+        for (int i = 0; i < p.k; i++) {
+            if (!residual && p.orig[i][x] == p.fixed[i][x]) continue;
+            const int kind = residual ? 1 : 0;
+            const int64_t d = p.map.dat_offset(i, p.base + int64_t(x));
+            int owner = -1;
+            if (d >= 0) {  // the last record whose offset is not above d
+                int lo = 0, hi = p.nrec;
+                while (lo < hi) {
+                    const int mid = (lo + hi) >> 1;
+                    if (p.off[mid] <= d) lo = mid + 1;
+                    else hi = mid;
+                }
+                if (lo > 0 && d < p.end[lo - 1]) owner = lo - 1;
+            }
+            if (owner < 0) {
+                atomicAdd(p.unowned + kind, 1ull);
+                continue;
+            }
+            atomicAdd((kind ? p.uncorrectable : p.damaged) + owner, 1ull);
+            atomicOr(p.mask + owner, 1u << i);
+        }
+    }
+}
+
+unsigned attribute_grid(u64 n) {
+    int dev = 0, sms = 132;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    return unsigned(std::max<u64>(1, std::min<u64>((n + 255) / 256, u64(sms) * 8)));
+}
+
+}  // namespace
+
+int check_needle_damage_args(int needles_cap, const swec_needle_damage* needles, const uint64_t* unowned, int n_records,
+                             const swec_needle_damage* records) {
+    if (needles_cap < 0 || (needles_cap > 0 && !needles))
+        return fail(SWEC_ERR_INVALID_ARG, "needles_cap must be >= 0, and needles non-NULL when it is > 0");
+    if (!unowned) return fail(SWEC_ERR_INVALID_ARG, "unowned is NULL");
+    if (n_records < 0 || (n_records > 0 && !records))
+        return fail(SWEC_ERR_INVALID_ARG, "n_records must be >= 0, and records non-NULL when it is > 0");
+    return SWEC_OK;
+}
+
+NeedleDamage::~NeedleDamage() {
+    if (spans_) cudaFree(spans_);
+    if (counters_) cudaFree(counters_);
+    if (masks_) cudaFree(masks_);
+    if (saved_) cudaFree(saved_);
+}
+
+int NeedleDamage::init(int k, int m, const StripeMap& map, const swec_needle_damage* recs, int n, int version, int slots,
+                       size_t piece, cudaStream_t s) {
+    k_ = k;
+    m_ = m;
+    n_ = n;
+    map_ = map;
+    piece_ = piece;
+    order_.resize(size_t(n));
+    std::iota(order_.begin(), order_.end(), 0);
+    std::stable_sort(order_.begin(), order_.end(), [&](int a, int b) { return recs[a].offset < recs[b].offset; });
+    std::vector<int64_t> spans(size_t(2 * std::max(n, 1)), 0);
+    for (int j = 0; j < n; j++) {
+        const swec_needle_damage& r = recs[order_[size_t(j)]];
+        spans[size_t(j)] = r.offset;
+        spans[size_t(n + j)] = r.size < 0 ? r.offset : r.offset + needle_actual_size(r.size, version);
+    }
+    const size_t nc = size_t(2 * n + 2);
+    SWEC_CUDA(cudaMalloc(reinterpret_cast<void**>(&spans_), spans.size() * sizeof(int64_t)));
+    SWEC_CUDA(cudaMalloc(reinterpret_cast<void**>(&counters_), nc * sizeof(unsigned long long)));
+    SWEC_CUDA(cudaMalloc(reinterpret_cast<void**>(&masks_), size_t(std::max(n, 1)) * sizeof(unsigned)));
+    if (slots > 0 && piece > 0) SWEC_CUDA(cudaMalloc(reinterpret_cast<void**>(&saved_), size_t(slots) * size_t(k) * piece));
+    SWEC_CUDA(cudaMemcpyAsync(spans_, spans.data(), spans.size() * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+    SWEC_CUDA(cudaMemsetAsync(counters_, 0, nc * sizeof(unsigned long long), s));
+    SWEC_CUDA(cudaMemsetAsync(masks_, 0, size_t(std::max(n, 1)) * sizeof(unsigned), s));
+    SWEC_CUDA(cudaStreamSynchronize(s));
+    return SWEC_OK;
+}
+
+int NeedleDamage::save(uint8_t* const* shards, size_t len, int slot, cudaStream_t s) {
+    uint8_t* at = saved_ + size_t(slot) * size_t(k_) * piece_;
+    for (int i = 0; i < k_; i++)
+        SWEC_CUDA(cudaMemcpyAsync(at + size_t(i) * piece_, shards[i], len, cudaMemcpyDeviceToDevice, s));
+    return SWEC_OK;
+}
+
+int NeedleDamage::launch(const uint8_t* const* orig, uint8_t* const* fixed, uint8_t* const* comp, size_t len, int64_t base,
+                         int slot, cudaStream_t s) {
+    if (len == 0) return SWEC_OK;
+    AttributeParams p;
+    memset(&p, 0, sizeof p);
+    for (int i = 0; i < k_; i++) {
+        p.orig[i] = orig ? orig[i] : saved_ + (size_t(slot) * size_t(k_) + size_t(i)) * piece_;
+        p.fixed[i] = fixed[i];
+    }
+    for (int q = 0; q < m_; q++) {
+        p.comp[q] = comp[q];
+        p.stored[q] = fixed[k_ + q];
+    }
+    p.n = len;
+    p.base = base;
+    p.k = k_;
+    p.m = m_;
+    p.nrec = n_;
+    p.map = map_;
+    p.off = spans_;
+    p.end = spans_ + n_;
+    p.damaged = counters_;
+    p.uncorrectable = counters_ + n_;
+    p.unowned = counters_ + 2 * n_;
+    p.mask = masks_;
+    nd_attribute_kernel<<<attribute_grid(len), 256, 0, s>>>(p);
+    g_kernel_launches++;
+    SWEC_CUDA(cudaGetLastError());
+    return SWEC_OK;
+}
+
+int NeedleDamage::collect(swec_needle_damage* recs, uint64_t unowned[2]) {
+    std::vector<unsigned long long> c(size_t(2 * n_ + 2));
+    std::vector<unsigned> mask(size_t(std::max(n_, 1)));
+    SWEC_CUDA(cudaMemcpy(c.data(), counters_, c.size() * sizeof c[0], cudaMemcpyDeviceToHost));
+    SWEC_CUDA(cudaMemcpy(mask.data(), masks_, mask.size() * sizeof mask[0], cudaMemcpyDeviceToHost));
+    for (int j = 0; j < n_; j++) {
+        swec_needle_damage& r = recs[order_[size_t(j)]];
+        r.damaged_bytes = c[size_t(j)];
+        r.uncorrectable_bytes = c[size_t(n_ + j)];
+        r.shard_mask = mask[size_t(j)];
+    }
+    unowned[0] = c[size_t(2 * n_)];
+    unowned[1] = c[size_t(2 * n_ + 1)];
+    return SWEC_OK;
+}
+
+}  // namespace swec
+
+using namespace swec;
+
+extern "C" {
+
+// Per 256 MiB piece: the shards copied to scratch, the parity re-encoded and the correcting locate run on the copy (its
+// report is the one the locate call gives), the corrected data re-encoded, then the attribution against the caller's
+// data shards, which are never written.
+int swec_locate_needle_damage_device(swec_encoder* e, const void* const* shards, size_t n, int64_t dat_size, int64_t large,
+                                     int64_t small, int radius, swec_needle_damage* records, int n_records,
+                                     swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges,
+                                     uint64_t unowned[2], void* stream) {
+    int rc = check_needle_damage_args(0, nullptr, unowned, n_records, records);
+    if (rc) return rc;
+    if (!e || !shards) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
+    if ((rc = check_locate_args(e->m, radius, report, ranges, ranges_cap))) return rc;
+    if (dat_size < 0 || large <= 0 || small <= 0) return fail(SWEC_ERR_INVALID_ARG, "bad geometry");
+    const int k = e->k, m = e->m;
+    for (int i = 0; i < k + m; i++)
+        if (!shards[i]) return fail(SWEC_ERR_INVALID_ARG, "NULL shard");
+    const uint8_t* const* sh = reinterpret_cast<const uint8_t* const*>(shards);
+    std::lock_guard<std::mutex> lock(e->mu);
+    if ((rc = e->ensure_device())) return rc;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    const Matrix rows = parity_rows(e);
+    const size_t piece = std::min(n, size_t(256) << 20);
+    DamageLocator locator;
+    NeedleDamage nd;
+    if ((rc = locator.init(rows, int64_t(n), radius, s, /*correct=*/true))) return rc;
+    if ((rc = nd.init(k, m, StripeMap::encode(dat_size, k, large, small), records, n_records, 3, 0, 0, s))) return rc;
+    StreamScratch scratch(s);
+    if (piece) SWEC_CUDA(scratch.alloc(size_t(k + 2 * m) * piece));
+    for (size_t off = 0; off < n; off += piece) {
+        const size_t len = std::min(piece, n - off);
+        const uint8_t* orig[SWEC_MAX_SHARDS];
+        const uint8_t* data[SWEC_MAX_SHARDS];
+        uint8_t* work[SWEC_MAX_SHARDS];
+        uint8_t* comp[SWEC_MAX_SHARDS];
+        for (int i = 0; i < k + m; i++) {
+            work[i] = scratch.as<uint8_t>() + size_t(i) * piece;
+            SWEC_CUDA(cudaMemcpyAsync(work[i], sh[i] + off, len, cudaMemcpyDeviceToDevice, s));
+        }
+        for (int i = 0; i < k; i++) {
+            orig[i] = sh[i] + off;
+            data[i] = work[i];
+        }
+        for (int q = 0; q < m; q++) comp[q] = scratch.as<uint8_t>() + size_t(k + m + q) * piece;
+        if ((rc = e->apply(rows, data, comp, len, Layout{}, s))) return rc;
+        if ((rc = locator.launch(comp, work, len, int64_t(off), s))) return rc;
+        if ((rc = e->apply(rows, data, comp, len, Layout{}, s))) return rc;
+        if ((rc = nd.launch(orig, work, comp, len, int64_t(off), 0, s))) return rc;
+    }
+    SWEC_CUDA(cudaStreamSynchronize(s));
+    if ((rc = locator.collect(report, ranges, ranges_cap, n_ranges))) return rc;
+    return nd.collect(records, unowned);
+}
+
+}  // extern "C"

@@ -18,7 +18,8 @@ from dataclasses import dataclass
 
 import numpy as np
 
-from ._native import STATUS, DamageRange, DamageReport, Interval, NeedleRead, ReconstructItem, SwecError, check, lib
+from ._native import (STATUS, DamageRange, DamageReport, Interval, NeedleDamage, NeedleRead, ReconstructItem, SwecError,
+                      check, lib)
 
 DataShardsCount = 10                               # ec_encoder.go:20
 ParityShardsCount = 4                              # ec_encoder.go:21
@@ -195,6 +196,25 @@ class Encoder:
                                                max_ranges, C.byref(n), stream))
         return _damage_result(report, ranges, n.value, max_ranges)
 
+    def locate_needle_damage_device(self, shard_ptrs, shard_len: int, dat_size: int, records, radius: int = 1,
+                                    large_block: int = ErasureCodingLargeBlockSize,
+                                    small_block: int = ErasureCodingSmallBlockSize, max_ranges: int = 4096,
+                                    stream: int = 0) -> dict:
+        """locate_damage_device, and which records of the volume image striped into the data shards the damage hits
+        (swec_locate_needle_damage_device).  records: (needle_id, offset, size) of every live record, sized as needle
+        version 3.  Returns the result of locate_damage_device plus "needles" (one dict per record, in order, zero counts
+        included) and "unowned" = [damaged, uncorrectable] bytes that no record owns.  The shards are only read."""
+        records = list(records)
+        arr = (NeedleDamage * max(1, len(records)))()
+        for r, (nid, off, size) in zip(arr, records):
+            r.needle_id, r.offset, r.size = nid, off, size
+        report, ranges, n, unowned = DamageReport(), (DamageRange * max(1, max_ranges))(), C.c_int(0), (C.c_uint64 * 2)()
+        check(lib().swec_locate_needle_damage_device(self._h, _ptrs(shard_ptrs), shard_len, dat_size, large_block,
+                                                     small_block, radius, arr, len(records), C.byref(report), ranges,
+                                                     max_ranges, C.byref(n), unowned, stream))
+        return {**_damage_result(report, ranges, n.value, max_ranges), "needles": _needle_damage(arr[:len(records)]),
+                "unowned": [int(unowned[0]), int(unowned[1])]}
+
     def reconstruct_checked_device(self, shard_ptrs, present, shard_len: int, radius: int = 1, max_ranges: int = 4096,
                                    stream: int = 0) -> dict:
         """reconstruct_device that reads every present shard and corrects the damage it locates in the first k present
@@ -332,6 +352,11 @@ def _damage_result(report, ranges, n_ranges: int, max_ranges: int) -> dict:
             "first_uncorrectable": int(report.first_uncorrectable), "last_uncorrectable": int(report.last_uncorrectable),
             "shards": shards, "ranges": [(r.shard_id, r.offset, r.length) for r in ranges[:min(n_ranges, max_ranges)]],
             "n_ranges": n_ranges}
+
+
+def _needle_damage(recs) -> list[dict]:
+    return [{"needle_id": int(r.needle_id), "offset": int(r.offset), "size": int(r.size), "shard_mask": int(r.shard_mask),
+             "damaged_bytes": int(r.damaged_bytes), "uncorrectable_bytes": int(r.uncorrectable_bytes)} for r in recs]
 
 
 def locate_ec_damage(base_file_name: str, additional_dirs: list[str] | None = None, ctx: ECContext | None = None,
@@ -548,6 +573,22 @@ class EcVolume:
         check(lib().swec_ec_volume_scrub_needles(self._h, volume_id, C.byref(n), broken, C.byref(nb), buf, len(buf),
                                                  C.byref(ne)))
         return int(n.value), list(broken[: nb.value]), (buf.value.decode().split("\n") if ne.value else [])
+
+    def locate_needle_damage(self, radius: int = 1, max_ranges: int = 4096, max_needles: int = 1 << 16) -> dict:
+        """locate_ec_damage on the volume's shards (all k+m must be local), and which live needles the damage hits
+        (swec_ec_volume_locate_needle_damage).  Returns the locate_ec_damage dict plus "needles" (ascending id, the first
+        max_needles of those with a non-zero count: needle_id, offset, size, shard_mask, damaged_bytes — a repair
+        restores them — and uncorrectable_bytes — it cannot), "n_needles" and "unowned" = [damaged, uncorrectable] bytes
+        that no live needle owns.  The shard files are only read."""
+        report, ranges, n, ok = DamageReport(), (DamageRange * max(1, max_ranges))(), C.c_int(0), C.c_int(0)
+        needles, n_needles, unowned = (NeedleDamage * max(1, max_needles))(), C.c_int(0), (C.c_uint64 * 2)()
+        check(lib().swec_ec_volume_locate_needle_damage(self._h, radius, C.byref(report), ranges, max_ranges, C.byref(n),
+                                                        needles, max_needles, C.byref(n_needles), unowned, C.byref(ok)))
+        return {"ok": bool(ok.value), **_damage_result(report, ranges, n.value, max_ranges),
+                "needles": _needle_damage(needles[:min(n_needles.value, max_needles)]), "n_needles": n_needles.value,
+                "unowned": [int(unowned[0]), int(unowned[1])]}
+
+    LocateNeedleDamage = locate_needle_damage
 
     def close(self) -> None:
         h, self._h = getattr(self, "_h", None), None
