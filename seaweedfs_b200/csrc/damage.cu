@@ -425,18 +425,38 @@ void unchecked_report(swec_damage_report* report, int* n_ranges) {
     if (n_ranges) *n_ranges = 0;
 }
 
-void drop_missing_parity(const uint8_t* present, int k, std::vector<int>* outs, Matrix* fused) {
-    std::vector<int> kept;
-    Matrix rows(0, fused->cols);
-    for (size_t o = 0; o < outs->size(); o++) {
-        const int id = (*outs)[o];
-        if (id >= k && !present[id]) continue;
-        kept.push_back(id);
-        rows.v.insert(rows.v.end(), fused->row(int(o)), fused->row(int(o)) + fused->cols);
-        rows.rows++;
+bool CheckedPlan::build(const Matrix& gen, int k, const uint8_t* present, bool decode) {
+    this->decode = decode;
+    std::vector<uint8_t> mask(size_t(gen.rows), 0);  // the information set alone: every other shard gets a row
+    for (int i = 0, n = 0; i < gen.rows && n < k; i++)
+        if (present[i]) mask[size_t(i)] = 1, n++;
+    std::vector<int> all;
+    Matrix rows;
+    if (!rs_reconstruct_plan(gen, k, mask.data(), false, &info, &all, &rows)) return false;
+    outs.clear();
+    fused = Matrix(0, k);
+    check_rows.clear();
+    rebuilt_rows.clear();
+    for (size_t o = 0; o < all.size(); o++) {
+        const int id = all[o];
+        if (decode && id >= k && !present[id]) continue;  // a missing parity shard
+        (present[id] ? check_rows : rebuilt_rows).push_back(int(outs.size()));
+        outs.push_back(id);
+        fused.v.insert(fused.v.end(), rows.row(int(o)), rows.row(int(o)) + k);
+        fused.rows++;
     }
-    *outs = kept;
-    *fused = rows;
+    return true;
+}
+
+int CheckedPlan::position(int id) const {
+    const int k = int(info.size()), c = this->c();
+    for (int j = 0; j < k; j++)
+        if (info[size_t(j)] == id) return j;
+    for (int i = 0; i < c; i++)
+        if (check(i) == id) return k + i;
+    for (size_t o = 0; o < outs.size(); o++)
+        if (outs[o] == id) return k + c + int(o);
+    return -1;
 }
 
 DamageLocator::~DamageLocator() {
@@ -478,23 +498,20 @@ int DamageLocator::init(const Matrix& parity, int64_t shard_len, int radius, cud
     return SWEC_OK;
 }
 
-int DamageLocator::init_rebuild(const Matrix& fused, const std::vector<int>& info, const std::vector<int>& outs,
-                                const uint8_t* present, int64_t shard_len, int radius, cudaStream_t s, bool decode) {
-    const int k = fused.cols;
-    std::vector<int> check;  // rows of `fused`
-    out_rows_.clear();
-    for (size_t o = 0; o < outs.size(); o++) (present[outs[o]] ? check : out_rows_).push_back(int(o));
-    const int c = int(check.size());
+int DamageLocator::init_rebuild(const CheckedPlan& plan, int64_t shard_len, int radius, cudaStream_t s) {
+    const Matrix& fused = plan.fused;
+    const int k = fused.cols, c = plan.c();
     Matrix pc(c, k);
     for (int i = 0; i < c; i++)
-        for (int j = 0; j < k; j++) pc.at(i, j) = fused.at(check[size_t(i)], j);
+        for (int j = 0; j < k; j++) pc.at(i, j) = fused.at(plan.check_rows[size_t(i)], j);
     // the punctured code has distance c+1: radius t needs 2t <= c
     if (int rc = init(pc, shard_len, std::min(radius, c / 2), s)) return rc;
     rebuild_ = true;
-    decode_ = decode;
-    check_rows_ = check;
-    for (int j = 0; j < k; j++) ids_[size_t(j)] = info[size_t(j)];
-    for (int i = 0; i < c; i++) ids_[size_t(k + i)] = outs[size_t(check[size_t(i)])];
+    decode_ = plan.decode;
+    check_rows_ = plan.check_rows;
+    out_rows_ = plan.rebuilt_rows;
+    for (int j = 0; j < k; j++) ids_[size_t(j)] = plan.info[size_t(j)];
+    for (int i = 0; i < c; i++) ids_[size_t(k + i)] = plan.check(i);
     u8 log[256], exp[512];
     log_exp_tables(log, exp);
     RebuildTables rt;

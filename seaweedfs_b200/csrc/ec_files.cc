@@ -709,50 +709,62 @@ struct Checked {
     bool checked = false;  // set once the report comes from a locator (c >= 1)
 };
 
-// The checked rebuild's pipeline.  The first k present shards are the information set I; the other c present shards
-// are read too, as the check shards of the punctured code.  Per slot: one apply of the m x k rows of every shard outside
-// I (its c check shards re-encoded, its f missing shards rebuilt), then the rebuilding locator, which compares the c
-// check rows with the stored ones and takes the errors it locates in I out of the f rebuilt rows.  Only those come back
-// and are written.
-int rebuild_checked(swec_encoder* enc, const std::vector<int>& in, const std::vector<int>& in_d,
-                    const std::vector<uint8_t>& present, const std::vector<int>& out, const std::vector<int>& out_d,
-                    int64_t todo, Checked* chk) {
-    const int k = enc->k, total = enc->k + enc->m;
-    std::vector<uint8_t> info(static_cast<size_t>(total), 0);
-    for (int i = 0, n = 0; i < total && n < k; i++)
-        if (present[size_t(i)]) info[size_t(i)] = 1, n++;
-    std::vector<int> ins, outs;  // outs: every shard outside I, ascending, one row of `fused` each
-    Matrix fused;
-    if (!rs_reconstruct_plan(enc->gen, k, info.data(), false, &ins, &outs, &fused))
-        return fail(SWEC_ERR_TOO_FEW_SHARDS, "not enough shards");
-    std::vector<int> checks;     // check shard ids, ascending: streams k .. k+c of a slot
-    std::vector<int> out_rows;   // the fused row of out[r]
-    for (size_t o = 0; o < outs.size(); o++) {
-        if (present[size_t(outs[o])]) checks.push_back(outs[o]);
-        else out_rows.push_back(int(o));
-    }
-    const int c = int(checks.size());
-    const size_t chunk = file_chunk(todo);
+// Submits an item of a checked pipeline whose length and writes are set, at shard offset `col`.
+using SubmitFn = std::function<int(Item&& it, int64_t col)>;
+
+// The pipeline of the checked rebuild and decode over columns [0, cols) of the shards, after reserving `reserve_size`
+// bytes of each file in `reserve`.  The items `walk` gives, in slots of `chunk` columns, each read the k information
+// and c check streams at their plan positions.  Per slot: one apply of plan.fused (the check shards re-encoded, the
+// missing shards rebuilt), then, with c >= 1, the rebuilding or decoding locator, which compares the c check rows with
+// the stored ones and corrects the errors it locates in the information set.  With c = 0 (exactly k shards present)
+// the set is rebuilt and the report says nothing was checked.
+int checked_pipeline(swec_encoder* enc, const CheckedPlan& plan, const std::vector<int>& in, const std::vector<int>& in_d,
+                     int64_t cols, const std::vector<int>& reserve, int64_t reserve_size, Checked* chk,
+                     const std::function<int(size_t chunk, const SubmitFn& submit)>& walk) {
+    const int k = enc->k, c = plan.c();
+    const size_t chunk = file_chunk(cols);
     DamageLocator locator;
-    FilePipeline pipe(enc, fused, chunk, /*verify=*/true, &locator, /*stored=*/c);
+    FilePipeline pipe(enc, plan.fused, chunk, /*verify=*/c > 0, c > 0 ? &locator : nullptr, /*stored=*/c);
     int rc = pipe.start();
     if (rc) return rc;
-    if ((rc = locator.init_rebuild(fused, ins, outs, present.data(), todo, chk->radius, enc->stream))) return rc;
-    if (!out.empty()) reserve_extents(out, todo);
-    for (int64_t o = 0; rc == SWEC_OK && o < todo; o += int64_t(chunk)) {
-        Item it;
-        it.len = size_t(std::min<int64_t>(int64_t(chunk), todo - o));
-        it.shard_off = o;
-        for (int i = 0; i < k; i++) it.reads.push_back({i, in[size_t(ins[size_t(i)])], o, 0, it.len, in_d[size_t(ins[size_t(i)])]});
-        for (int i = 0; i < c; i++)
-            it.reads.push_back({k + i, in[size_t(checks[size_t(i)])], o, 0, it.len, in_d[size_t(checks[size_t(i)])]});
-        for (size_t r = 0; r < out.size(); r++) it.writes.push_back({k + c + out_rows[r], out[r], o, 0, it.len, out_d[r]});
-        rc = pipe.submit(std::move(it));
-    }
+    if (c > 0 && (rc = locator.init_rebuild(plan, cols, chk->radius, enc->stream))) return rc;
+    if (!reserve.empty()) reserve_extents(reserve, reserve_size);
+    walk(chunk, [&](Item&& it, int64_t col) {
+        it.shard_off = col;
+        for (int p = 0; p < k + c; p++) {
+            const size_t id = size_t(p < k ? plan.info[size_t(p)] : plan.check(p - k));
+            it.reads.push_back({p, in[id], col, 0, it.len, in_d[id]});
+        }
+        return pipe.submit(std::move(it));
+    });  // a failed submit ends the walk, and finish() returns its error
     if ((rc = pipe.finish())) return rc;
+    if (c == 0) {
+        unchecked_report(chk->report, chk->n_ranges);
+        return SWEC_OK;
+    }
     if ((rc = locator.collect(chk->report, chk->ranges, chk->ranges_cap, chk->n_ranges))) return rc;
     chk->checked = true;
     return SWEC_OK;
+}
+
+// The checked rebuild: every present shard is read, as the check shards of the punctured code beyond the first k, and
+// the rebuilt shards are written to `out` (in ascending id of the missing shards).
+int rebuild_checked(swec_encoder* enc, const std::vector<int>& in, const std::vector<int>& in_d,
+                    const std::vector<uint8_t>& present, const std::vector<int>& out, const std::vector<int>& out_d,
+                    int64_t todo, Checked* chk) {
+    CheckedPlan plan;
+    if (!plan.build(enc->gen, enc->k, present.data(), /*decode=*/false)) return fail(SWEC_ERR_TOO_FEW_SHARDS, "not enough shards");
+    return checked_pipeline(enc, plan, in, in_d, todo, out, todo, chk, [&](size_t chunk, const SubmitFn& submit) {
+        int rc = SWEC_OK;
+        for (int64_t o = 0; rc == SWEC_OK && o < todo; o += int64_t(chunk)) {
+            Item it;
+            it.len = size_t(std::min<int64_t>(int64_t(chunk), todo - o));
+            for (size_t r = 0; r < out.size(); r++)
+                it.writes.push_back({plan.position(plan.rebuilt(int(r))), out[r], o, 0, it.len, out_d[r]});
+            rc = submit(std::move(it), o);
+        }
+        return rc;
+    });
 }
 
 // swec_rebuild_ec_files, and with `chk` swec_rebuild_ec_files_checked: the same files, checks, errors and order.  The
@@ -822,8 +834,7 @@ int rebuild_files(const char* base, const char* const* dirs, int ndirs, int k, i
     const bool ragged = !missing.empty() && size > mib && size % mib != 0;
     const int64_t todo = ragged ? size / mib * mib : size;
 
-    const int checks = m - int(missing.size());  // present shards beyond the first k
-    if (chk && checks > 0) {
+    if (chk) {
         if ((rc = rebuild_checked(enc.get(), in, in_d, present, out, out_d, todo, chk))) return rc;
     } else {
         std::vector<int> ins, outs_idx;  // outs_idx == missing: fused row r rebuilds the shard of out[r]
@@ -842,101 +853,66 @@ int rebuild_files(const char* base, const char* const* dirs, int ndirs, int k, i
             rc = pipe.submit(std::move(it));
         }
         if ((rc = pipe.finish())) return rc;
-        if (chk) unchecked_report(chk->report, chk->n_ranges);  // no present shard beyond the first k: nothing to check
     }
     if (ragged) return shard_size_error(mib, size % mib);
     undo.armed = false;
     return SWEC_OK;
 }
 
-// The checked decode's pipeline over columns [0, cols) of the shards.  Its items follow swec_write_dat_file's copy
-// plan: rows of large blocks cut at the slot size, then the small rows, several to a slot as in swec_generate_ec_files,
-// the ragged tail row last; no item straddles a row boundary.  Each item reads the k information and c check streams.
-// One apply of the rows of the missing data shards and of the check shards, then the decoding locator (c >= 1), which
-// corrects the information streams that are data shards in the slot and the rebuilt rows.  The item's writes un-stripe
-// the k data streams into the .dat at the plan's offsets.
+// The checked decode over columns [0, cols) of the shards.  Its items follow swec_write_dat_file's copy plan: rows of
+// large blocks cut at the slot size, then the small rows, several to a slot as in swec_generate_ec_files, the ragged
+// tail row last; no item straddles a row boundary.  The apply computes the rows of the missing data shards and of the
+// check shards, and the decoding locator also corrects the information streams that are data shards in the slot.  The
+// item's writes un-stripe the k data streams into the .dat at the plan's offsets.
 int decode_dat(swec_encoder* enc, const std::vector<int>& in, const std::vector<int>& in_d,
                const std::vector<uint8_t>& present, int dat, int dat_d, const StripeGeometry& g, int64_t dat_size,
                int64_t cols, Checked* chk) {
-    const int k = enc->k, total = enc->k + enc->m;
-    std::vector<uint8_t> info(static_cast<size_t>(total), 0);
-    for (int i = 0, n = 0; i < total && n < k; i++)
-        if (present[size_t(i)]) info[size_t(i)] = 1, n++;
-    std::vector<int> ins, outs;  // outs: the missing data shards and the check shards, ascending, one row of `fused` each
-    Matrix fused;
-    if (!rs_reconstruct_plan(enc->gen, k, info.data(), false, &ins, &outs, &fused))
-        return fail(SWEC_ERR_TOO_FEW_SHARDS, "not enough shards");
-    drop_missing_parity(present.data(), k, &outs, &fused);
-    std::vector<int> checks;                           // check shard ids, ascending: streams k .. k+c of a slot
-    std::vector<int> stream(static_cast<size_t>(k));   // the slot stream that holds data shard s
-    for (int j = 0; j < k; j++)
-        if (ins[size_t(j)] < k) stream[size_t(ins[size_t(j)])] = j;
-    for (int id : outs)
-        if (present[size_t(id)]) checks.push_back(id);
-    const int c = int(checks.size());
-    for (size_t o = 0; o < outs.size(); o++)  // computed row o is stream k + c + o
-        if (!present[size_t(outs[o])]) stream[size_t(outs[o])] = k + c + int(o);
-    const size_t chunk = file_chunk(cols);
-    DamageLocator locator;
-    FilePipeline pipe(enc, fused, chunk, /*verify=*/c > 0, c > 0 ? &locator : nullptr, /*stored=*/c);
-    int rc = pipe.start();
-    if (rc) return rc;
-    if (c > 0 && (rc = locator.init_rebuild(fused, ins, outs, present.data(), cols, chk->radius, enc->stream, /*decode=*/true)))
+    const int k = enc->k;
+    CheckedPlan plan;
+    if (!plan.build(enc->gen, k, present.data(), /*decode=*/true)) return fail(SWEC_ERR_TOO_FEW_SHARDS, "not enough shards");
+    std::vector<int> stream(static_cast<size_t>(k));  // the slot stream that holds data shard s
+    for (int s = 0; s < k; s++) stream[size_t(s)] = plan.position(s);
+    return checked_pipeline(enc, plan, in, in_d, cols, {dat}, dat_size, chk, [&](size_t chunk, const SubmitFn& submit) {
+        // columns [o, o + len) of a row whose blocks start at .dat offset row_dat, `block` bytes apart, taken from
+        // offset src of the item's streams; shard s holds tail_bytes(s) of the tail row
+        auto unstripe = [&](Item& it, int64_t row_dat, int64_t block, bool tail, int64_t o, int64_t len, size_t src) {
+            for (int s = 0; s < k; s++) {
+                const int64_t n = std::min(len, (tail ? g.tail_bytes(s) : block) - o);
+                if (n > 0) it.writes.push_back({stream[size_t(s)], dat, row_dat + int64_t(s) * block + o, src, size_t(n), dat_d});
+            }
+        };
+        int rc = SWEC_OK;
+        for (int64_t r = 0; rc == SWEC_OK && r < g.large_rows; r++)
+            for (int64_t o = 0; rc == SWEC_OK && o < g.large; o += int64_t(chunk)) {
+                Item it;
+                it.len = size_t(std::min<int64_t>(int64_t(chunk), g.large - o));
+                unstripe(it, r * g.large_row(), g.large, false, o, int64_t(it.len), 0);
+                rc = submit(std::move(it), r * g.large + o);
+            }
+        // the small rows, then the tail row, whose columns are the ones shard 0 gives it
+        const int64_t nrows = g.small_rows + (g.tail > 0 ? 1 : 0);
+        auto width = [&](int64_t j) { return j < g.small_rows ? g.small : g.tail_bytes(0); };
+        auto row_dat = [&](int64_t j) { return g.small_dat_offset() + j * g.small_row(); };
+        int64_t j = 0;
+        for (; rc == SWEC_OK && j < nrows && g.small > int64_t(chunk); j++)  // small blocks bigger than a slot: row by row
+            for (int64_t o = 0; rc == SWEC_OK && o < width(j); o += int64_t(chunk)) {
+                Item it;
+                it.len = size_t(std::min<int64_t>(int64_t(chunk), width(j) - o));
+                unstripe(it, row_dat(j), g.small, j == g.small_rows, o, int64_t(it.len), 0);
+                rc = submit(std::move(it), g.small_shard_offset() + j * g.small + o);
+            }
+        const int64_t rows_per_item = std::max<int64_t>(1, int64_t(chunk) / g.small);
+        while (rc == SWEC_OK && j < nrows) {
+            Item it;
+            const int64_t first = j;
+            for (; j < nrows && j - first < rows_per_item; j++) {
+                unstripe(it, row_dat(j), g.small, j == g.small_rows, 0, width(j), it.len);
+                it.len += size_t(width(j));
+            }
+            rc = submit(std::move(it), g.small_shard_offset() + first * g.small);
+        }
         return rc;
-    reserve_extents(std::vector<int>{dat}, dat_size);
-    // columns [o, o + len) of a row whose blocks start at .dat offset row_dat, `block` bytes apart, taken from offset
-    // src of the item's streams; shard s holds tail_bytes(s) of the tail row
-    auto unstripe = [&](Item& it, int64_t row_dat, int64_t block, bool tail, int64_t o, int64_t len, size_t src) {
-        for (int s = 0; s < k; s++) {
-            const int64_t n = std::min(len, (tail ? g.tail_bytes(s) : block) - o);
-            if (n > 0) it.writes.push_back({stream[size_t(s)], dat, row_dat + int64_t(s) * block + o, src, size_t(n), dat_d});
-        }
-    };
-    auto submit = [&](Item&& it, int64_t col) -> int {
-        it.shard_off = col;
-        for (int i = 0; i < k; i++)
-            it.reads.push_back({i, in[size_t(ins[size_t(i)])], col, 0, it.len, in_d[size_t(ins[size_t(i)])]});
-        for (int i = 0; i < c; i++)
-            it.reads.push_back({k + i, in[size_t(checks[size_t(i)])], col, 0, it.len, in_d[size_t(checks[size_t(i)])]});
-        return pipe.submit(std::move(it));
-    };
-    for (int64_t r = 0; rc == SWEC_OK && r < g.large_rows; r++)
-        for (int64_t o = 0; rc == SWEC_OK && o < g.large; o += int64_t(chunk)) {
-            Item it;
-            it.len = size_t(std::min<int64_t>(int64_t(chunk), g.large - o));
-            unstripe(it, r * g.large_row(), g.large, false, o, int64_t(it.len), 0);
-            rc = submit(std::move(it), r * g.large + o);
-        }
-    // the small rows, then the tail row, whose columns are the ones shard 0 gives it
-    const int64_t nrows = g.small_rows + (g.tail > 0 ? 1 : 0);
-    auto width = [&](int64_t j) { return j < g.small_rows ? g.small : g.tail_bytes(0); };
-    auto row_dat = [&](int64_t j) { return g.small_dat_offset() + j * g.small_row(); };
-    int64_t j = 0;
-    for (; rc == SWEC_OK && j < nrows && g.small > int64_t(chunk); j++)  // small blocks bigger than a slot: row by row
-        for (int64_t o = 0; rc == SWEC_OK && o < width(j); o += int64_t(chunk)) {
-            Item it;
-            it.len = size_t(std::min<int64_t>(int64_t(chunk), width(j) - o));
-            unstripe(it, row_dat(j), g.small, j == g.small_rows, o, int64_t(it.len), 0);
-            rc = submit(std::move(it), g.small_shard_offset() + j * g.small + o);
-        }
-    const int64_t rows_per_item = std::max<int64_t>(1, int64_t(chunk) / g.small);
-    while (rc == SWEC_OK && j < nrows) {
-        Item it;
-        const int64_t first = j;
-        for (; j < nrows && j - first < rows_per_item; j++) {
-            unstripe(it, row_dat(j), g.small, j == g.small_rows, 0, width(j), it.len);
-            it.len += size_t(width(j));
-        }
-        rc = submit(std::move(it), g.small_shard_offset() + first * g.small);
-    }
-    if ((rc = pipe.finish())) return rc;
-    if (c == 0) {  // exactly k shards present: rebuilt, not checked
-        unchecked_report(chk->report, chk->n_ranges);
-        return SWEC_OK;
-    }
-    if ((rc = locator.collect(chk->report, chk->ranges, chk->ranges_cap, chk->n_ranges))) return rc;
-    chk->checked = true;
-    return SWEC_OK;
+    });
 }
 
 }  // namespace

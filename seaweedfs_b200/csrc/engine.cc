@@ -777,6 +777,35 @@ int swec_write_dat_device(swec_encoder* e, const void* const* data_shards, int64
 
 namespace {
 
+// The device-level damage and checked calls: per piece, one apply of plan.fused from the information shards, the check
+// rows into scratch and the rebuilt rows into the caller's buffers, then (c >= 1) the initialised locator; returns once
+// the stream is done.  The computed check rows go to scratch a piece at a time: a 3 GiB shard set needs 1 GiB of it,
+// not 12 GiB.  A data byte corrected in a piece has already been encoded, and no later piece reads it.
+int locate_pieces(swec_encoder* e, const CheckedPlan& plan, uint8_t* const* sh, size_t n, DamageLocator& locator,
+                  cudaStream_t s) {
+    const int k = e->k, c = plan.c();
+    const size_t piece = std::min(n, size_t(256) << 20);
+    StreamScratch scratch(s);
+    if (piece && c > 0) SWEC_CUDA(scratch.alloc(size_t(c) * piece));
+    for (size_t off = 0; off < n && !plan.outs.empty(); off += piece) {
+        const size_t len = std::min(piece, n - off);
+        const uint8_t* in[SWEC_MAX_SHARDS];
+        uint8_t* at[SWEC_MAX_SHARDS];  // the shards at their locator positions: information, then check shards
+        uint8_t* comp[SWEC_MAX_SHARDS];
+        for (int j = 0; j < k; j++) in[j] = at[j] = sh[plan.info[size_t(j)]] + off;
+        for (int i = 0; i < c; i++) {
+            at[k + i] = sh[plan.check(i)] + off;
+            comp[plan.check_rows[size_t(i)]] = scratch.as<uint8_t>() + size_t(i) * piece;
+        }
+        for (int o : plan.rebuilt_rows) comp[o] = sh[plan.outs[size_t(o)]] + off;
+        int rc = e->apply(plan.fused, in, comp, len, Layout{}, s);
+        if (rc == SWEC_OK && c > 0) rc = locator.launch(comp, at, len, int64_t(off), s);
+        if (rc) return rc;
+    }
+    SWEC_CUDA(cudaStreamSynchronize(s));
+    return SWEC_OK;
+}
+
 // swec_locate_damage_device, and with `correct` swec_correct_damage_device: the shards are written only then.
 int damage_device(swec_encoder* e, const void* const* shards, size_t n, int radius, bool correct,
                   swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges, void* stream) {
@@ -787,29 +816,16 @@ int damage_device(swec_encoder* e, const void* const* shards, size_t n, int radi
     for (int i = 0; i < k + m; i++)
         if (!shards[i]) return fail(SWEC_ERR_INVALID_ARG, "NULL shard");
     uint8_t* const* sh = reinterpret_cast<uint8_t* const*>(const_cast<void* const*>(shards));
+    // every shard present: the data shards are the information set, fused is the parity rows, the checks are parity
+    const std::vector<uint8_t> all(static_cast<size_t>(k + m), 1);
+    CheckedPlan plan;
+    plan.build(e->gen, k, all.data(), false);
     std::lock_guard<std::mutex> lock(e->mu);
     if ((rc = e->ensure_device())) return rc;
     cudaStream_t s = pick_stream(e, stream);
-    const Matrix rows = parity_rows(e);
     DamageLocator locator;
-    if ((rc = locator.init(rows, int64_t(n), radius, s, correct))) return rc;
-    // The computed parity goes to scratch a piece at a time: a 3 GiB shard set needs 1 GiB of it, not 12 GiB.  A data
-    // byte corrected in a piece has already been encoded, and no later piece reads it.
-    const size_t piece = std::min(n, size_t(256) << 20);
-    StreamScratch scratch(s);
-    if (piece) SWEC_CUDA(scratch.alloc(size_t(m) * piece));
-    for (size_t off = 0; off < n; off += piece) {
-        const size_t len = std::min(piece, n - off);
-        const uint8_t* in[SWEC_MAX_SHARDS];
-        uint8_t* at[SWEC_MAX_SHARDS];
-        uint8_t* comp[SWEC_MAX_SHARDS];
-        for (int i = 0; i < k + m; i++) at[i] = sh[i] + off;
-        for (int i = 0; i < k; i++) in[i] = at[i];
-        for (int p = 0; p < m; p++) comp[p] = scratch.as<uint8_t>() + size_t(p) * piece;
-        if ((rc = e->apply(rows, in, comp, len, Layout{}, s))) return rc;
-        if ((rc = locator.launch(comp, at, len, int64_t(off), s))) return rc;
-    }
-    SWEC_CUDA(cudaStreamSynchronize(s));
+    if ((rc = locator.init(plan.fused, int64_t(n), radius, s, correct))) return rc;
+    if ((rc = locate_pieces(e, plan, sh, n, locator, s))) return rc;
     return locator.collect(report, ranges, ranges_cap, n_ranges);
 }
 
@@ -843,47 +859,18 @@ int checked_device(swec_encoder* e, void* const* shards, const uint8_t* present,
     int rc = check_rebuild_args(radius, report, ranges, ranges_cap);
     if (rc) return rc;
     const int k = e->k, total = e->k + e->m;
-    std::vector<uint8_t> info(static_cast<size_t>(total), 0);
-    int npresent = 0;
-    for (int i = 0; i < total; i++)
-        if (present[i] && npresent++ < k) info[size_t(i)] = 1;
-    if (npresent < k) return fail(SWEC_ERR_TOO_FEW_SHARDS, "fewer than data_shards shards present");
+    CheckedPlan plan;
+    if (!plan.build(e->gen, k, present, decode)) return fail(SWEC_ERR_TOO_FEW_SHARDS, "fewer than data_shards shards present");
     for (int i = 0; i < total; i++)
         if (!shards[i] && (present[i] || i < k || !decode))
             return fail(SWEC_ERR_INVALID_ARG, present[i] ? "NULL shard" : "missing shard has no buffer");
-    std::vector<int> ins, outs;  // outs: the shards outside the information set, ascending, one row of `fused` each
-    Matrix fused;
-    if (!rs_reconstruct_plan(e->gen, k, info.data(), false, &ins, &outs, &fused))
-        return fail(SWEC_ERR_TOO_FEW_SHARDS, "fewer than data_shards shards present");
-    if (decode) drop_missing_parity(present, k, &outs, &fused);
-    std::vector<int> checks;
-    for (int id : outs)
-        if (present[id]) checks.push_back(id);
-    const int c = int(checks.size());
-    uint8_t* const* sh = reinterpret_cast<uint8_t* const*>(shards);
     std::lock_guard<std::mutex> lock(e->mu);
     if ((rc = e->ensure_device())) return rc;
     cudaStream_t s = pick_stream(e, stream);
     DamageLocator locator;
-    if (c > 0 && (rc = locator.init_rebuild(fused, ins, outs, present, int64_t(n), radius, s, decode))) return rc;
-    // the computed check rows go to scratch a piece at a time, as in damage_device
-    const size_t piece = std::min(n, size_t(256) << 20);
-    StreamScratch scratch(s);
-    if (piece && c > 0) SWEC_CUDA(scratch.alloc(size_t(c) * piece));
-    for (size_t off = 0; off < n && !outs.empty(); off += piece) {
-        const size_t len = std::min(piece, n - off);
-        const uint8_t* in[SWEC_MAX_SHARDS];
-        uint8_t* at[SWEC_MAX_SHARDS];  // information shards, then stored check shards
-        uint8_t* comp[SWEC_MAX_SHARDS];
-        for (int i = 0; i < k; i++) in[i] = at[i] = sh[ins[size_t(i)]] + off;
-        for (int i = 0; i < c; i++) at[k + i] = sh[checks[size_t(i)]] + off;
-        for (size_t o = 0, ci = 0; o < outs.size(); o++)
-            comp[o] = present[outs[o]] ? scratch.as<uint8_t>() + (ci++) * piece : sh[outs[o]] + off;
-        if ((rc = e->apply(fused, in, comp, len, Layout{}, s))) return rc;
-        if (c > 0 && (rc = locator.launch(comp, at, len, int64_t(off), s))) return rc;
-    }
-    SWEC_CUDA(cudaStreamSynchronize(s));
-    if (c == 0) {  // every present shard is an information shard: nothing to check
+    if (plan.c() > 0 && (rc = locator.init_rebuild(plan, int64_t(n), radius, s))) return rc;
+    if ((rc = locate_pieces(e, plan, reinterpret_cast<uint8_t* const*>(shards), n, locator, s))) return rc;
+    if (plan.c() == 0) {  // every present shard is an information shard: nothing to check
         unchecked_report(report, n_ranges);
         return SWEC_OK;
     }

@@ -341,7 +341,7 @@ def test_needle_damage_kernels_in_the_library(swec):
 
 
 def test_locate_kernel_sass_is_unchanged(swec):
-    """damage.cu is untouched: every pinned swec_locate_kernel instantiation has its recorded SASS."""
+    """The locate kernels are untouched: every pinned swec_locate_kernel instantiation has its recorded SASS."""
     from seaweedfs_b200 import _native
     golden = json.load(open(os.path.join(ROOT, "tests", "golden", "locate_kernel_sass.json")))
     cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
