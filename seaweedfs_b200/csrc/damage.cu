@@ -520,7 +520,8 @@ int DamageLocator::init_rebuild(const CheckedPlan& plan, int64_t shard_len, int 
         for (int j = 0; j < k; j++)
             if (const u8 v = fused.at(out_rows_[r], j)) rt.logr[r * 32 + size_t(j)] = log[v];
     SWEC_CUDA(cudaMalloc(reinterpret_cast<void**>(&rtables_), sizeof rt));
-    SWEC_CUDA(cudaMemcpy(rtables_, &rt, sizeof rt, cudaMemcpyHostToDevice));
+    SWEC_CUDA(cudaMemcpyAsync(rtables_, &rt, sizeof rt, cudaMemcpyHostToDevice, s));
+    SWEC_CUDA(cudaStreamSynchronize(s));
     return SWEC_OK;
 }
 

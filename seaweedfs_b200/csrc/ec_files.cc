@@ -196,22 +196,18 @@ double reserve_extents(const std::vector<int>& outs, int64_t size) {
     return PipeStats::now() - t0;
 }
 
-// K input streams + R computed streams per slot, pitch = chunk bytes.
+// K input streams, then `stored` streams read from disk, then R computed streams per slot, pitch = chunk bytes.
 class FilePipeline {
   public:
+    // What runs on each item after the apply: the R computed rows, the slot's K + stored read streams, the item's
+    // columns and shard offset, and the index of its slot, in the slot's stream order.
+    using Step = std::function<int(uint8_t* const* computed, uint8_t* const* shards, size_t len, int64_t base, int slot,
+                                   cudaStream_t s)>;
     PipeStats stats;
-    // With a locator: when set, called on each item in place of the locator's launch, with the computed rows, the
-    // slot's streams, the item's columns and the index of its slot, in the slot's stream order.
-    std::function<int(uint8_t* const* computed, uint8_t* const* shards, size_t len, int64_t base, int slot, cudaStream_t s)>
-        piece_fn;
-    // verify = true: streams [K, K+S) are stored bytes read from disk (S = `stored`, R when negative); the R computed
-    // rows go to streams [K+S, K+S+R) and are only compared on the device (no D2H, no writes) — counted per parity
-    // stream, or, with a locator, decoded into the shards it blames.  A correcting locator also fixes those shards in
-    // the slot, a rebuilding one the rebuilt rows, and the streams the item writes come back to be written.
-    FilePipeline(swec_encoder* enc, const Matrix& rows, size_t chunk, bool verify = false, DamageLocator* locator = nullptr,
-                 int stored = -1)
-        : enc_(enc), rows_(rows), chunk_(chunk), verify_(verify), stored_(verify ? (stored < 0 ? rows.rows : stored) : 0),
-          locator_(locator) {}
+    // Without a step the R computed rows come back to be written.  With one, the streams the item writes (corrected,
+    // rebuilt or computed) come back, once each, after the step.
+    FilePipeline(swec_encoder* enc, const Matrix& rows, size_t chunk, int stored = 0, Step step = {})
+        : enc_(enc), rows_(rows), chunk_(chunk), stored_(stored), step_(std::move(step)) {}
     ~FilePipeline() { shutdown(); }
 
     int start() {
@@ -221,10 +217,6 @@ class FilePipeline {
         if (rc) return rc;
         const size_t nslots = stage_slots();
         const size_t streams = size_t(rows_.cols + stored_ + rows_.rows);
-        if (verify_ && !locator_) {
-            SWEC_CUDA(cudaMalloc(reinterpret_cast<void**>(&dev_bad_), sizeof(unsigned long long) * size_t(rows_.rows)));
-            SWEC_CUDA(cudaMemset(dev_bad_, 0, sizeof(unsigned long long) * size_t(rows_.rows)));
-        }
         // one size for every kind of pipeline of this code on this device (generate: k+m streams, rebuild: k + missing,
         // verify: k+2m, checked rebuild: k + c + m <= k+2m), so that a parked ring fits whichever call comes next
         const size_t slot_bytes = std::max(streams, size_t(enc_->k + 2 * enc_->m)) * chunk_;
@@ -318,13 +310,10 @@ class FilePipeline {
             rc = enc_->apply(rows_, din, dout, len, Layout{}, b.stream);
         }
         if (rc) return set_error(rc, s);
-        if (locator_) {
+        if (step_) {
             uint8_t* shards[SWEC_MAX_SHARDS];
             for (int i = 0; i < K + stored_; i++) shards[i] = b.dev + size_t(i) * chunk_;
-            rc = piece_fn ? piece_fn(dout, shards, len, item.shard_off, int(s - slots_.data()), b.stream)
-                          : locator_->launch(dout, shards, len, item.shard_off, b.stream);
-            if (rc) return set_error(rc, s);
-            // corrected or rebuilt streams that are written: they come back whole, once each
+            if ((rc = step_(dout, shards, len, item.shard_off, int(s - slots_.data()), b.stream))) return set_error(rc, s);
             uint64_t back = 0;
             for (const WriteOp& w : item.writes) {
                 if ((back >> w.stream) & 1) continue;
@@ -333,9 +322,6 @@ class FilePipeline {
                     e = cudaMemcpyAsync(b.host + size_t(w.stream) * chunk_, b.dev + size_t(w.stream) * chunk_, len,
                                         cudaMemcpyDeviceToHost, b.stream);
             }
-        } else if (verify_) {
-            for (int r = 0; r < R && e == cudaSuccess; r++)
-                e = launch_compare(dout[r], b.dev + size_t(K + r) * chunk_, len, dev_bad_ + r, b.stream);
         } else if (len == chunk_) {
             e = cudaMemcpyAsync(b.host + size_t(K) * chunk_, dout[0], size_t(R) * chunk_, cudaMemcpyDeviceToHost, b.stream);
         } else {
@@ -400,19 +386,10 @@ class FilePipeline {
             if (parked.size() < kMaxParkedRings) parked.push_back(std::move(ring_));  // leaves ring_ without slots
         }
         ring_.release();
-        if (dev_bad_) cudaFree(dev_bad_);
-        dev_bad_ = nullptr;
         started_ = false;
     }
 
     size_t slot_count() const { return slots_.size(); }  // after start()
-
-    // verify mode, after finish(): mismatching 16-byte vectors per parity row
-    int mismatches(unsigned long long* out) {
-        if (!dev_bad_) return fail(SWEC_ERR_INVALID_ARG, "not a verify pipeline");
-        SWEC_CUDA(cudaMemcpy(out, dev_bad_, sizeof(unsigned long long) * size_t(rows_.rows), cudaMemcpyDeviceToHost));
-        return SWEC_OK;
-    }
 
   private:
     // Every failure reaches first_ under mu_, here or in the writer loop, and a wake-up follows, so no waiter can test
@@ -485,10 +462,8 @@ class FilePipeline {
     size_t chunk_;
     const size_t io_piece_ = std::max<size_t>(4096, env_size("SWEC_FILE_IO_PIECE", size_t(2) << 20) & ~size_t(4095));
     double t_begin_ = 0;
-    bool verify_ = false;
-    int stored_ = 0;                    // streams read after the K inputs
-    DamageLocator* locator_ = nullptr;  // not owned
-    unsigned long long* dev_bad_ = nullptr;
+    int stored_ = 0;  // streams read after the K inputs
+    Step step_;
     StagingRing ring_;
     std::vector<Slot> slots_;  // one per ring slot
     std::deque<Slot*> free_, inflight_;
@@ -499,6 +474,13 @@ class FilePipeline {
     FirstError first_;      // of submit(), the reader's and writer's I/O tasks and the writer
     bool stop_ = false, started_ = false;
 };
+
+// The step of the damage pipelines: the locator compares, and corrects or rebuilds, in the slot.
+FilePipeline::Step locate_step(DamageLocator& locator) {
+    return [&locator](uint8_t* const* computed, uint8_t* const* shards, size_t len, int64_t base, int, cudaStream_t s) {
+        return locator.launch(computed, shards, len, base, s);
+    };
+}
 
 }  // namespace
 
@@ -539,18 +521,6 @@ int open_shard(const std::string& b, const char* const* dirs, int ndirs, int i, 
     if ((*fd = fds->keep(open(path.c_str(), O_RDONLY))) < 0) return io_fail("open " + path);
     if (dfd) *dfd = fds->keep(open_direct(path, O_RDONLY, direct));
     return SWEC_OK;
-}
-
-int shard_size_error(int64_t expected, int64_t actual) {
-    return fail(SWEC_ERR_SHARD_SIZE, "ec shard size expected " + std::to_string(expected) + " actual " + std::to_string(actual));
-}
-
-// rebuildEcFiles (ec_encoder.go:323-377): every shard has the length of the first one checked (*size < 0: none yet)
-int check_length(int fd, int64_t* size) {
-    struct stat st;
-    if (fstat(fd, &st) != 0) return io_fail("fstat shard");
-    if (*size < 0) *size = st.st_size;
-    return *size == st.st_size ? SWEC_OK : shard_size_error(*size, st.st_size);
 }
 
 // Every shard of the set opened, all of one length: what a parity scrub needs (verify_ec_shards, ec_encoder.rs:177-278).
@@ -636,7 +606,7 @@ int repair_pages(swec_encoder* enc, const Matrix& rows, const std::string& b, co
     }
     const size_t chunk = file_chunk(size);
     DamageLocator locator;
-    FilePipeline pipe(enc, rows, chunk, /*verify=*/true, &locator);
+    FilePipeline pipe(enc, rows, chunk, rows.rows, locate_step(locator));
     int rc = pipe.start();
     if (rc) return rc;
     if ((rc = locator.init(rows, size, radius, enc->stream, /*correct=*/true))) return rc;
@@ -657,13 +627,14 @@ int repair_pages(swec_encoder* enc, const Matrix& rows, const std::string& b, co
 }
 
 // Pass 1 of the damage calls, swec_locate_ec_damage itself: every column of the k+m shard files `in`, all `size` bytes,
-// through a verify pipeline with a locator.  `runs` (may be NULL) receives every page run, for pass 2.
+// through a pipeline that reads the m parity shards too and runs the locator on each slot.  `runs` (may be NULL)
+// receives every page run, for pass 2.
 int locate_pass(swec_encoder* enc, const Matrix& rows, const std::vector<int>& in, int64_t size, int radius,
                 swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges,
                 std::vector<swec_damage_range>* runs) {
     const size_t chunk = file_chunk(size);
     DamageLocator locator;
-    FilePipeline pipe(enc, rows, chunk, /*verify=*/true, &locator);
+    FilePipeline pipe(enc, rows, chunk, rows.rows, locate_step(locator));
     int rc = pipe.start();
     if (rc) return rc;
     rc = locator.init(rows, size, radius, enc->stream);
@@ -709,8 +680,49 @@ struct Checked {
     bool checked = false;  // set once the report comes from a locator (c >= 1)
 };
 
-// Submits an item of a checked pipeline whose length and writes are set, at shard offset `col`.
+// Submits an item whose length is set, at shard offset `col`: the caller adds what else the item needs.
 using SubmitFn = std::function<int(Item&& it, int64_t col)>;
+// Adds what an item needs of one stripe row segment: columns [col, col + len) of the row whose k blocks start at .dat
+// offset row_dat, `block` bytes apart (`tail`: the last, partial small row), at offset src of the item's streams.
+using RowFn = std::function<void(Item& it, int64_t row_dat, int64_t block, bool tail, int64_t col, int64_t len, size_t src)>;
+
+// The items of a .dat's striping (ec_encoder.go:280-321), in order: rows of large blocks cut at the slot size, then the
+// small rows, chunk / small to an item (row by row, cut at the slot size, when a small block is bigger than a slot),
+// the tail row last and `tail_width` columns wide.  No item straddles a row of large blocks.  Every row segment of an
+// item goes to row(), then the item to submit(); the walk stops at the first failed submit and returns its status.
+int walk_items(const StripeGeometry& g, size_t chunk, int64_t tail_width, const RowFn& row, const SubmitFn& submit) {
+    int rc = SWEC_OK;
+    const auto cut = [&](int64_t row_dat, int64_t block, bool tail, int64_t width, int64_t col0) {
+        for (int64_t o = 0; rc == SWEC_OK && o < width; o += int64_t(chunk)) {
+            Item it;
+            it.len = size_t(std::min<int64_t>(int64_t(chunk), width - o));
+            row(it, row_dat, block, tail, o, int64_t(it.len), 0);
+            rc = submit(std::move(it), col0 + o);
+        }
+    };
+    for (int64_t r = 0; r < g.large_rows; r++) cut(r * g.large_row(), g.large, false, g.large, r * g.large);
+    const int64_t nrows = g.small_rows + (g.tail > 0 ? 1 : 0);
+    const auto width = [&](int64_t j) { return j < g.small_rows ? g.small : tail_width; };
+    const auto row_dat = [&](int64_t j) { return g.small_dat_offset() + j * g.small_row(); };
+    const auto col = [&](int64_t j) { return g.small_shard_offset() + j * g.small; };
+    if (g.small > int64_t(chunk)) {
+        for (int64_t j = 0; j < nrows; j++) cut(row_dat(j), g.small, j == g.small_rows, width(j), col(j));
+        return rc;
+    }
+    // Small rows are tiny (10 x 1 MiB): many of them share one slot.  Row j of an item scatters to offset j * small of
+    // its streams, so every shard still takes ONE contiguous run per item.  A default 30,000 MiB volume is 2 large
+    // rows + 952 small ones: a third of its bytes take this path.
+    const int64_t rows_per_item = int64_t(chunk) / g.small;
+    for (int64_t first = 0; rc == SWEC_OK && first < nrows; first += rows_per_item) {
+        Item it;
+        for (int64_t j = first; j < std::min(nrows, first + rows_per_item); j++) {
+            row(it, row_dat(j), g.small, j == g.small_rows, 0, width(j), it.len);
+            it.len += size_t(width(j));
+        }
+        rc = submit(std::move(it), col(first));
+    }
+    return rc;
+}
 
 // The pipeline of the checked rebuild and decode over columns [0, cols) of the shards, after reserving `reserve_size`
 // bytes of each file in `reserve`.  The items `walk` gives, in slots of `chunk` columns, each read the k information
@@ -724,7 +736,7 @@ int checked_pipeline(swec_encoder* enc, const CheckedPlan& plan, const std::vect
     const int k = enc->k, c = plan.c();
     const size_t chunk = file_chunk(cols);
     DamageLocator locator;
-    FilePipeline pipe(enc, plan.fused, chunk, /*verify=*/c > 0, c > 0 ? &locator : nullptr, /*stored=*/c);
+    FilePipeline pipe(enc, plan.fused, chunk, c, c > 0 ? locate_step(locator) : FilePipeline::Step{});
     int rc = pipe.start();
     if (rc) return rc;
     if (c > 0 && (rc = locator.init_rebuild(plan, cols, chk->radius, enc->stream))) return rc;
@@ -859,11 +871,10 @@ int rebuild_files(const char* base, const char* const* dirs, int ndirs, int k, i
     return SWEC_OK;
 }
 
-// The checked decode over columns [0, cols) of the shards.  Its items follow swec_write_dat_file's copy plan: rows of
-// large blocks cut at the slot size, then the small rows, several to a slot as in swec_generate_ec_files, the ragged
-// tail row last; no item straddles a row boundary.  The apply computes the rows of the missing data shards and of the
-// check shards, and the decoding locator also corrects the information streams that are data shards in the slot.  The
-// item's writes un-stripe the k data streams into the .dat at the plan's offsets.
+// The checked decode over columns [0, cols) of the shards, in the items of walk_items() with the tail row as wide as
+// shard 0's part of it.  The apply computes the rows of the missing data shards and of the check shards, and the
+// decoding locator also corrects the information streams that are data shards in the slot.  The item's writes un-stripe
+// the k data streams into the .dat at the plan's offsets; shard s holds tail_bytes(s) of the tail row.
 int decode_dat(swec_encoder* enc, const std::vector<int>& in, const std::vector<int>& in_d,
                const std::vector<uint8_t>& present, int dat, int dat_d, const StripeGeometry& g, int64_t dat_size,
                int64_t cols, Checked* chk) {
@@ -872,46 +883,14 @@ int decode_dat(swec_encoder* enc, const std::vector<int>& in, const std::vector<
     if (!plan.build(enc->gen, k, present.data(), /*decode=*/true)) return fail(SWEC_ERR_TOO_FEW_SHARDS, "not enough shards");
     std::vector<int> stream(static_cast<size_t>(k));  // the slot stream that holds data shard s
     for (int s = 0; s < k; s++) stream[size_t(s)] = plan.position(s);
-    return checked_pipeline(enc, plan, in, in_d, cols, {dat}, dat_size, chk, [&](size_t chunk, const SubmitFn& submit) {
-        // columns [o, o + len) of a row whose blocks start at .dat offset row_dat, `block` bytes apart, taken from
-        // offset src of the item's streams; shard s holds tail_bytes(s) of the tail row
-        auto unstripe = [&](Item& it, int64_t row_dat, int64_t block, bool tail, int64_t o, int64_t len, size_t src) {
-            for (int s = 0; s < k; s++) {
-                const int64_t n = std::min(len, (tail ? g.tail_bytes(s) : block) - o);
-                if (n > 0) it.writes.push_back({stream[size_t(s)], dat, row_dat + int64_t(s) * block + o, src, size_t(n), dat_d});
-            }
-        };
-        int rc = SWEC_OK;
-        for (int64_t r = 0; rc == SWEC_OK && r < g.large_rows; r++)
-            for (int64_t o = 0; rc == SWEC_OK && o < g.large; o += int64_t(chunk)) {
-                Item it;
-                it.len = size_t(std::min<int64_t>(int64_t(chunk), g.large - o));
-                unstripe(it, r * g.large_row(), g.large, false, o, int64_t(it.len), 0);
-                rc = submit(std::move(it), r * g.large + o);
-            }
-        // the small rows, then the tail row, whose columns are the ones shard 0 gives it
-        const int64_t nrows = g.small_rows + (g.tail > 0 ? 1 : 0);
-        auto width = [&](int64_t j) { return j < g.small_rows ? g.small : g.tail_bytes(0); };
-        auto row_dat = [&](int64_t j) { return g.small_dat_offset() + j * g.small_row(); };
-        int64_t j = 0;
-        for (; rc == SWEC_OK && j < nrows && g.small > int64_t(chunk); j++)  // small blocks bigger than a slot: row by row
-            for (int64_t o = 0; rc == SWEC_OK && o < width(j); o += int64_t(chunk)) {
-                Item it;
-                it.len = size_t(std::min<int64_t>(int64_t(chunk), width(j) - o));
-                unstripe(it, row_dat(j), g.small, j == g.small_rows, o, int64_t(it.len), 0);
-                rc = submit(std::move(it), g.small_shard_offset() + j * g.small + o);
-            }
-        const int64_t rows_per_item = std::max<int64_t>(1, int64_t(chunk) / g.small);
-        while (rc == SWEC_OK && j < nrows) {
-            Item it;
-            const int64_t first = j;
-            for (; j < nrows && j - first < rows_per_item; j++) {
-                unstripe(it, row_dat(j), g.small, j == g.small_rows, 0, width(j), it.len);
-                it.len += size_t(width(j));
-            }
-            rc = submit(std::move(it), g.small_shard_offset() + first * g.small);
+    const RowFn unstripe = [&](Item& it, int64_t row_dat, int64_t block, bool tail, int64_t col, int64_t len, size_t src) {
+        for (int s = 0; s < k; s++) {
+            const int64_t n = std::min(len, (tail ? g.tail_bytes(s) : block) - col);
+            if (n > 0) it.writes.push_back({stream[size_t(s)], dat, row_dat + int64_t(s) * block + col, src, size_t(n), dat_d});
         }
-        return rc;
+    };
+    return checked_pipeline(enc, plan, in, in_d, cols, {dat}, dat_size, chk, [&](size_t chunk, const SubmitFn& submit) {
+        return walk_items(g, chunk, g.tail_bytes(0), unstripe, submit);
     });
 }
 
@@ -932,9 +911,8 @@ int needle_damage_files(swec_encoder* enc, const std::vector<int>& in, int64_t s
     const size_t chunk = file_chunk(size);
     DamageLocator locator;
     NeedleDamage nd;
-    FilePipeline pipe(enc, rows, chunk, /*verify=*/true, &locator);
-    pipe.piece_fn = [&](uint8_t* const* computed, uint8_t* const* shards, size_t len, int64_t base, int slot,
-                        cudaStream_t s) -> int {
+    FilePipeline pipe(enc, rows, chunk, rows.rows, [&](uint8_t* const* computed, uint8_t* const* shards, size_t len,
+                                                      int64_t base, int slot, cudaStream_t s) -> int {
         int r = nd.save(shards, len, slot, s);
         if (r == SWEC_OK) r = locator.launch(computed, shards, len, base, s);
         if (r == SWEC_OK) {
@@ -945,7 +923,7 @@ int needle_damage_files(swec_encoder* enc, const std::vector<int>& in, int64_t s
         }
         if (r == SWEC_OK) r = nd.launch(nullptr, shards, computed, len, base, slot, s);
         return r;
-    };
+    });
     if ((rc = pipe.start())) return rc;
     if ((rc = locator.init(rows, size, radius, enc->stream, /*correct=*/true))) return rc;
     if ((rc = nd.init(k, enc->m, map, recs->data(), int(recs->size()), version, int(pipe.slot_count()), chunk, enc->stream)))
@@ -1011,43 +989,16 @@ int swec_generate_ec_files(const char* base, int64_t buffer_size, int64_t large,
     const StripeGeometry g(st.st_size, k, large, small);
     pipe.stats.prealloc += reserve_extents(outs, g.shard_size());
 
-    int64_t processed = 0, shard_off = 0;
-    auto encode_row = [&](int64_t block) -> int {  // encodeData on one row of k blocks, chunk by chunk
-        for (int64_t o = 0; o < block; o += int64_t(chunk)) {
-            Item it;
-            it.len = size_t(std::min<int64_t>(int64_t(chunk), block - o));
-            for (int i = 0; i < k; i++) it.reads.push_back({i, dat, processed + block * i + o, 0, it.len, dat_d});
-            for (int i = 0; i < total; i++) it.writes.push_back({i, outs[size_t(i)], shard_off + o, 0, it.len, outs_d[size_t(i)]});
-            const int r = pipe.submit(std::move(it));
-            if (r) return r;
-        }
-        processed += block * k;
-        shard_off += block;
-        return SWEC_OK;
-    };
-    for (int64_t r = 0; rc == SWEC_OK && r < g.large_rows; r++) rc = encode_row(large);  // ec_encoder.go:304-311
-    // the small rows (ec_encoder.go:312-319); the tail row is read as a whole row, zero past EOF (ec_encoder.go:258-262)
-    int64_t rows_left = g.small_rows + (g.tail > 0 ? 1 : 0);
-    for (; rc == SWEC_OK && rows_left > 0 && small > int64_t(chunk); rows_left--)  // small blocks bigger than a slot: row by row
-        rc = encode_row(small);
-    // Small rows are tiny (10 x 1 MiB): many of them share one slot.  Row j of the
-    // batch is one contiguous k*small run of the .dat whose k blocks scatter to offset j*small of the k input
-    // streams, so every shard still receives ONE contiguous write per item.  A default 30,000 MiB volume is
-    // 2 large rows + 952 small ones — a third of its bytes take this path.
-    const int64_t rows_per_item = std::max<int64_t>(1, int64_t(chunk) / small);
-    while (rc == SWEC_OK && rows_left > 0) {
-        const int64_t n = std::min(rows_per_item, rows_left);
-        Item it;
-        it.len = size_t(n * small);
-        for (int64_t j = 0; j < n; j++)
-            for (int i = 0; i < k; i++)
-                it.reads.push_back({i, dat, processed + j * g.small_row() + int64_t(i) * small, size_t(j * small), size_t(small), dat_d});
-        for (int i = 0; i < total; i++) it.writes.push_back({i, outs[size_t(i)], shard_off, 0, it.len, outs_d[size_t(i)]});
-        rc = pipe.submit(std::move(it));
-        shard_off += n * small;
-        processed += n * g.small_row();
-        rows_left -= n;
-    }
+    // encodeData (ec_encoder.go:304-319): the tail row is read as a whole small row, zero past EOF (ec_encoder.go:258-262)
+    walk_items(
+        g, chunk, small,
+        [&](Item& it, int64_t row_dat, int64_t block, bool, int64_t col, int64_t len, size_t src) {
+            for (int i = 0; i < k; i++) it.reads.push_back({i, dat, row_dat + block * i + col, src, size_t(len), dat_d});
+        },
+        [&](Item&& it, int64_t col) {
+            for (int i = 0; i < total; i++) it.writes.push_back({i, outs[size_t(i)], col, 0, it.len, outs_d[size_t(i)]});
+            return pipe.submit(std::move(it));
+        });
     rc = pipe.finish();  // the first error, submit()'s included
     pipe.report("generate_ec_files");
     const double t_piped = PipeStats::now();
@@ -1097,10 +1048,23 @@ int swec_verify_ec_files(const char* base, const char* const* dirs, int ndirs, i
     if ((rc = open_all_shards(b, dirs, ndirs, k + m, &fds, &in, &size))) return rc;
     const Matrix rows = parity_rows(enc.get());
     const size_t chunk = file_chunk(size);
-    FilePipeline pipe(enc.get(), rows, chunk, /*verify=*/true);
+    // mismatching 16-byte vectors per parity row, zeroed before any slot stream compares into them; declared before
+    // the pipeline so that they are freed only after its shutdown has drained every compare
+    if ((rc = enc->ensure_device())) return rc;
+    StreamScratch dev_bad(enc->stream);
+    const size_t bad_bytes = sizeof(unsigned long long) * size_t(m);
+    SWEC_CUDA(dev_bad.alloc(bad_bytes));
+    SWEC_CUDA(cudaMemsetAsync(dev_bad.p, 0, bad_bytes, enc->stream));
+    SWEC_CUDA(cudaStreamSynchronize(enc->stream));
+    FilePipeline pipe(enc.get(), rows, chunk, m, [&](uint8_t* const* computed, uint8_t* const* shards, size_t len, int64_t,
+                                                     int, cudaStream_t s) -> int {
+        for (int r = 0; r < m; r++) SWEC_CUDA(launch_compare(computed[r], shards[k + r], len, dev_bad.as<unsigned long long>() + r, s));
+        return SWEC_OK;
+    });
     if ((rc = pipe.start())) return rc;
     std::vector<unsigned long long> bad(static_cast<size_t>(m), 0);
-    if ((rc = scrub_columns(pipe, in, size, chunk)) || (rc = pipe.mismatches(bad.data()))) return rc;
+    if ((rc = scrub_columns(pipe, in, size, chunk))) return rc;
+    SWEC_CUDA(cudaMemcpy(bad.data(), dev_bad.p, bad_bytes, cudaMemcpyDeviceToHost));
     bool all_ok = true;
     for (int p = 0; p < m; p++) {
         if (mismatched_vectors) mismatched_vectors[p] = bad[size_t(p)];

@@ -813,13 +813,8 @@ int swec_ec_volume_locate_needle_damage(swec_ec_volume* v, int radius, swec_dama
         if (v->shard_fd[size_t(i)] < 0)
             return fail(SWEC_ERR_TOO_FEW_SHARDS, "locating needle damage needs all shards; missing " + shard_ext(i));
     int64_t size = -1;
-    for (int i = 0; i < total; i++) {
-        struct stat st;
-        if (fstat(v->shard_fd[size_t(i)], &st) != 0) return fail(SWEC_ERR_IO, std::string("fstat shard: ") + strerror(errno));
-        if (size < 0) size = st.st_size;
-        if (st.st_size != size)
-            return fail(SWEC_ERR_SHARD_SIZE, "ec shard size expected " + std::to_string(size) + " actual " + std::to_string(st.st_size));
-    }
+    for (int i = 0; i < total; i++)
+        if ((rc = check_length(v->shard_fd[size_t(i)], &size))) return rc;
     if (v->device < 0) return fail(SWEC_ERR_NO_DEVICE, "no CUDA device: the volume was opened with device < 0");
     // live records: .ecx entries that are not deleted, minus the journalled ids (FindNeedleFromEcx, ec_volume.go:419-429)
     v->refresh_journal();

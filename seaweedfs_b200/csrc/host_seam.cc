@@ -177,11 +177,6 @@ bool constant_pitch(const uint8_t* const* p, int n, size_t min_pitch, size_t* pi
     return true;
 }
 
-struct DeviceCounter {  // verify's count of mismatching vectors
-    unsigned long long* p = nullptr;
-    ~DeviceCounter() { cudaFree(p); }
-};
-
 }  // namespace
 
 int apply_host(swec_encoder_impl* e, const Matrix& rows, const uint8_t* const* in, uint8_t* const* out, size_t n,
@@ -219,11 +214,14 @@ int apply_host(swec_encoder_impl* e, const Matrix& rows, const uint8_t* const* i
     const bool out_2d = !check && b.all_out_direct && R > 1 && constant_pitch(out, R, n, &out_pitch);
     const bool packed = !check && b.all_pageable;
 
-    DeviceCounter dev_bad;
+    // verify's count of mismatching vectors, zeroed before any slot stream compares into it; it outlives run(), which
+    // drains every slot on its way out
+    StreamScratch dev_bad(e->stream);
     const int rc = call.run(chunk, [&](SlotTurns& turns, size_t* next) -> int {
         if (check) {
-            SWEC_CUDA(cudaMalloc(reinterpret_cast<void**>(&dev_bad.p), 8));
-            SWEC_CUDA(cudaMemset(dev_bad.p, 0, 8));
+            SWEC_CUDA(dev_bad.alloc(8));
+            SWEC_CUDA(cudaMemsetAsync(dev_bad.p, 0, 8, e->stream));
+            SWEC_CUDA(cudaStreamSynchronize(e->stream));
         }
         StagingRing& ring = e->ring;
         const size_t stride = e->slot_chunk();  // per-stream pitch inside a slot (>= chunk)
@@ -274,7 +272,7 @@ int apply_host(swec_encoder_impl* e, const Matrix& rows, const uint8_t* const* i
                         uint8_t* theirs = s.dev + size_t(K + R + r) * stride;
                         const uint8_t* src = direct ? out[r] + off : s.host + size_t(K + r) * stride;
                         SWEC_CUDA(cudaMemcpyAsync(theirs, src, len, cudaMemcpyDefault, s.stream));
-                        SWEC_CUDA(launch_compare(dout[r], theirs, len, dev_bad.p, s.stream));
+                        SWEC_CUDA(launch_compare(dout[r], theirs, len, dev_bad.as<unsigned long long>(), s.stream));
                     } else if (direct) {
                         SWEC_CUDA(cudaMemcpyAsync(out[r] + off, dout[r], len, cudaMemcpyDefault, s.stream));
                     } else {

@@ -5,7 +5,9 @@
 #include <libgen.h>
 #include <sys/stat.h>
 
+#include <cerrno>
 #include <cstdio>
+#include <cstring>
 
 #include "engine.h"
 #include "mini_json.h"
@@ -33,6 +35,17 @@ std::string find_shard_file(const std::string& base, const char* const* dirs, in
         if (is_file(cand)) return cand;
     }
     return "";
+}
+
+int shard_size_error(int64_t expected, int64_t actual) {
+    return fail(SWEC_ERR_SHARD_SIZE, "ec shard size expected " + std::to_string(expected) + " actual " + std::to_string(actual));
+}
+
+int check_length(int fd, int64_t* size) {
+    struct stat st;
+    if (fstat(fd, &st) != 0) return fail(SWEC_ERR_IO, std::string("fstat shard: ") + strerror(errno));
+    if (*size < 0) *size = st.st_size;
+    return *size == st.st_size ? SWEC_OK : shard_size_error(*size, st.st_size);
 }
 
 // .vif is protobuf-JSON (weed/storage/volume_info/volume_info.go:73-95); we only need

@@ -59,6 +59,9 @@ bool is_file(const std::string& path);     // exists and is not a directory
 // findShardFile (ec_encoder.go:131-169): <base>.ecNN, else <dir>/<basename(base)>.ecNN for each of the dirs in
 // order; empty when there is none
 std::string find_shard_file(const std::string& base, const char* const* dirs, int ndirs, int i);
+int shard_size_error(int64_t expected, int64_t actual);  // SWEC_ERR_SHARD_SIZE, with the reference's text
+// rebuildEcFiles (ec_encoder.go:323-377): every shard has the length of the first one checked (*size < 0: none yet)
+int check_length(int fd, int64_t* size);
 // ecShardConfig.{dataShards,parityShards} of a .vif file; false when absent/unreadable
 bool read_vif_ratio(const std::string& path, int* ds, int* ps);
 // the EC ratio of a volume: from a valid <base>.vif, else 10+4
