@@ -219,11 +219,7 @@ int swec_check_index_file(const char* path, int needle_version, int64_t* entries
         add("expected an index file of size " + std::to_string(raw.size()) + ", got " + std::to_string(n * kIndexEntrySize));
     *entries = n;
     *n_errors = count;
-    if (errors && errors_cap) {
-        const size_t m = std::min(text.size(), errors_cap - 1);
-        memcpy(errors, text.data(), m);
-        errors[m] = 0;
-    }
+    copy_findings(text, errors, errors_cap);
     return SWEC_OK;
 }
 

@@ -31,7 +31,6 @@
 
 #include "damage.h"
 #include "engine.h"
-#include "mini_json.h"
 #include "needle_damage.h"
 #include "needles.h"
 #include "volume_format.h"
@@ -40,52 +39,17 @@ namespace swec {
 
 namespace {
 
-// SaveVolumeInfo (weed/storage/volume_info/volume_info.go:73-95): protojson with EmitUnpopulated and
-// a two-space indent.  protojson renders 64-bit integers as strings and deliberately does not promise
-// byte-stable whitespace, so readers (ours: read_vif_ratio; Go: protojson.Unmarshal) parse, not compare.
-int save_volume_info(const std::string& path, uint32_t version, int64_t dat_size, uint64_t expire_at_sec, int ds,
-                     int ps) {
-    struct stat st;
-    if (stat(path.c_str(), &st) == 0 && access(path.c_str(), W_OK) != 0)
-        return fail(SWEC_ERR_IO, "failed to check " + path + " not writable");
-    char text[512];
-    const int n = snprintf(text, sizeof text,
-                           "{\n"
-                           "  \"files\": [],\n"
-                           "  \"version\": %u,\n"
-                           "  \"replication\": \"\",\n"
-                           "  \"bytesOffset\": 0,\n"
-                           "  \"datFileSize\": \"%" PRId64 "\",\n"
-                           "  \"expireAtSec\": \"%" PRIu64 "\",\n"
-                           "  \"readOnly\": false,\n"
-                           "  \"ecShardConfig\": {\n"
-                           "    \"dataShards\": %d,\n"
-                           "    \"parityShards\": %d\n"
-                           "  }\n"
-                           "}",
-                           version, dat_size, expire_at_sec, ds, ps);
-    const int fd = open(path.c_str(), O_TRUNC | O_CREAT | O_WRONLY, 0644);
-    if (fd < 0) return fail(SWEC_ERR_IO, "failed to write " + path + ": " + strerror(errno));
-    int put = 0;
-    while (put < n) {
-        const ssize_t w = write(fd, text + put, size_t(n - put));
-        if (w < 0) {
-            if (errno == EINTR) continue;
-            const int e = errno;
-            close(fd);
-            return fail(SWEC_ERR_IO, "failed to write " + path + ": " + strerror(e));
-        }
-        put += int(w);
-    }
-    close(fd);
-    return SWEC_OK;
-}
-
-// A numeric field of a protobuf-JSON .vif (64-bit integers are rendered as strings); false when absent.
-bool vif_number(const std::string& txt, const char* key, int64_t* out) {
-    const std::string k(key);
-    const char* alt = k == "datFileSize" ? "dat_file_size" : k == "expireAtSec" ? "expire_at_sec" : nullptr;
-    return mini_json::top_int(txt, key, alt, out);
+// VolumeEcShardsToVolume's index steps (volume_grpc_erasure_coding.go:621-644): fold .ecj first so deleted needles are
+// not counted live, refuse a volume without live needles, then FindDatFileSize (ec_decoder.go:94-135) with the needle
+// version from the superblock of the shard file `ec00`, or from `version` when there is none
+int decoded_dat_size(const std::string& ib, const std::string& ec00, int version, int64_t* size) {
+    int rc = swec_rebuild_ecx_file(ib.c_str());
+    if (rc) return rc;
+    int live = 0;
+    if ((rc = swec_has_live_needles(ib.c_str(), &live))) return rc;
+    if (!live) return fail(SWEC_ERR_NO_LIVE_NEEDLES, "ec volume has no live entries");  // EcNoLiveEntriesSubstring
+    if (ec00.empty()) return dat_file_size_from_ecx(ib, version, size);
+    return swec_find_dat_file_size(ec00.substr(0, ec00.size() - 5).c_str(), ib.c_str(), size);
 }
 
 }  // namespace
@@ -98,7 +62,7 @@ extern "C" {
 int swec_ec_shards_generate(const char* data_base, const char* index_base, uint32_t needle_version,
                             uint64_t expire_at_sec, int device) {
     if (!data_base) return fail(SWEC_ERR_INVALID_ARG, "data_base_file_name is NULL");
-    const std::string db(data_base), ib(index_base && *index_base ? index_base : data_base);
+    const std::string db(data_base), ib = index_base_of(data_base, index_base, false);
     int k, m;
     ec_ratio(db, &k, &m);
 
@@ -148,9 +112,7 @@ int swec_ec_shards_rebuild(const char* data_base, const char* index_base, const 
     int rc = swec_rebuild_ec_files(data_base, additional_dirs, n_additional_dirs, 0, 0, device, rebuilt, n_rebuilt);
     if (rc) return rc;
     // RebuildEcxFile on the index base, falling back to the data directory (:211-217)
-    std::string ib(index_base && *index_base ? index_base : data_base);
-    if (!is_file(ib + ".ecx") && ib != data_base) ib = data_base;
-    return swec_rebuild_ecx_file(ib.c_str());
+    return swec_rebuild_ecx_file(index_base_of(data_base, index_base, true).c_str());
 }
 
 int swec_ec_shards_to_volume(const char* data_base, const char* index_base, const char* const* additional_dirs,
@@ -166,17 +128,10 @@ int swec_ec_shards_to_volume(const char* data_base, const char* index_base, cons
         if (path.empty()) return fail(SWEC_ERR_TOO_FEW_SHARDS, "ec volume missing shard " + std::to_string(i));
         names.push_back(path);
     }
-    std::string ib(index_base && *index_base ? index_base : data_base);
-    if (!is_file(ib + ".ecx")) ib = db;  // :608-611
-    int rc = swec_rebuild_ecx_file(ib.c_str());  // fold .ecj first so deleted needles are not counted live
-    if (rc) return rc;
-    int live = 0;
-    if ((rc = swec_has_live_needles(ib.c_str(), &live))) return rc;
-    if (!live) return fail(SWEC_ERR_NO_LIVE_NEEDLES, "ec volume has no live entries");  // EcNoLiveEntriesSubstring
+    const std::string ib = index_base_of(data_base, index_base, true);  // :608-611
     int64_t size = 0;
-    // FindDatFileSize reads the needle version from <data_base>.ec00 (ec_decoder.go:94-111)
-    std::string ec00_base = names[0].substr(0, names[0].size() - 5);
-    if ((rc = swec_find_dat_file_size(ec00_base.c_str(), ib.c_str(), &size))) return rc;
+    int rc = decoded_dat_size(ib, names[0], 0, &size);
+    if (rc) return rc;
     std::vector<const char*> cnames;
     for (const auto& s : names) cnames.push_back(s.c_str());
     if ((rc = swec_write_dat_file(db.c_str(), size, cnames.data(), k, kLargeBlockSize, kSmallBlockSize))) return rc;
@@ -207,26 +162,14 @@ int swec_ec_shards_to_volume_checked(const char* data_base, const char* index_ba
     if (found < k)
         return fail(SWEC_ERR_TOO_FEW_SHARDS, "ec volume " + db + " has " + std::to_string(found) + " of its " +
                                                  std::to_string(k + m) + " shards, needs at least " + std::to_string(k));
-    std::string ib(index_base && *index_base ? index_base : data_base);
-    if (!is_file(ib + ".ecx")) ib = db;
+    const std::string ib = index_base_of(data_base, index_base, true);
     // FindDatFileSize reads the needle version from .ec00's superblock; without .ec00, .vif keeps it.  Known before
     // anything is written.
-    int64_t vif_version = 0;
-    if (names[0].empty()) {
-        std::vector<uint8_t> raw;
-        if (read_file(db + ".vif", &raw) || read_file(ib + ".vif", &raw))
-            if (!vif_number(std::string(raw.begin(), raw.end()), "version", &vif_version)) vif_version = 0;
-        if (vif_version <= 0)
-            return fail(SWEC_ERR_TOO_FEW_SHARDS, "ec volume " + db + " has no .ec00 and no needle version in its .vif");
-    }
-    int rc = swec_rebuild_ecx_file(ib.c_str());  // fold .ecj first so deleted needles are not counted live
-    if (rc) return rc;
-    int live = 0;
-    if ((rc = swec_has_live_needles(ib.c_str(), &live))) return rc;
-    if (!live) return fail(SWEC_ERR_NO_LIVE_NEEDLES, "ec volume has no live entries");  // EcNoLiveEntriesSubstring
+    int64_t version = 0;
+    if (names[0].empty() && (version = read_volume_info(db, ib).version) <= 0)
+        return fail(SWEC_ERR_TOO_FEW_SHARDS, "ec volume " + db + " has no .ec00 and no needle version in its .vif");
     int64_t size = 0;
-    if (names[0].empty()) rc = dat_file_size_from_ecx(ib, int(vif_version), &size);
-    else rc = swec_find_dat_file_size(names[0].substr(0, names[0].size() - 5).c_str(), ib.c_str(), &size);
+    int rc = decoded_dat_size(ib, names[0], int(version), &size);
     if (rc) return rc;
     std::vector<const char*> cnames;
     for (const auto& s : names) cnames.push_back(s.empty() ? nullptr : s.c_str());
@@ -257,17 +200,22 @@ struct swec_ec_volume {
     // hundreds of EC volumes; a lookup touches ~25 pages of the page cache (the reference does 25 ReadAt calls)
     const uint8_t* ecx_map = nullptr;
     size_t ecx_bytes = 0;
-    std::vector<uint8_t> ecj;
     std::vector<uint64_t> deleted;  // ids of .ecj, sorted and unique: the reference's in-memory deletedNeedles set
-    int64_t ecj_size_seen = -1, ecj_mtime_ns_seen = 0;
-    uint64_t ecj_inode_seen = 0;
-    void index_journal() {
-        deleted = swec::ecj_ids(ecj);
-        std::sort(deleted.begin(), deleted.end());
-        deleted.erase(std::unique(deleted.begin(), deleted.end()), deleted.end());
-    }
-    void refresh_journal(bool force = false);
+    struct JournalStamp {           // .ecj as deleted last saw it; size -1 = read it again
+        int64_t size = -1, mtime_ns = 0;
+        uint64_t inode = 0;
+    } ecj_seen;
     swec_encoder* enc = nullptr;  // created on the first recovery, keeps its staging ring and kernels
+
+    int64_t entries() const { return int64_t(ecx_bytes) / swec::kIndexEntrySize; }
+    swec::IndexEntry entry(int64_t i) const { return swec::index_entry(ecx_map + i * swec::kIndexEntrySize); }
+    int64_t find(uint64_t id) const { return swec::search_sorted_index(ecx_map, entries(), id); }  // entry number or -1
+    bool journalled(uint64_t id) const { return std::binary_search(deleted.begin(), deleted.end(), id); }
+    static JournalStamp stamp(const struct stat* st) {  // nullptr: there is no journal
+        if (!st) return {0, 0, 0};
+        return {int64_t(st->st_size), int64_t(st->st_mtim.tv_sec) * 1000000000ll + st->st_mtim.tv_nsec, uint64_t(st->st_ino)};
+    }
+    void refresh_journal();
     ~swec_ec_volume() {
         if (ecx_map && ecx_bytes) munmap(const_cast<uint8_t*>(ecx_map), ecx_bytes);
         for (int fd : shard_fd)
@@ -276,21 +224,19 @@ struct swec_ec_volume {
     }
 };
 
-void swec_ec_volume::refresh_journal(bool force) {
+void swec_ec_volume::refresh_journal() {
     // the deletion journal grows while the volume is mounted (DeleteNeedleFromEcx appends to .ecj): pick up new
     // entries when the file moved — size, mtime or inode, so a journal folded and re-created to the same length is
     // seen too — the reference keeps the same set in memory (ec_volume.go:351-384)
     struct stat st;
-    const bool have = stat((index_base + ".ecj").c_str(), &st) == 0;
-    const int64_t now = have ? int64_t(st.st_size) : 0;
-    const int64_t mt = have ? int64_t(st.st_mtim.tv_sec) * 1000000000ll + st.st_mtim.tv_nsec : 0;
-    const uint64_t ino = have ? uint64_t(st.st_ino) : 0;
-    if (!force && now == ecj_size_seen && mt == ecj_mtime_ns_seen && ino == ecj_inode_seen) return;
-    if (now == 0 || !swec::read_file(index_base + ".ecj", &ecj)) ecj.clear();
-    ecj_size_seen = now;
-    ecj_mtime_ns_seen = mt;
-    ecj_inode_seen = ino;
-    index_journal();
+    const JournalStamp now = stamp(stat((index_base + ".ecj").c_str(), &st) == 0 ? &st : nullptr);
+    if (now.size == ecj_seen.size && now.mtime_ns == ecj_seen.mtime_ns && now.inode == ecj_seen.inode) return;
+    std::vector<uint8_t> ecj;  // stays empty when the journal cannot be read
+    if (now.size > 0) swec::read_file(index_base + ".ecj", &ecj);
+    ecj_seen = now;
+    deleted = swec::ecj_ids(ecj);
+    std::sort(deleted.begin(), deleted.end());
+    deleted.erase(std::unique(deleted.begin(), deleted.end()), deleted.end());
 }
 
 extern "C" {
@@ -300,27 +246,18 @@ int swec_ec_volume_open(const char* data_base, const char* index_base, const cha
     if (!out) return fail(SWEC_ERR_INVALID_ARG, "out is NULL");
     *out = nullptr;
     if (!data_base || (n_additional_dirs > 0 && !additional_dirs)) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
-    const std::string db(data_base);
-    std::string ib(index_base && *index_base ? index_base : data_base);
-    if (!is_file(ib + ".ecx")) ib = db;  // NewEcVolume falls back to the data directory (ec_volume.go:72-85)
+    const std::string db(data_base), ib = index_base_of(data_base, index_base, true);
     std::unique_ptr<swec_ec_volume> v(new (std::nothrow) swec_ec_volume());
     if (!v) return fail(SWEC_ERR_NOMEM, "out of memory");
     v->device = device;
     v->index_base = ib;
 
     // what NewEcVolume loads: ratio, needle version and datFileSize from .vif (ec_volume.go:114-154)
-    ec_ratio(db, &v->k, &v->m);
+    const VolumeInfo vif = read_volume_info(db, ib);
+    v->k = vif.k;
+    v->m = vif.m;
+    if (vif.version > 0) v->version = int(vif.version);
     const int total = v->k + v->m;
-    int64_t dat_file_size = 0;
-    {
-        std::vector<uint8_t> raw;
-        if (read_file(db + ".vif", &raw) || read_file(ib + ".vif", &raw)) {
-            const std::string vif(raw.begin(), raw.end());
-            int64_t x = 0;
-            if (vif_number(vif, "version", &x) && x > 0) v->version = int(x);
-            if (vif_number(vif, "datFileSize", &x)) dat_file_size = x;
-        }
-    }
     // local shards: data_base's directory, then the other disks
     v->shard_fd.assign(size_t(total), -1);
     int64_t ecd_file_size = -1;
@@ -340,7 +277,7 @@ int swec_ec_volume_open(const char* data_base, const char* index_base, const cha
     if (nlocal == 0) return fail(SWEC_ERR_TOO_FEW_SHARDS, "ec shard " + db + " not found");
     // LocateEcShardNeedleInterval: .vif's datFileSize is authoritative; old volumes fall back to the
     // shard file size minus one (ec_volume.go:399-417)
-    v->shard_dat_size = dat_file_size > 0 ? dat_file_size / v->k : ecd_file_size - 1;
+    v->shard_dat_size = vif.dat_file_size > 0 ? vif.dat_file_size / v->k : ecd_file_size - 1;
     {
         const int efd = open((ib + ".ecx").c_str(), O_RDONLY);
         if (efd < 0) return fail(SWEC_ERR_IO, "cannot open ec volume index " + ib + ".ecx: " + strerror(errno));
@@ -373,12 +310,7 @@ int swec_ec_volume_read_needles(swec_ec_volume* v, swec_needle_read* reads, int 
     if (!v || (n_reads > 0 && !reads)) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
     std::lock_guard<std::mutex> lock(v->mu);
     const int k = v->k, total = v->k + v->m, version = v->version;
-    const int64_t large = kLargeBlockSize, small = kSmallBlockSize;
-
     v->refresh_journal();
-    const uint8_t* ex = v->ecx_map;
-    const int64_t entries = int64_t(v->ecx_bytes) / kIndexEntrySize;
-    auto journalled = [&](uint64_t id) { return std::binary_search(v->deleted.begin(), v->deleted.end(), id); };
 
     // ---- pass 1: locate every needle, read what is local, collect what must be recovered
     struct Recover {
@@ -390,6 +322,7 @@ int swec_ec_volume_read_needles(swec_ec_volume* v, swec_needle_read* reads, int 
         std::vector<uint8_t> present;
     };
     std::vector<Recover> recs;
+    std::vector<Chunk> chunks;
     for (int r = 0; r < n_reads; r++) {
         swec_needle_read& rd = reads[r];
         rd.offset = 0;
@@ -397,15 +330,15 @@ int swec_ec_volume_read_needles(swec_ec_volume* v, swec_needle_read* reads, int 
         rd.n_bytes = 0;
         rd.n_recovered_intervals = 0;
         rd.status = SWEC_OK;
-        const int64_t found = search_sorted_index(ex, entries, rd.needle_id);
+        const int64_t found = v->find(rd.needle_id);
         if (found < 0) {
             rd.status = SWEC_ERR_NOT_FOUND;
             continue;
         }
-        const IndexEntry entry = index_entry(ex + found * kIndexEntrySize);
+        const IndexEntry entry = v->entry(found);
         const int64_t offset = entry.offset;
         int32_t size = entry.size;
-        if (journalled(rd.needle_id)) size = kTombstone;  // FindNeedleFromEcx (ec_volume.go:419-429)
+        if (v->journalled(rd.needle_id)) size = kTombstone;  // FindNeedleFromEcx (ec_volume.go:419-429)
         rd.offset = offset;
         rd.size = size;
         if (size_deleted(size)) {
@@ -421,18 +354,13 @@ int swec_ec_volume_read_needles(swec_ec_volume* v, swec_needle_read* reads, int 
             rd.status = SWEC_ERR_INVALID_ARG;
             continue;
         }
-        std::vector<swec_interval> ivs(max_intervals(want, small));
-        const int niv = swec_locate_data(large, small, v->shard_dat_size, offset, want, k, ivs.data(), int(ivs.size()));
-        if (niv < 0) {
-            rd.status = niv;
+        if (const int rc = locate_chunks(v->shard_dat_size, k, offset, want, &chunks)) {
+            rd.status = rc;
             continue;
         }
         size_t pos = 0;
-        for (int j = 0; j < niv && rd.status == SWEC_OK; j++) {
-            int sid = 0;
-            int64_t soff = 0;
-            swec_interval_to_shard(&ivs[j], large, small, k, &sid, &soff);
-            const size_t len = size_t(ivs[j].size);
+        for (const auto& [sid, soff, bytes] : chunks) {
+            const size_t len = size_t(bytes);
             bool ok = false;
             if (v->shard_fd[size_t(sid)] >= 0) {  // readLocalEcShardInterval (store_ec.go:407-422): all or nothing
                 const ssize_t got = pread(v->shard_fd[size_t(sid)], rd.buf + pos, len, off_t(soff));
@@ -655,46 +583,31 @@ int scrub_walk(swec_ec_volume* v, NeedleScrub* needles, int64_t* entries, uint32
         if (k2) found.push_back(buf.data()), extra_lines = k2 - 1;
     }
     auto add = [&](const std::string& m) { found.push_back(m); };
-    const int k = v->k, total = v->k + v->m;
-    const int64_t large = kLargeBlockSize, small = kSmallBlockSize;
+    const int total = v->k + v->m;
     std::vector<int64_t> shard_size(size_t(total), -1);
     for (int i = 0; i < total; i++) {
         struct stat st;
         if (v->shard_fd[size_t(i)] >= 0 && fstat(v->shard_fd[size_t(i)], &st) == 0) shard_size[size_t(i)] = st.st_size;
     }
     std::vector<uint8_t> broken(size_t(total), 0), chunk;
-    const uint8_t* ex = v->ecx_map;
-    const int64_t n_entries = int64_t(v->ecx_bytes) / kIndexEntrySize;
+    std::vector<Chunk> chunks;
     int64_t walked = 0;
-    for (int64_t e = 0; e < n_entries; e++) {
+    for (int64_t e = 0; e < v->entries(); e++) {
         walked++;
-        const auto [id, offset, size] = index_entry(ex + e * kIndexEntrySize);
+        const auto [id, offset, size] = v->entry(e);
         if (size == kTombstone) continue;  // Size.IsTombstone
         const int64_t want = needle_actual_size(size, v->version);
-        std::vector<swec_interval> ivs(max_intervals(want, small));
-        const int niv = want > 0 ? swec_locate_data(large, small, v->shard_dat_size, offset, want, k, ivs.data(), int(ivs.size())) : 0;
-        if (niv < 0) return niv;
+        if (const int rc = locate_chunks(v->shard_dat_size, v->k, offset, want, &chunks)) return rc;
         uint8_t* record = nullptr;  // where the record is gathered for the needle check, when all of it is local
-        if (needles && size >= 0) {
-            bool local = true;
-            for (int j = 0; j < niv && local; j++) {
-                int sid = 0;
-                int64_t soff = 0;
-                swec_interval_to_shard(&ivs[size_t(j)], large, small, k, &sid, &soff);
-                local = v->shard_fd[size_t(sid)] >= 0;
-            }
-            if (local) {
-                const int rc = needles->reserve(size_t(want), &record);
-                if (rc) return rc;
-            }
+        if (needles && size >= 0 &&
+            std::all_of(chunks.begin(), chunks.end(), [&](const Chunk& c) { return v->shard_fd[size_t(c.shard)] >= 0; })) {
+            const int rc = needles->reserve(size_t(want), &record);
+            if (rc) return rc;
         }
         int64_t read = 0, pos = 0;
-        for (int j = 0; j < niv; j++) {
-            int sid = 0;
-            int64_t soff = 0;
-            swec_interval_to_shard(&ivs[size_t(j)], large, small, k, &sid, &soff);
-            const int64_t ssize = ivs[size_t(j)].size;
-            const std::string where = std::to_string(j + 1) + "/" + std::to_string(niv);
+        for (size_t j = 0; j < chunks.size(); j++) {
+            const auto [sid, soff, ssize] = chunks[j];
+            const std::string where = std::to_string(j + 1) + "/" + std::to_string(chunks.size());
             uint8_t* dst = record ? record + pos : nullptr;
             pos += ssize;
             if (v->shard_fd[size_t(sid)] < 0) {  // not local: skipped, counted as read
@@ -753,11 +666,7 @@ int scrub_walk(swec_ec_volume* v, NeedleScrub* needles, int64_t* entries, uint32
     for (int i = 0; i < total; i++)
         if (broken[size_t(i)]) broken_shards[(*n_broken)++] = uint32_t(i);
     *n_errors = count;
-    if (errors && errors_cap) {
-        const size_t m = std::min(text.size(), errors_cap - 1);
-        memcpy(errors, text.data(), m);
-        errors[m] = 0;
-    }
+    copy_findings(text, errors, errors_cap);
     return SWEC_OK;
 }
 
@@ -819,10 +728,9 @@ int swec_ec_volume_locate_needle_damage(swec_ec_volume* v, int radius, swec_dama
     // live records: .ecx entries that are not deleted, minus the journalled ids (FindNeedleFromEcx, ec_volume.go:419-429)
     v->refresh_journal();
     std::vector<swec_needle_damage> recs;
-    const int64_t entries = int64_t(v->ecx_bytes) / kIndexEntrySize;
-    for (int64_t e = 0; e < entries; e++) {
-        const IndexEntry x = index_entry(v->ecx_map + e * kIndexEntrySize);
-        if (size_deleted(x.size) || std::binary_search(v->deleted.begin(), v->deleted.end(), x.key)) continue;
+    for (int64_t e = 0; e < v->entries(); e++) {
+        const IndexEntry x = v->entry(e);
+        if (size_deleted(x.size) || v->journalled(x.key)) continue;
         swec_needle_damage r{};
         r.needle_id = x.key;
         r.offset = x.offset;
@@ -852,7 +760,7 @@ int swec_ec_volume_counts(swec_ec_volume* v, uint64_t* file_count, uint64_t* del
     if (!v) return fail(SWEC_ERR_INVALID_ARG, "NULL volume");
     std::lock_guard<std::mutex> lock(v->mu);
     v->refresh_journal();
-    if (file_count) *file_count = uint64_t(v->ecx_bytes / kIndexEntrySize);
+    if (file_count) *file_count = uint64_t(v->entries());
     if (delete_count) *delete_count = uint64_t(v->deleted.size());
     return SWEC_OK;
 }
@@ -863,14 +771,14 @@ int swec_ec_volume_counts(swec_ec_volume* v, uint64_t* file_count, uint64_t* del
 int swec_ec_volume_delete_needle(swec_ec_volume* v, uint64_t needle_id) {
     if (!v) return fail(SWEC_ERR_INVALID_ARG, "NULL volume");
     std::lock_guard<std::mutex> lock(v->mu);
-    const int64_t found = search_sorted_index(v->ecx_map, int64_t(v->ecx_bytes) / kIndexEntrySize, needle_id);
-    if (found < 0) return SWEC_OK;                                                    // already gone
-    if (size_deleted(index_entry(v->ecx_map + found * kIndexEntrySize).size)) return SWEC_OK;  // folded into .ecx by an earlier rebuild
+    const int64_t found = v->find(needle_id);
+    if (found < 0) return SWEC_OK;                          // already gone
+    if (size_deleted(v->entry(found).size)) return SWEC_OK;  // folded into .ecx by an earlier rebuild
     // the in-memory set is authoritative between external changes of the file (refresh_journal notices those by
     // size / mtime / inode): an O(log n) membership test and an 8-byte append per delete, like the reference's map
     // check + append — not a re-read of the whole journal
     v->refresh_journal();
-    if (std::binary_search(v->deleted.begin(), v->deleted.end(), needle_id)) return SWEC_OK;  // idempotent
+    if (v->journalled(needle_id)) return SWEC_OK;  // idempotent
     const std::string path = v->index_base + ".ecj";
     const int fd = open(path.c_str(), O_WRONLY | O_CREAT, 0644);
     if (fd < 0) return fail(SWEC_ERR_IO, "cannot open ec volume journal " + path + ": " + strerror(errno));
@@ -892,15 +800,8 @@ int swec_ec_volume_delete_needle(swec_ec_volume* v, uint64_t needle_id) {
     struct stat after;
     const bool stat_ok = fstat(fd, &after) == 0;
     close(fd);
-    v->ecj.insert(v->ecj.end(), b, b + 8);
     v->deleted.insert(std::upper_bound(v->deleted.begin(), v->deleted.end(), needle_id), needle_id);
-    if (stat_ok) {
-        v->ecj_size_seen = int64_t(after.st_size);
-        v->ecj_mtime_ns_seen = int64_t(after.st_mtim.tv_sec) * 1000000000ll + after.st_mtim.tv_nsec;
-        v->ecj_inode_seen = uint64_t(after.st_ino);
-    } else {
-        v->ecj_size_seen = -1;  // re-read on the next use
-    }
+    v->ecj_seen = stat_ok ? swec_ec_volume::stamp(&after) : swec_ec_volume::JournalStamp{};  // else re-read on the next use
     return SWEC_OK;
 }
 

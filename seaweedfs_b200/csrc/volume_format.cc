@@ -2,10 +2,13 @@
 // (swec_expected_shard_size, swec_locate_data, swec_interval_to_shard).
 #include "volume_format.h"
 
+#include <fcntl.h>
 #include <libgen.h>
 #include <sys/stat.h>
+#include <unistd.h>
 
 #include <cerrno>
+#include <cinttypes>
 #include <cstdio>
 #include <cstring>
 
@@ -48,31 +51,72 @@ int check_length(int fd, int64_t* size) {
     return *size == st.st_size ? SWEC_OK : shard_size_error(*size, st.st_size);
 }
 
-// .vif is protobuf-JSON (weed/storage/volume_info/volume_info.go:73-95); we only need
-// ecShardConfig.{dataShards,parityShards} (weed/pb/volume_server.proto:561-577).
-bool read_vif_ratio(const std::string& path, int* ds, int* ps) {
-    std::vector<uint8_t> raw;
-    if (!read_file(path, &raw)) return false;
-    const std::string txt(raw.begin(), raw.end());
-    int64_t a = 0, b = 0;
-    if (!mini_json::nested_int(txt, "ecShardConfig", "ec_shard_config", "dataShards", "data_shards", &a) ||
-        !mini_json::nested_int(txt, "ecShardConfig", "ec_shard_config", "parityShards", "parity_shards", &b))
-        return false;
-    if (a < 0 || b < 0 || a > 255 || b > 255) return false;
-    *ds = int(a);
-    *ps = int(b);
-    return true;
+std::string index_base_of(const char* data_base, const char* index_base, bool fallback) {
+    const std::string ib(index_base && *index_base ? index_base : data_base);
+    return fallback && !is_file(ib + ".ecx") ? std::string(data_base) : ib;
 }
 
 void ec_ratio(const std::string& base, int* k, int* m) {
-    int ds = 0, ps = 0;
-    if (read_vif_ratio(base + ".vif", &ds, &ps) && ds > 0 && ps > 0 && ds + ps <= SWEC_MAX_SHARDS) {
-        *k = ds;
-        *m = ps;
-    } else {
-        *k = kDefaultDataShards;
-        *m = kDefaultParityShards;
+    const VolumeInfo vi = read_volume_info(base, base);
+    *k = vi.k;
+    *m = vi.m;
+}
+
+VolumeInfo read_volume_info(const std::string& data_base, const std::string& index_base) {
+    std::vector<uint8_t> raw;
+    const bool own = read_file(data_base + ".vif", &raw);
+    std::string txt(raw.begin(), raw.end());
+    // ecShardConfig (weed/pb/volume_server.proto:561-577), when it is a ratio the codec takes
+    int64_t a = 0, b = 0, version = 0, dat_size = 0;
+    const bool ratio = mini_json::nested_int(txt, "ecShardConfig", "ec_shard_config", "dataShards", "data_shards", &a) &&
+                       mini_json::nested_int(txt, "ecShardConfig", "ec_shard_config", "parityShards", "parity_shards", &b) &&
+                       a > 0 && b > 0 && a < SWEC_MAX_SHARDS && b <= SWEC_MAX_SHARDS - a;
+    if (own || read_file(index_base + ".vif", &raw)) {  // 64-bit integers are rendered as strings
+        txt.assign(raw.begin(), raw.end());
+        mini_json::top_int(txt, "version", nullptr, &version);
+        mini_json::top_int(txt, "datFileSize", "dat_file_size", &dat_size);
     }
+    return {ratio ? int(a) : kDefaultDataShards, ratio ? int(b) : kDefaultParityShards, version, dat_size};
+}
+
+// protojson with EmitUnpopulated and a two-space indent.  protojson renders 64-bit integers as strings and deliberately
+// does not promise byte-stable whitespace, so readers (ours: read_volume_info; Go: protojson.Unmarshal) parse, not
+// compare.
+int save_volume_info(const std::string& path, uint32_t version, int64_t dat_size, uint64_t expire_at_sec, int ds, int ps) {
+    struct stat st;
+    if (stat(path.c_str(), &st) == 0 && access(path.c_str(), W_OK) != 0)
+        return fail(SWEC_ERR_IO, "failed to check " + path + " not writable");
+    char text[512];
+    const int n = snprintf(text, sizeof text,
+                           "{\n"
+                           "  \"files\": [],\n"
+                           "  \"version\": %u,\n"
+                           "  \"replication\": \"\",\n"
+                           "  \"bytesOffset\": 0,\n"
+                           "  \"datFileSize\": \"%" PRId64 "\",\n"
+                           "  \"expireAtSec\": \"%" PRIu64 "\",\n"
+                           "  \"readOnly\": false,\n"
+                           "  \"ecShardConfig\": {\n"
+                           "    \"dataShards\": %d,\n"
+                           "    \"parityShards\": %d\n"
+                           "  }\n"
+                           "}",
+                           version, dat_size, expire_at_sec, ds, ps);
+    const int fd = open(path.c_str(), O_TRUNC | O_CREAT | O_WRONLY, 0644);
+    if (fd < 0) return fail(SWEC_ERR_IO, "failed to write " + path + ": " + strerror(errno));
+    int put = 0;
+    while (put < n) {
+        const ssize_t w = write(fd, text + put, size_t(n - put));
+        if (w < 0) {
+            if (errno == EINTR) continue;
+            const int e = errno;
+            close(fd);
+            return fail(SWEC_ERR_IO, "failed to write " + path + ": " + strerror(e));
+        }
+        put += int(w);
+    }
+    close(fd);
+    return SWEC_OK;
 }
 
 int64_t search_sorted_index(const uint8_t* index, int64_t entries, uint64_t key) {
@@ -103,6 +147,27 @@ bool read_file(const std::string& path, std::vector<uint8_t>* out) {
     while ((n = fread(buf, 1, sizeof buf, f)) > 0) out->insert(out->end(), buf, buf + n);
     fclose(f);
     return true;
+}
+
+void copy_findings(const std::string& text, char* errors, size_t errors_cap) {
+    if (!errors || !errors_cap) return;
+    const size_t m = std::min(text.size(), errors_cap - 1);
+    memcpy(errors, text.data(), m);
+    errors[m] = 0;
+}
+
+int locate_chunks(int64_t shard_dat_size, int k, int64_t offset, int64_t size, std::vector<Chunk>* out) {
+    // a read of `size` bytes crosses at most size / small + 2 blocks
+    std::vector<swec_interval> ivs(size_t((size > 0 ? size : 0) / kSmallBlockSize) + 4);
+    const int n = swec_locate_data(kLargeBlockSize, kSmallBlockSize, shard_dat_size, offset, size, k, ivs.data(), int(ivs.size()));
+    out->clear();
+    if (n < 0) return n;
+    for (int j = 0; j < n; j++) {
+        Chunk c{0, 0, ivs[size_t(j)].size};
+        swec_interval_to_shard(&ivs[size_t(j)], kLargeBlockSize, kSmallBlockSize, k, &c.shard, &c.offset);
+        out->push_back(c);
+    }
+    return SWEC_OK;
 }
 
 }  // namespace swec

@@ -49,8 +49,10 @@ struct StripeGeometry {
     int64_t tail_bytes(int i) const { return std::clamp<int64_t>(tail - int64_t(i) * small, 0, small); }
 };
 
-// room for the intervals of a read of `size` bytes: it crosses at most size / small + 2 blocks
-inline size_t max_intervals(int64_t size, int64_t small) { return size_t((size > 0 ? size : 0) / small) + 4; }
+// where a .dat byte range lies: LocateData + ToShardIdAndOffset (ec_locate.go:16-98) on the default block sizes cut the
+// `size` bytes at `offset` into (shard, shard offset, length) pieces, in .dat order; the status is swec_locate_data's
+struct Chunk { int shard; int64_t offset, size; };
+int locate_chunks(int64_t shard_dat_size, int k, int64_t offset, int64_t size, std::vector<Chunk>* out);
 
 // ---- shard files
 
@@ -62,11 +64,20 @@ std::string find_shard_file(const std::string& base, const char* const* dirs, in
 int shard_size_error(int64_t expected, int64_t actual);  // SWEC_ERR_SHARD_SIZE, with the reference's text
 // rebuildEcFiles (ec_encoder.go:323-377): every shard has the length of the first one checked (*size < 0: none yet)
 int check_length(int fd, int64_t* size);
-// ecShardConfig.{dataShards,parityShards} of a .vif file; false when absent/unreadable
-bool read_vif_ratio(const std::string& path, int* ds, int* ps);
-// the EC ratio of a volume: from a valid <base>.vif, else 10+4
-// (volume_grpc_erasure_coding.go:61-77, ec_encoder.go:76-95, ec_volume.go:114-154)
+// the index base a handler works on: index_base when given, else data_base; with `fallback` also data_base when
+// <index_base>.ecx does not exist (NewEcVolume, ec_volume.go:72-85; volume_grpc_erasure_coding.go:211-217,608-611)
+std::string index_base_of(const char* data_base, const char* index_base, bool fallback);
+
+// ---- .vif: protobuf-JSON of VolumeInfo (weed/storage/volume_info/volume_info.go:73-95)
+
+// what NewEcVolume loads from .vif (ec_volume.go:114-154): the EC ratio from a valid <data_base>.vif, else 10+4; the
+// needle version and datFileSize (0 = absent) from <data_base>.vif when it can be opened, else from <index_base>.vif
+struct VolumeInfo { int k, m; int64_t version, dat_file_size; };
+VolumeInfo read_volume_info(const std::string& data_base, const std::string& index_base);
+// the EC ratio of a volume (volume_grpc_erasure_coding.go:61-77, ec_encoder.go:76-95)
 void ec_ratio(const std::string& base, int* k, int* m);
+// SaveVolumeInfo (volume_info.go:73-95), written in place
+int save_volume_info(const std::string& path, uint32_t version, int64_t dat_size, uint64_t expire_at_sec, int ds, int ps);
 
 // ---- index entries: 8-byte needle id, 4-byte offset in units of 8 bytes, 4-byte size, all big-endian
 //      (needle_types.go:58-64, offset_4bytes.go:14-60, needle_map/needle_value.go:24-30)
@@ -102,6 +113,8 @@ int64_t search_sorted_index(const uint8_t* index, int64_t entries, uint64_t key)
 std::vector<uint64_t> ecj_ids(const std::vector<uint8_t>& ecj);
 
 bool read_file(const std::string& path, std::vector<uint8_t>* out);  // the whole file; false when it cannot be opened
+// the findings text of a check into the caller's errors[errors_cap]: cut at errors_cap - 1 bytes and NUL-terminated
+void copy_findings(const std::string& text, char* errors, size_t errors_cap);
 
 // FindDatFileSize (ec_decoder.go:113-135) with the needle version given: the end of the furthest live needle of
 // <index_base>.ecx, at least the superblock

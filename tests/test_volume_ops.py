@@ -3,6 +3,7 @@ VolumeEcShardsToVolume (weed/server/volume_grpc_erasure_coding.go:43-225,578-668
 The CPU tests cover everything that needs no GPU (ec.decode side, ordering, cleanup-on-error, error
 mapping) with shard files written by the oracle; the GPU tests run the full encode → damage → rebuild →
 decode cycle on the reference's fixture volume and compare every produced file with the oracle's."""
+import ctypes as C
 import json
 import os
 
@@ -435,4 +436,190 @@ def test_scrub_local_finds_short_shards(swec, oracle, tmp_path):
     assert 0 < count <= n_entries and broken == [0]
     assert findings[0].startswith("local shard 0 for needle ") and f"is too short ({size0 // 2})" in findings[0]
     assert findings[-1].startswith("expected ") and " bytes for needle " in findings[-1]
+    vol.close()
+
+
+# ---- where the handlers find their index, and what they take from .vif
+
+def split_volume(oracle, tmp_path, seed):
+    """needle_volume with its .ecx in a separate index directory (a server's -dir.idx): (data base, index base, dat,
+    live entries)."""
+    base, dat, live = needle_volume(oracle, tmp_path, seed=seed)
+    (tmp_path / "idx").mkdir()
+    index = str(tmp_path / "idx" / "7")
+    os.rename(base + ".ecx", index + ".ecx")
+    return base, index, dat, live
+
+
+def _reads_ok(vol, dat, live):
+    out = vol.read_needles([key for key, _, _ in live])
+    return all(r["status"] == "SWEC_OK" and (r["bytes"] == expected_record(dat, off * 8, size)).all()
+               for (_, off, size), r in zip(live, out))
+
+
+def test_handlers_use_a_given_index_base(swec, oracle, tmp_path):
+    """With .ecx under the index base, the mount reads and journals there, the rebuild folds .ecj there, the decode
+    writes .idx there, and generate reads .idx from there (it is about to write .ecx, so it never falls back)."""
+    ec = swec.erasure_coding
+    base, index, dat, live = split_volume(oracle, tmp_path, seed=71)
+    ecx = open(index + ".ecx", "rb").read()
+    vol = ec.EcVolume(base, index, device=-1)
+    assert vol.info()["shard_dat_size"] == len(dat) // 10 and _reads_ok(vol, dat, live[:40])
+    vol.delete_needle(live[0][0])
+    assert open(index + ".ecj", "rb").read() == live[0][0].to_bytes(8, "big") and not os.path.exists(base + ".ecj")
+    vol.close()
+
+    assert ec.VolumeEcShardsRebuild(base, index, device=-1) == []          # nothing missing: only the .ecj fold
+    folded = rn.fold_ecj_into_ecx(ecx, live[0][0].to_bytes(8, "big"))
+    assert open(index + ".ecx", "rb").read() == folded and not os.path.exists(index + ".ecj")
+
+    open(index + ".ecj", "wb").write(live[1][0].to_bytes(8, "big"))
+    size = ec.VolumeEcShardsToVolume(base, index)
+    folded = rn.fold_ecj_into_ecx(folded, live[1][0].to_bytes(8, "big"))
+    assert size == rn.find_dat_file_size(folded, 3) and (np.fromfile(base + ".dat", dtype=np.uint8) == dat[:size]).all()
+    assert open(index + ".idx", "rb").read() == rn.idx_from_ec_index(folded, b"") and not os.path.exists(base + ".idx")
+
+    gen = tmp_path / "gen"
+    (gen / "idx").mkdir(parents=True)
+    gdat, gidx = synthetic_volume(seed=3, needles=20)
+    gdat.tofile(str(gen / "9.dat"))
+    open(str(gen / "idx" / "9.idx"), "wb").write(gidx)
+    with pytest.raises(swec.SwecError) as e:                              # past the .ecx step, stopped by the device
+        ec.VolumeEcShardsGenerate(str(gen / "9"), str(gen / "idx" / "9"), device=-1)
+    assert e.value.name == "SWEC_ERR_NO_DEVICE"
+    assert sorted(os.listdir(gen)) == ["9.dat", "idx"] and os.listdir(gen / "idx") == ["9.idx"]
+
+
+def test_handlers_fall_back_to_the_data_base_without_index_ecx(swec, oracle, tmp_path):
+    """An index base without .ecx is passed over for the data base by the mount, the rebuild and the decode; a journal
+    lying under the index base is neither read nor folded."""
+    ec = swec.erasure_coding
+    base, dat, live = needle_volume(oracle, tmp_path, seed=73)
+    (tmp_path / "idx").mkdir()
+    index = str(tmp_path / "idx" / "7")
+    stray = live[2][0].to_bytes(8, "big")
+    open(index + ".ecj", "wb").write(stray)
+    ecx = open(base + ".ecx", "rb").read()
+    vol = ec.EcVolume(base, index, device=-1)
+    assert _reads_ok(vol, dat, live[:40])
+    vol.delete_needle(live[0][0])
+    assert open(base + ".ecj", "rb").read() == live[0][0].to_bytes(8, "big")
+    vol.close()
+
+    assert ec.VolumeEcShardsRebuild(base, index, device=-1) == []
+    folded = rn.fold_ecj_into_ecx(ecx, live[0][0].to_bytes(8, "big"))
+    assert open(base + ".ecx", "rb").read() == folded and not os.path.exists(base + ".ecj")
+
+    size = ec.VolumeEcShardsToVolume(base, index)
+    assert size == rn.find_dat_file_size(folded, 3) and (np.fromfile(base + ".dat", dtype=np.uint8) == dat[:size]).all()
+    assert open(base + ".idx", "rb").read() == rn.idx_from_ec_index(folded, b"")
+    assert os.listdir(tmp_path / "idx") == ["7.ecj"] and open(index + ".ecj", "rb").read() == stray
+
+
+def test_vif_precedence_between_data_and_index_base(swec, oracle, tmp_path):
+    """NewEcVolume's .vif: the ratio comes from <data_base>.vif alone; the needle version and datFileSize come from
+    <data_base>.vif whenever it can be opened, even without those fields, and from <index_base>.vif only otherwise."""
+    ec = swec.erasure_coding
+    base, index, dat, _ = split_volume(oracle, tmp_path, seed=79)
+    shard = os.path.getsize(base + ".ec00")
+
+    def info():
+        vol = ec.EcVolume(base, index, device=-1)
+        got = vol.info()
+        vol.close()
+        return got["data_shards"], got["parity_shards"], got["version"], got["shard_dat_size"]
+
+    json.dump({"version": 1, "datFileSize": "7000000", "ecShardConfig": {"dataShards": 6, "parityShards": 3}},
+              open(index + ".vif", "w"))
+    json.dump({"version": 2, "datFileSize": str(len(dat)), "ecShardConfig": {"dataShards": 12, "parityShards": 2}},
+              open(base + ".vif", "w"))
+    assert info() == (12, 2, 2, len(dat) // 12)
+    os.remove(base + ".vif")
+    assert info() == (10, 4, 1, 7000000 // 10)                            # the index base's .vif has no say in the ratio
+    json.dump({"ecShardConfig": {"dataShards": 12, "parityShards": 2}}, open(base + ".vif", "w"))
+    assert info() == (12, 2, 3, shard - 1)
+
+
+def test_checked_decode_with_a_given_index_base(swec, oracle, tmp_path):
+    """swec_ec_shards_to_volume_checked from the k data shard files alone (a host copy: no GPU) with .ecx under its own
+    base writes what the plain decode writes, .idx under the index base.  Without .ec00 the needle version comes from
+    the data base's .vif, else the index base's; with none the call stops before it writes or folds anything."""
+    ec = swec.erasure_coding
+    base, index, dat, live = split_volume(oracle, tmp_path, seed=83)
+    for i in range(10, 14):
+        os.remove(base + ".ec%02d" % i)
+    ecj = live[0][0].to_bytes(8, "big")
+    open(index + ".ecj", "wb").write(ecj)
+    folded = rn.fold_ecj_into_ecx(open(index + ".ecx", "rb").read(), ecj)
+    res = ec.ec_shards_to_volume_checked(base, index, device=-1)
+    size = res["dat_file_size"]
+    assert res["ok"] is False and res["columns"] == 0 and size == rn.find_dat_file_size(folded, 3)
+    assert (np.fromfile(base + ".dat", dtype=np.uint8) == dat[:size]).all()
+    assert open(index + ".idx", "rb").read() == rn.idx_from_ec_index(folded, b"") and not os.path.exists(base + ".idx")
+
+    (tmp_path / "b").mkdir()
+    base, index, dat, live = split_volume(oracle, tmp_path / "b", seed=89)
+    os.remove(base + ".ec00")
+    os.remove(base + ".vif")
+    open(index + ".ecj", "wb").write(ecj)
+    ecx = open(index + ".ecx", "rb").read()
+
+    def refused(what):
+        with pytest.raises(swec.SwecError) as e:
+            ec.ec_shards_to_volume_checked(base, index, device=-1)
+        assert str(e.value) == "SWEC_ERR_TOO_FEW_SHARDS: ec volume %s has no .ec00 and no needle version in its .vif" % base, what
+        assert open(index + ".ecx", "rb").read() == ecx and open(index + ".ecj", "rb").read() == ecj, what
+        assert not any(os.path.exists(b + x) for b in (base, index) for x in (".dat", ".idx")), what
+
+    refused("no .vif")
+    json.dump({"ecShardConfig": {"dataShards": 10, "parityShards": 4}}, open(base + ".vif", "w"))
+    json.dump({"version": 3}, open(index + ".vif", "w"))
+    refused("the data base's .vif has no version")                      # the index base's is not consulted
+    os.remove(base + ".vif")
+    with pytest.raises(swec.SwecError) as e:                              # the index base's version: on to the device
+        ec.ec_shards_to_volume_checked(base, index, device=-1)
+    assert e.value.name == "SWEC_ERR_NO_DEVICE"
+    assert not any(os.path.exists(b + x) for b in (base, index) for x in (".dat", ".idx"))
+
+
+def _cut(L, call, cap):
+    """call(buf, cap, n_errors) into a buffer of cap + 8 bytes of 0xAA: (bytes, n_errors)."""
+    buf = C.create_string_buffer(b"\xaa" * (cap + 8), cap + 8)
+    n = C.c_int(-1)
+    assert call(buf if cap else None, cap, C.byref(n)) == 0, L.swec_last_error()
+    return buf.raw, n.value
+
+
+def test_findings_are_cut_at_errors_cap(swec, oracle, tmp_path):
+    """The findings of scrub_local and check_index_file are cut at errors_cap - 1 bytes and NUL-terminated, the rest of
+    the buffer untouched; n_errors still counts every finding."""
+    ec = swec.erasure_coding
+    L = swec.lib()
+    base, dat, live = needle_volume(oracle, tmp_path, seed=97)
+    os.truncate(base + ".ec00", os.path.getsize(base + ".ec00") // 2)
+    vol = ec.EcVolume(base, device=-1)
+    _, _, findings = vol.scrub_local()
+    broken, nb, entries = (C.c_uint32 * 32)(), C.c_int(0), C.c_int64(0)
+
+    def scrub(buf, cap, n):
+        return L.swec_ec_volume_scrub_local(vol._h, C.byref(entries), broken, C.byref(nb), buf, cap, n)
+
+    index = str(tmp_path / "over.ecx")                                   # two overlaps and a partial entry: 3 findings
+    open(index, "wb").write(rn._entry(1, 1, 100) + rn._entry(2, 2, 100) + rn._entry(3, 3, 100) + b"\0" * 5)
+    _, lines = ec.check_index_file(index)
+
+    def check(buf, cap, n):
+        return L.swec_check_index_file(index.encode(), 3, C.byref(entries), buf, cap, n)
+
+    for call, found in ((scrub, findings), (check, lines)):
+        full = "\n".join(found).encode()
+        assert len(found) >= 2 and len(full) > 40
+        for cap in (0, 1, 2, 40, len(full), len(full) + 1, len(full) + 2):
+            raw, n = _cut(L, call, cap)
+            assert n == len(found), (cap, n)
+            if cap:
+                cut = min(len(full), cap - 1)
+                assert raw[:cut] == full[:cut] and raw[cut] == 0 and raw[cut + 1:] == b"\xaa" * (cap + 7 - cut), cap
+            else:
+                assert raw == b"\xaa" * 8
     vol.close()
