@@ -60,17 +60,10 @@ unsigned long long aot_recon_launches() { return g_aot_launches.load(); }
 cudaError_t launch_aot_recon(int idx, const SwecApplyParams& p, cudaStream_t s) {
     if (p.nvec == 0) return cudaSuccess;
     if (idx < 0 || idx >= SWEC_AOT_RECON_COUNT) return cudaErrorInvalidValue;
-    int sms = 132, dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const u64 per_cta = u64(kAotThreads) * kAotUnroll;
-    const u64 need = (p.nvec + per_cta - 1) / per_cta;
     // light kernels (one output row: few registers) fit two CTAs per SM; the 4-row worst case one, like encode
-    const u64 cap = u64(sms) * (kAotReconKeys[idx].r >= 3 ? 1 : 2);
-    const unsigned grid = unsigned(need < cap ? need : cap);
+    const unsigned grid = grid_for(p.nvec, u64(kAotThreads) * kAotUnroll, kAotReconKeys[idx].r >= 3 ? 1 : 2);
     const bool lp = low_power_now();
     note_kernel_work(double(p.nvec) * 16.0 * double(kAotReconKeys[idx].k + kAotReconKeys[idx].r) / 3.0e12 * 1e3);
-    g_kernel_launches++;
     g_aot_launches++;
     switch (idx) {
 #define SWEC_AOT_CASE(I)                                                                              \
@@ -82,7 +75,7 @@ cudaError_t launch_aot_recon(int idx, const SwecApplyParams& p, cudaStream_t s) 
 #undef SWEC_AOT_CASE
         default: return cudaErrorInvalidValue;
     }
-    return cudaGetLastError();
+    return launched();
 }
 
 }  // namespace swec

@@ -371,17 +371,24 @@ __global__ void __launch_bounds__(256) swec_locate_kernel(const __grid_constant_
 
 template <int MT, int MODE>
 unsigned locate_grid(u64 n) {
-    static int per_sm = 0;  // resident CTAs per SM, the same on every device of this architecture
-    if (!per_sm &&
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, swec_locate_kernel<MT, MODE>, 256, 0) != cudaSuccess) {
-        cudaGetLastError();
-        per_sm = 4;
+    static const int per_sm = [] {  // resident CTAs per SM, the same on every device of this architecture
+        int c = 0;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, swec_locate_kernel<MT, MODE>, 256, 0) != cudaSuccess) {
+            cudaGetLastError();
+            c = 4;
+        }
+        return std::max(1, c);
+    }();
+    return grid_cap((n / 16 + 255) / 256 + 1, per_sm);
+}
+
+// The instantiation for m among the compiled-in MT values of MODE, else the run-time m one (MT = 0).
+template <int MODE, int MT = 0, int... MORE>
+void launch_locate(int m, const LocateParams& p, u64 n, cudaStream_t s) {
+    if constexpr (MT != 0) {
+        if (m != MT) return launch_locate<MODE, MORE...>(m, p, n, s);
     }
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const u64 need = (n / 16 + 255) / 256 + 1;
-    return unsigned(std::min<u64>(need, u64(sms) * u64(std::max(1, per_sm))));
+    swec_locate_kernel<MT, MODE><<<locate_grid<MT, MODE>(n), 256, 0, s>>>(p);
 }
 
 // logs of the field's non-zero bytes (to base 2), and two periods of powers of 2
@@ -459,13 +466,6 @@ int CheckedPlan::position(int id) const {
     return -1;
 }
 
-DamageLocator::~DamageLocator() {
-    if (rtables_) cudaFree(rtables_);
-    if (tables_) cudaFree(tables_);
-    if (counters_) cudaFree(counters_);
-    if (pages_) cudaFree(pages_);
-}
-
 int DamageLocator::init(const Matrix& parity, int64_t shard_len, int radius, cudaStream_t s, bool correct) {
     k_ = parity.cols;
     m_ = parity.rows;
@@ -487,14 +487,13 @@ int DamageLocator::init(const Matrix& parity, int64_t shard_len, int radius, cud
     const int64_t pages = (shard_len + (int64_t(1) << kPageShift) - 1) >> kPageShift;
     page_words_ = std::max<size_t>(1, size_t((pages + 31) / 32));
     const size_t page_bytes = size_t(k_ + m_ + 1) * page_words_ * 4;
-    SWEC_CUDA(cudaMalloc(reinterpret_cast<void**>(&tables_), sizeof t));
-    SWEC_CUDA(cudaMalloc(reinterpret_cast<void**>(&counters_), kCounters * sizeof(unsigned long long)));
-    SWEC_CUDA(cudaMalloc(reinterpret_cast<void**>(&pages_), page_bytes));
-    SWEC_CUDA(cudaMemcpyAsync(tables_, &t, sizeof t, cudaMemcpyHostToDevice, s));
-    SWEC_CUDA(cudaMemsetAsync(counters_, 0, kCounters * sizeof(unsigned long long), s));
-    SWEC_CUDA(cudaMemsetAsync(counters_ + kSets, 0xff, kSets * sizeof(unsigned long long), s));  // first = max
-    SWEC_CUDA(cudaMemsetAsync(pages_, 0, page_bytes, s));
-    SWEC_CUDA(cudaStreamSynchronize(s));
+    SWEC_CUDA(counters_.alloc(kCounters * sizeof(unsigned long long)));
+    SWEC_CUDA(pages_.alloc(page_bytes));
+    unsigned long long* ctr = counters_.as<unsigned long long>();
+    SWEC_CUDA(cudaMemsetAsync(ctr, 0, kCounters * sizeof(unsigned long long), s));
+    SWEC_CUDA(cudaMemsetAsync(ctr + kSets, 0xff, kSets * sizeof(unsigned long long), s));  // first = max
+    SWEC_CUDA(cudaMemsetAsync(pages_.as<void>(), 0, page_bytes, s));
+    SWEC_CUDA(tables_.upload(&t, 1, s));  // synchronises s, after the clears
     return SWEC_OK;
 }
 
@@ -519,9 +518,7 @@ int DamageLocator::init_rebuild(const CheckedPlan& plan, int64_t shard_len, int 
     for (size_t r = 0; r < out_rows_.size(); r++)
         for (int j = 0; j < k; j++)
             if (const u8 v = fused.at(out_rows_[r], j)) rt.logr[r * 32 + size_t(j)] = log[v];
-    SWEC_CUDA(cudaMalloc(reinterpret_cast<void**>(&rtables_), sizeof rt));
-    SWEC_CUDA(cudaMemcpyAsync(rtables_, &rt, sizeof rt, cudaMemcpyHostToDevice, s));
-    SWEC_CUDA(cudaStreamSynchronize(s));
+    SWEC_CUDA(rtables_.upload(&rt, 1, s));
     return SWEC_OK;
 }
 
@@ -538,7 +535,7 @@ int DamageLocator::launch(uint8_t* const* computed, uint8_t* const* shards, size
     if (rebuild_) {
         for (size_t r = 0; r < out_rows_.size(); r++) p.fix[r] = computed[out_rows_[r]];
         p.nout = int(out_rows_.size());
-        p.rtables = rtables_;
+        p.rtables = rtables_.as<u32>();
     }
     if (decode_)  // nout + k <= k + m slots: the rebuilt streams are missing data shards
         for (int j = 0; j < k_; j++) p.fix[p.nout + j] = ids_[size_t(j)] < k_ ? shards[j] : nullptr;
@@ -547,36 +544,25 @@ int DamageLocator::launch(uint8_t* const* computed, uint8_t* const* shards, size
     p.k = k_;
     p.m = m_;
     p.radius = radius_;
-    p.tables = tables_;
-    p.ctr = counters_;
-    p.pages = pages_;
+    p.tables = tables_.as<u32>();
+    p.ctr = counters_.as<unsigned long long>();
+    p.pages = pages_.as<u32>();
     p.page_words = page_words_;
-    if (decode_) {
-        if (m_ == 4) swec_locate_kernel<4, kDecode><<<locate_grid<4, kDecode>(n), 256, 0, s>>>(p);
-        else if (m_ == 3) swec_locate_kernel<3, kDecode><<<locate_grid<3, kDecode>(n), 256, 0, s>>>(p);
-        else swec_locate_kernel<0, kDecode><<<locate_grid<0, kDecode>(n), 256, 0, s>>>(p);
-    } else if (rebuild_) {
-        if (m_ == 3) swec_locate_kernel<3, kRebuild><<<locate_grid<3, kRebuild>(n), 256, 0, s>>>(p);
-        else swec_locate_kernel<0, kRebuild><<<locate_grid<0, kRebuild>(n), 256, 0, s>>>(p);
-    } else if (correct_) {
-        if (m_ == 4) swec_locate_kernel<4, kCorrect><<<locate_grid<4, kCorrect>(n), 256, 0, s>>>(p);
-        else swec_locate_kernel<0, kCorrect><<<locate_grid<0, kCorrect>(n), 256, 0, s>>>(p);
-    } else {
-        if (m_ == 4) swec_locate_kernel<4, kLocate><<<locate_grid<4, kLocate>(n), 256, 0, s>>>(p);
-        else swec_locate_kernel<0, kLocate><<<locate_grid<0, kLocate>(n), 256, 0, s>>>(p);
-    }
-    g_kernel_launches++;
-    SWEC_CUDA(cudaGetLastError());
+    if (decode_) launch_locate<kDecode, 4, 3>(m_, p, n, s);
+    else if (rebuild_) launch_locate<kRebuild, 3>(m_, p, n, s);
+    else if (correct_) launch_locate<kCorrect, 4>(m_, p, n, s);
+    else launch_locate<kLocate, 4>(m_, p, n, s);
+    SWEC_CUDA(launched());
     return SWEC_OK;
 }
 
 int DamageLocator::collect(swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges,
                            std::vector<swec_damage_range>* all) {
     const int n = k_ + m_;
-    std::vector<unsigned long long> c(kCounters);
-    std::vector<uint32_t> bits(size_t(n + 1) * page_words_);
-    SWEC_CUDA(cudaMemcpy(c.data(), counters_, c.size() * sizeof c[0], cudaMemcpyDeviceToHost));
-    SWEC_CUDA(cudaMemcpy(bits.data(), pages_, bits.size() * 4, cudaMemcpyDeviceToHost));
+    std::vector<unsigned long long> c;
+    std::vector<uint32_t> bits;  // n + 1 page bitmaps
+    SWEC_CUDA(counters_.read(&c));
+    SWEC_CUDA(pages_.read(&bits));
     unchecked_report(report, nullptr);
     report->columns = uint64_t(shard_len_);
     report->damaged_columns = c[3 * kSets];

@@ -9,6 +9,7 @@
 #include <vector>
 
 #include "../../include/swec.h"
+#include "engine.h"
 #include "gf256.h"
 
 namespace swec {
@@ -50,7 +51,6 @@ class DamageLocator {
     DamageLocator() = default;
     DamageLocator(const DamageLocator&) = delete;
     DamageLocator& operator=(const DamageLocator&) = delete;
-    ~DamageLocator();
 
     // parity: the m x k parity rows of the code.  correct: every launch also replaces the blamed bytes of the columns it
     // decodes within the radius by their decoded values.  Clears the counters on `s` and synchronises it.
@@ -81,10 +81,10 @@ class DamageLocator {
     std::vector<int> check_rows_, out_rows_;  // rebuild mode: rows of `computed` that are check shards / rebuilt shards
     int64_t shard_len_ = 0;
     size_t page_words_ = 0;  // 32-bit words of one page bitmap
-    uint32_t* tables_ = nullptr;
-    unsigned long long* counters_ = nullptr;
-    uint32_t* pages_ = nullptr;
-    uint32_t* rtables_ = nullptr;  // rebuild mode: log R
+    DeviceBuffer tables_;    // LocateTables
+    DeviceBuffer counters_;  // unsigned long long: bytes, first and last of every set, damaged columns
+    DeviceBuffer pages_;     // uint32_t: one page bitmap per set
+    DeviceBuffer rtables_;   // rebuild mode: RebuildTables (log R)
 };
 
 }  // namespace swec

@@ -80,11 +80,7 @@ std::atomic<long> g_opt_jit_min_bytes{long(env_size("SWEC_JIT_MIN_BYTES", size_t
 
 swec_encoder_impl::~swec_encoder_impl() {
     if (device < 0) return;
-    if (cudaSetDevice(device) != cudaSuccess) return;
-    for (auto& kv : tables) {
-        cudaFree(kv.second.compact);
-        cudaFree(kv.second.replicated);
-    }
+    if (cudaSetDevice(device) != cudaSuccess) return;  // the tables are freed after this body, on `device`
     ring.release();
     if (stream) cudaStreamDestroy(stream);
 }
@@ -115,11 +111,11 @@ static std::vector<uint8_t> matrix_key(const Matrix& rows) {
     return key;
 }
 
-int swec_encoder_impl::get_tables(const Matrix& rows, DeviceTables* out, cudaStream_t s) {
+int swec_encoder_impl::get_tables(const Matrix& rows, const DeviceTables** out, cudaStream_t s) {
     const auto key = matrix_key(rows);
     auto it = tables.find(key);
     if (it != tables.end()) {
-        *out = it->second;
+        *out = &it->second;
         return SWEC_OK;
     }
     const GF& gf = GF::get();
@@ -135,14 +131,9 @@ int swec_encoder_impl::get_tables(const Matrix& rows, DeviceTables* out, cudaStr
                 for (int lane = 0; lane < 32; lane++) repl[e * 32 + size_t(lane)] = w;
             }
     DeviceTables t;
-    SWEC_CUDA(cudaMalloc(reinterpret_cast<void**>(&t.compact), compact.size() * 4));
-    SWEC_CUDA(cudaMalloc(reinterpret_cast<void**>(&t.replicated), repl.size() * 4));
-    // synchronous copies from pageable memory: the vectors die at return
-    SWEC_CUDA(cudaMemcpyAsync(t.compact, compact.data(), compact.size() * 4, cudaMemcpyHostToDevice, s));
-    SWEC_CUDA(cudaMemcpyAsync(t.replicated, repl.data(), repl.size() * 4, cudaMemcpyHostToDevice, s));
-    SWEC_CUDA(cudaStreamSynchronize(s));
-    tables[key] = t;
-    *out = t;
+    SWEC_CUDA(t.compact.upload(compact.data(), compact.size(), s));
+    SWEC_CUDA(t.replicated.upload(repl.data(), repl.size(), s));
+    *out = &(tables[key] = std::move(t));
     return SWEC_OK;
 }
 
@@ -196,12 +187,12 @@ int swec_encoder_impl::apply(const Matrix& rows, const uint8_t* const* in, uint8
             const int rn = std::min(4, R - r0);
             Matrix sub(rn, K);
             memcpy(sub.v.data(), rows.row(r0), size_t(rn) * size_t(K));
-            DeviceTables t;
+            const DeviceTables* t;
             if (const int rc = get_tables(sub, &t, s)) return rc;
             SwecApplyParams p;
             fill(p, r0, rn, byte_tail ? tail_off : 0);
-            if (byte_tail) SWEC_CUDA(launch_bytes_apply(p, t.compact, K, rn, tail, s));
-            else SWEC_CUDA(launch_table_apply(p, t.replicated, K, rn, s));
+            if (byte_tail) SWEC_CUDA(launch_bytes_apply(p, t->compact.as<u32>(), K, rn, tail, s));
+            else SWEC_CUDA(launch_table_apply(p, t->replicated.as<u32>(), K, rn, s));
         }
         return SWEC_OK;
     };

@@ -13,6 +13,7 @@
 #include <memory>
 #include <mutex>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/swec.h"
@@ -48,6 +49,44 @@ struct StreamScratch {
     template <class T> T* as() const { return static_cast<T*>(p); }
 };
 
+// Device memory that outlives any one stream: plain cudaMalloc, and cudaFree (on the current device) when the owner
+// goes.  A failed alloc or upload leaves nothing to free by hand.
+class DeviceBuffer {
+  public:
+    DeviceBuffer() = default;
+    DeviceBuffer(DeviceBuffer&& o) noexcept : p_(o.p_), bytes_(o.bytes_) { o.p_ = nullptr; }
+    DeviceBuffer& operator=(DeviceBuffer&& o) noexcept {
+        std::swap(p_, o.p_);
+        std::swap(bytes_, o.bytes_);
+        return *this;
+    }
+    ~DeviceBuffer() { if (p_) cudaFree(p_); }
+
+    cudaError_t alloc(size_t bytes) {
+        *this = DeviceBuffer();
+        void* p = nullptr;
+        const cudaError_t e = cudaMalloc(&p, bytes);
+        if (e == cudaSuccess) p_ = p, bytes_ = bytes;
+        return e;
+    }
+    // alloc, then copy host[0..n) on `s` and synchronise `s` (so work queued on s before is done too)
+    template <class T> cudaError_t upload(const T* host, size_t n, cudaStream_t s) {
+        cudaError_t e = alloc(n * sizeof(T));
+        if (e == cudaSuccess) e = cudaMemcpyAsync(p_, host, n * sizeof(T), cudaMemcpyHostToDevice, s);
+        return e == cudaSuccess ? cudaStreamSynchronize(s) : e;
+    }
+    // the whole buffer into *out, synchronously (cudaMemcpy)
+    template <class T> cudaError_t read(std::vector<T>* out) const {
+        out->resize(bytes_ / sizeof(T));
+        return cudaMemcpy(out->data(), p_, out->size() * sizeof(T), cudaMemcpyDeviceToHost);
+    }
+    template <class T> T* as() const { return static_cast<T*>(p_); }
+
+  private:
+    void* p_ = nullptr;
+    size_t bytes_ = 0;
+};
+
 // "file_direct_io" (SWEC_FILE_DIRECT): bit 0 = O_DIRECT reads of the .dat / shard inputs straight into the pinned
 // ring, bit 1 = O_DIRECT writes of the shard outputs — the page cache is bypassed both ways (disk-backed volumes only;
 // files that refuse O_DIRECT, tmpfs for one, and unaligned pieces silently take the buffered descriptor)
@@ -56,8 +95,8 @@ void file_pipeline_trim();  // ec_files.cc: release staging rings parked between
 
 // device-resident multiply tables of one R×K matrix (R ≤ 4)
 struct DeviceTables {
-    u32* compact = nullptr;     // [K][2][16]
-    u32* replicated = nullptr;  // [K][2][16][32]
+    DeviceBuffer compact;     // u32 [K][2][16]
+    DeviceBuffer replicated;  // u32 [K][2][16][32]
 };
 
 struct JitKernel;  // jit.cc
@@ -89,7 +128,7 @@ struct swec_encoder_impl {
     // out[r][x] = XOR_i rows[r][i] ⊗ in[i][x] on device memory, asynchronous on s.
     int apply(const Matrix& rows, const uint8_t* const* in, uint8_t* const* out, size_t n,
               const Layout& layout, cudaStream_t s);
-    int get_tables(const Matrix& rows4, DeviceTables* out, cudaStream_t s);
+    int get_tables(const Matrix& rows4, const DeviceTables** out, cudaStream_t s);
 };
 
 Matrix parity_rows(const swec_encoder_impl* e);  // the m parity rows of the generator

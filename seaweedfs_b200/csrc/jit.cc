@@ -401,18 +401,11 @@ int jit_debug_compile(const Matrix& rows, size_t* cubin_bytes, int* xtime_steps,
 
 cudaError_t jit_launch(const JitKernel& k, const SwecApplyParams& p, bool blocked, cudaStream_t s) {
     if (p.nvec == 0) return cudaSuccess;
-    int sms = 132, dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const u64 per_cta = u64(k.threads) * u64(k.unroll);
-    const u64 need = (p.nvec + per_cta - 1) / per_cta;
-    const u64 cap = u64(sms) * u64(encode_ctas_per_sm());
-    const unsigned grid = unsigned(need < cap ? need : cap);
+    const unsigned grid = grid_for(p.nvec, u64(k.threads) * u64(k.unroll), encode_ctas_per_sm());
     void* args[] = {const_cast<SwecApplyParams*>(&p)};
     note_kernel_work(double(p.nvec) * 16.0 * 14.0 / 3.0e12 * 1e3);  // ≈ k + r streams; feeds the power policy
-    g_kernel_launches++;
-    return cudaLaunchKernel(reinterpret_cast<const void*>(blocked ? k.blocked : k.flat), dim3(grid),
-                            dim3(unsigned(k.threads)), args, 0, s);
+    return launched(1, cudaLaunchKernel(reinterpret_cast<const void*>(blocked ? k.blocked : k.flat), dim3(grid),
+                                        dim3(unsigned(k.threads)), args, 0, s));
 }
 
 }  // namespace swec

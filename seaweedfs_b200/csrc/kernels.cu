@@ -21,6 +21,7 @@
 #define SWEC_XT_VARIANT 0
 #endif
 #include "device_common.cuh"
+#include "tma_fetch.cuh"
 #include "gen_rs10x4_encode.inc"
 // the same combiner once more with the low-power step (variant 2) bound to both spellings
 #undef SWEC_XT1A
@@ -58,39 +59,13 @@ __global__ void __launch_bounds__(THREADS) rs10x4_encode(const __grid_constant__
 // lane — word index ((i*2+h)*16+v)*32+lane — so lane l always hits bank l: conflict-free no matter
 // what the data bytes are.  K*4 KiB per CTA, fetched by one cp.async.bulk (TMA, SASS UBLKCP).
 
-__device__ __forceinline__ u32 smem_u32(const void* p) { return (u32)__cvta_generic_to_shared(p); }
-
 template <int KT>  // KT > 0: inputs known at compile time (loads hoisted); 0: run-time loop
 __global__ void __launch_bounds__(256) swec_table_kernel(const __grid_constant__ SwecApplyParams p,
                                                           const u32* __restrict__ tables, int k_rt, int r) {
     extern __shared__ __align__(128) u32 tab[];
     __shared__ __align__(8) u64 mbar;
     const int K = KT > 0 ? KT : k_rt;
-    const u32 bytes = (u32)K * 4096u;
-    if (threadIdx.x == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(&mbar)));
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(&mbar)), "r"(bytes)
-                     : "memory");
-        asm volatile(
-            "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                smem_u32(tab)),
-            "l"(tables), "r"(bytes), "r"(smem_u32(&mbar))
-            : "memory");
-    }
-    {
-        u32 done = 0;
-        while (!done) {
-            asm volatile(
-                "{ .reg .pred q; mbarrier.try_wait.parity.shared::cta.b64 q, [%1], 0; selp.u32 %0, 1, 0, q; }"
-                : "=r"(done)
-                : "r"(smem_u32(&mbar))
-                : "memory");
-        }
-    }
+    tma_fetch(tab, tables, (u32)K * 4096u, &mbar);
     const u32 lane4 = (threadIdx.x & 31u) * 4u;
     const char* tb = reinterpret_cast<const char*>(tab);
     const u64 stride = (u64)gridDim.x * blockDim.x;
@@ -223,25 +198,22 @@ __global__ void __launch_bounds__(256) swec_compare_kernel(const u8* __restrict_
 
 // ------------------------------------------------------------------ launchers
 
-static int g_sm_count[64];
-
-static int sm_count() {
+int sm_count() {
+    static std::atomic<int> cached[64];  // 0: not asked yet
     int dev = 0;
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64) return 132;
-    if (!g_sm_count[dev]) {
-        int n = 132;
+    int n = cached[dev].load(std::memory_order_relaxed);
+    if (!n) {
+        n = 132;
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        g_sm_count[dev] = n;
+        cached[dev].store(n, std::memory_order_relaxed);
     }
-    return g_sm_count[dev];
+    return n;
 }
 
-// grid: whole number of waves — SMs × resident CTAs — capped by the work available
-static unsigned grid_for(u64 items, int threads, int ctas_per_sm) {
-    const u64 need = (items + threads - 1) / threads;
-    const u64 cap = (u64)sm_count() * ctas_per_sm;
-    return (unsigned)(need < cap ? (need ? need : 1) : cap);
+unsigned grid_cap(u64 need, int ctas_per_sm) {
+    return unsigned(std::max<u64>(1, std::min<u64>(need, u64(sm_count()) * u64(ctas_per_sm))));
 }
 
 // ---- tuning options (defaults = measured best, DESIGN.md §6); env at start-up, swec_set_option later
@@ -342,14 +314,13 @@ static cudaError_t launch_rs10x4_shape(const SwecApplyParams& p, bool blocked, i
     else if (blocked) rs10x4_encode<THREADS, UNROLL, true, false><<<grid, THREADS, 0, s>>>(p);
     else if (lp) rs10x4_encode<THREADS, UNROLL, false, true><<<grid, THREADS, 0, s>>>(p);
     else rs10x4_encode<THREADS, UNROLL, false, false><<<grid, THREADS, 0, s>>>(p);
-    return cudaGetLastError();
+    return launched();
 }
 
 cudaError_t launch_rs10x4_encode(const SwecApplyParams& p, bool blocked, cudaStream_t s) {
     if (p.nvec == 0) return cudaSuccess;
     const long threads = g_opt_enc_threads.load(), unroll = g_opt_enc_unroll.load();
     const int c = encode_ctas_per_sm();
-    g_kernel_launches++;
     if (threads == 128 && unroll == 1) return launch_rs10x4_shape<128, 1>(p, blocked, c, s);
     if (threads == 128 && unroll == 2) return launch_rs10x4_shape<128, 2>(p, blocked, c, s);
     if (threads == 512 && unroll == 1) return launch_rs10x4_shape<512, 1>(p, blocked, c, s);
@@ -373,38 +344,33 @@ cudaError_t launch_table_apply(const SwecApplyParams& p, const u32* replicated_t
         if (e != cudaSuccess) return e;
         swec_table_kernel<0><<<grid, 256, smem, s>>>(p, replicated_tables, K, r);
     }
-    g_kernel_launches++;
-    return cudaGetLastError();
+    return launched();
 }
 
 cudaError_t launch_bytes_apply(const SwecApplyParams& p, const u32* compact_tables, int K, int r, u64 nbytes,
                                cudaStream_t s) {
     if (nbytes == 0) return cudaSuccess;
     swec_bytes_kernel<<<grid_for(nbytes, 256, 8), 256, 0, s>>>(p, compact_tables, K, r, nbytes);
-    g_kernel_launches++;
-    return cudaGetLastError();
+    return launched();
 }
 
 cudaError_t launch_synth(void* dst, u64 byte_offset, u64 nbytes, u64 seed, cudaStream_t s) {
     if (nbytes == 0) return cudaSuccess;
     swec_synth_kernel<<<grid_for(nbytes / 8, 256, 8), 256, 0, s>>>(static_cast<u64*>(dst), byte_offset / 8, nbytes / 8, seed);
-    g_kernel_launches++;
-    return cudaGetLastError();
+    return launched();
 }
 
 cudaError_t launch_digest(const void* src, u64 nbytes, u64* out_dev, cudaStream_t s) {
     cudaError_t e = cudaMemsetAsync(out_dev, 0, 8, s);
     if (e != cudaSuccess || nbytes == 0) return e;
     swec_digest_kernel<<<grid_for((nbytes + 7) / 8, 256, 8), 256, 0, s>>>(static_cast<const u8*>(src), nbytes, out_dev);
-    g_kernel_launches++;
-    return cudaGetLastError();
+    return launched();
 }
 
 cudaError_t launch_compare(const void* a, const void* b, u64 nbytes, unsigned long long* out_dev, cudaStream_t s) {
     if (nbytes == 0) return cudaSuccess;
     swec_compare_kernel<<<grid_for((nbytes + 15) / 16, 256, 8), 256, 0, s>>>(static_cast<const u8*>(a), static_cast<const u8*>(b), nbytes, out_dev);
-    g_kernel_launches++;
-    return cudaGetLastError();
+    return launched();
 }
 
 }  // namespace swec

@@ -10,6 +10,20 @@ namespace swec {
 
 extern std::atomic<unsigned long long> g_kernel_launches;
 
+// Every launch site ends with this: counts its n launches (swec_kernel_launches) and returns the launch error.
+inline cudaError_t launched(unsigned n, cudaError_t e) {
+    g_kernel_launches += n;
+    return e;
+}
+inline cudaError_t launched(unsigned n = 1) { return launched(n, cudaGetLastError()); }
+
+int sm_count();  // SMs of the current device, asked once per device; 132 when the driver cannot say
+// A persistent grid: `need` CTAs, capped at whole waves of ctas_per_sm resident CTAs per SM, and at least 1.
+unsigned grid_cap(u64 need, int ctas_per_sm);
+inline unsigned grid_for(u64 items, u64 per_cta, int ctas_per_sm) {  // one CTA per per_cta items, capped
+    return grid_cap((items + per_cta - 1) / per_cta, ctas_per_sm);
+}
+
 // tuning knobs: launch shape of the Horner kernels (swec_set_option / SWEC_ENC_THREADS, SWEC_ENC_UNROLL,
 // SWEC_CTAS_PER_SM).  ctas_per_sm = resident CTAs per SM the persistent grids are sized for.
 extern std::atomic<long> g_opt_enc_threads, g_opt_enc_unroll, g_opt_ctas_per_sm;

@@ -70,13 +70,6 @@ __global__ void __launch_bounds__(256) nd_attribute_kernel(const __grid_constant
     }
 }
 
-unsigned attribute_grid(u64 n) {
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    return unsigned(std::max<u64>(1, std::min<u64>((n + 255) / 256, u64(sms) * 8)));
-}
-
 }  // namespace
 
 int check_needle_damage_args(int needles_cap, const swec_needle_damage* needles, const uint64_t* unowned, int n_records,
@@ -87,13 +80,6 @@ int check_needle_damage_args(int needles_cap, const swec_needle_damage* needles,
     if (n_records < 0 || (n_records > 0 && !records))
         return fail(SWEC_ERR_INVALID_ARG, "n_records must be >= 0, and records non-NULL when it is > 0");
     return SWEC_OK;
-}
-
-NeedleDamage::~NeedleDamage() {
-    if (spans_) cudaFree(spans_);
-    if (counters_) cudaFree(counters_);
-    if (masks_) cudaFree(masks_);
-    if (saved_) cudaFree(saved_);
 }
 
 int NeedleDamage::init(int k, int m, const StripeMap& map, const swec_needle_damage* recs, int n, int version, int slots,
@@ -113,19 +99,17 @@ int NeedleDamage::init(int k, int m, const StripeMap& map, const swec_needle_dam
         spans[size_t(n + j)] = r.size < 0 ? r.offset : r.offset + needle_actual_size(r.size, version);
     }
     const size_t nc = size_t(2 * n + 2);
-    SWEC_CUDA(cudaMalloc(reinterpret_cast<void**>(&spans_), spans.size() * sizeof(int64_t)));
-    SWEC_CUDA(cudaMalloc(reinterpret_cast<void**>(&counters_), nc * sizeof(unsigned long long)));
-    SWEC_CUDA(cudaMalloc(reinterpret_cast<void**>(&masks_), size_t(std::max(n, 1)) * sizeof(unsigned)));
-    if (slots > 0 && piece > 0) SWEC_CUDA(cudaMalloc(reinterpret_cast<void**>(&saved_), size_t(slots) * size_t(k) * piece));
-    SWEC_CUDA(cudaMemcpyAsync(spans_, spans.data(), spans.size() * sizeof(int64_t), cudaMemcpyHostToDevice, s));
-    SWEC_CUDA(cudaMemsetAsync(counters_, 0, nc * sizeof(unsigned long long), s));
-    SWEC_CUDA(cudaMemsetAsync(masks_, 0, size_t(std::max(n, 1)) * sizeof(unsigned), s));
-    SWEC_CUDA(cudaStreamSynchronize(s));
+    SWEC_CUDA(counters_.alloc(nc * sizeof(unsigned long long)));
+    SWEC_CUDA(masks_.alloc(size_t(std::max(n, 1)) * sizeof(unsigned)));
+    if (slots > 0 && piece > 0) SWEC_CUDA(saved_.alloc(size_t(slots) * size_t(k) * piece));
+    SWEC_CUDA(cudaMemsetAsync(counters_.as<void>(), 0, nc * sizeof(unsigned long long), s));
+    SWEC_CUDA(cudaMemsetAsync(masks_.as<void>(), 0, size_t(std::max(n, 1)) * sizeof(unsigned), s));
+    SWEC_CUDA(spans_.upload(spans.data(), spans.size(), s));  // synchronises s, after the clears
     return SWEC_OK;
 }
 
 int NeedleDamage::save(uint8_t* const* shards, size_t len, int slot, cudaStream_t s) {
-    uint8_t* at = saved_ + size_t(slot) * size_t(k_) * piece_;
+    uint8_t* at = saved_.as<uint8_t>() + size_t(slot) * size_t(k_) * piece_;
     for (int i = 0; i < k_; i++)
         SWEC_CUDA(cudaMemcpyAsync(at + size_t(i) * piece_, shards[i], len, cudaMemcpyDeviceToDevice, s));
     return SWEC_OK;
@@ -137,7 +121,7 @@ int NeedleDamage::launch(const uint8_t* const* orig, uint8_t* const* fixed, uint
     AttributeParams p;
     memset(&p, 0, sizeof p);
     for (int i = 0; i < k_; i++) {
-        p.orig[i] = orig ? orig[i] : saved_ + (size_t(slot) * size_t(k_) + size_t(i)) * piece_;
+        p.orig[i] = orig ? orig[i] : saved_.as<uint8_t>() + (size_t(slot) * size_t(k_) + size_t(i)) * piece_;
         p.fixed[i] = fixed[i];
     }
     for (int q = 0; q < m_; q++) {
@@ -150,23 +134,22 @@ int NeedleDamage::launch(const uint8_t* const* orig, uint8_t* const* fixed, uint
     p.m = m_;
     p.nrec = n_;
     p.map = map_;
-    p.off = spans_;
-    p.end = spans_ + n_;
-    p.damaged = counters_;
-    p.uncorrectable = counters_ + n_;
-    p.unowned = counters_ + 2 * n_;
-    p.mask = masks_;
-    nd_attribute_kernel<<<attribute_grid(len), 256, 0, s>>>(p);
-    g_kernel_launches++;
-    SWEC_CUDA(cudaGetLastError());
+    p.off = spans_.as<int64_t>();
+    p.end = p.off + n_;
+    p.damaged = counters_.as<unsigned long long>();
+    p.uncorrectable = p.damaged + n_;
+    p.unowned = p.damaged + 2 * n_;
+    p.mask = masks_.as<unsigned>();
+    nd_attribute_kernel<<<grid_for(len, 256, 8), 256, 0, s>>>(p);
+    SWEC_CUDA(launched());
     return SWEC_OK;
 }
 
 int NeedleDamage::collect(swec_needle_damage* recs, uint64_t unowned[2]) {
-    std::vector<unsigned long long> c(size_t(2 * n_ + 2));
-    std::vector<unsigned> mask(size_t(std::max(n_, 1)));
-    SWEC_CUDA(cudaMemcpy(c.data(), counters_, c.size() * sizeof c[0], cudaMemcpyDeviceToHost));
-    SWEC_CUDA(cudaMemcpy(mask.data(), masks_, mask.size() * sizeof mask[0], cudaMemcpyDeviceToHost));
+    std::vector<unsigned long long> c;
+    std::vector<unsigned> mask;
+    SWEC_CUDA(counters_.read(&c));
+    SWEC_CUDA(masks_.read(&mask));
     for (int j = 0; j < n_; j++) {
         swec_needle_damage& r = recs[order_[size_t(j)]];
         r.damaged_bytes = c[size_t(j)];

@@ -13,6 +13,7 @@
 #include <vector>
 
 #include "../../include/swec.h"
+#include "engine.h"
 #include "stripe_map.h"
 
 namespace swec {
@@ -26,7 +27,6 @@ class NeedleDamage {
     NeedleDamage() = default;
     NeedleDamage(const NeedleDamage&) = delete;
     NeedleDamage& operator=(const NeedleDamage&) = delete;
-    ~NeedleDamage();
 
     // recs[n]: every live record (offset and size read; any order).  A record owns [offset, offset +
     // needle_actual_size(size, version)); of overlapping records, a byte belongs to the one with the greatest offset not
@@ -48,10 +48,10 @@ class NeedleDamage {
     StripeMap map_{};
     size_t piece_ = 0;
     std::vector<int> order_;                 // sorted position -> index in recs
-    int64_t* spans_ = nullptr;               // offset[n], end[n], sorted by offset
-    unsigned long long* counters_ = nullptr;  // damaged[n], uncorrectable[n], unowned[2]
-    unsigned* masks_ = nullptr;               // [n]
-    uint8_t* saved_ = nullptr;                // slots x k x piece
+    DeviceBuffer spans_;     // int64_t offset[n], end[n], sorted by offset
+    DeviceBuffer counters_;  // unsigned long long damaged[n], uncorrectable[n], unowned[2]
+    DeviceBuffer masks_;     // unsigned [n]
+    DeviceBuffer saved_;     // slots x k x piece bytes
 };
 
 // swec_ec_volume_locate_needle_damage's file work (ec_files.cc) on the k+m local shard files `in`, all `size` bytes:

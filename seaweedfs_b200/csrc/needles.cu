@@ -15,6 +15,7 @@
 #include "engine.h"
 #include "needle_format.h"
 #include "needles.h"
+#include "tma_fetch.cuh"
 
 namespace swec {
 
@@ -133,8 +134,6 @@ __global__ void __launch_bounds__(1024) needle_scan_kernel(u64* __restrict__ a, 
     }
 }
 
-__device__ __forceinline__ u32 smem_u32(const void* p) { return (u32)__cvta_generic_to_shared(p); }
-
 // table k, index i of this lane's copy (tl = the table base + lane*4)
 __device__ __forceinline__ u32 tab(const char* tl, u32 k, u32 i) {
     return *reinterpret_cast<const u32*>(tl + (((k << 8) | i) << 7));
@@ -177,30 +176,7 @@ __global__ void __launch_bounds__(kCrcThreads, 1)
                       const u64* __restrict__ first_chunk, const u32* __restrict__ tables, const u32* __restrict__ powers) {
     extern __shared__ __align__(128) u32 smem_tab[];
     __shared__ __align__(8) u64 mbar;
-    if (threadIdx.x == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(&mbar)));
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(&mbar)), "r"(kTableBytes)
-                     : "memory");
-        asm volatile(
-            "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                smem_u32(smem_tab)),
-            "l"(tables), "r"(kTableBytes), "r"(smem_u32(&mbar))
-            : "memory");
-    }
-    {
-        u32 done = 0;
-        while (!done) {
-            asm volatile(
-                "{ .reg .pred q; mbarrier.try_wait.parity.shared::cta.b64 q, [%1], 0; selp.u32 %0, 1, 0, q; }"
-                : "=r"(done)
-                : "r"(smem_u32(&mbar))
-                : "memory");
-        }
-    }
+    tma_fetch(smem_tab, tables, kTableBytes, &mbar);
     const char* tl = reinterpret_cast<const char*>(smem_tab) + (threadIdx.x & 31u) * 4u;
     const int data_at = version == 1 ? kNeedleHeaderSize : kNeedleHeaderSize + kDataSizeSize;
     const u64 total = first_chunk[n];
@@ -259,8 +235,7 @@ cudaError_t tables_for_current_device(Tables* out, cudaStream_t s) {
         if (e != cudaSuccess) return e;
         pw = rep + kTableBytes / sizeof(u32);
         needle_tables_kernel<<<1, 256, 0, s>>>(rep, pw);
-        g_kernel_launches++;
-        e = cudaGetLastError();
+        e = launched();
         if (e == cudaSuccess) e = cudaFuncSetAttribute(needle_crc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(kTableBytes));
         if (e == cudaSuccess) e = cudaStreamSynchronize(s);
         if (e != cudaSuccess) {
@@ -284,18 +259,14 @@ cudaError_t launch_needle_check(const void* dat, int64_t dat_size, int version, 
     Tables t;
     cudaError_t e = tables_for_current_device(&t, s);
     if (e != cudaSuccess) return e;
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const u8* d = static_cast<const u8*>(dat);
     u64* first_chunk = static_cast<u64*>(scratch);
     const unsigned per_record = unsigned((n + 255) / 256);
     needle_parse_kernel<<<per_record, 256, 0, s>>>(d, dat_size, version, checks, n, first_chunk);
     needle_scan_kernel<<<1, 1024, 0, s>>>(first_chunk, n);
-    needle_crc_kernel<<<sms, kCrcThreads, kTableBytes, s>>>(d, version, checks, n, first_chunk, t.replicated, t.powers);
+    needle_crc_kernel<<<sm_count(), kCrcThreads, kTableBytes, s>>>(d, version, checks, n, first_chunk, t.replicated, t.powers);
     needle_final_kernel<<<per_record, 256, 0, s>>>(checks, n, t.powers);
-    g_kernel_launches += 4;
-    return cudaGetLastError();
+    return launched(4);
 }
 
 }  // namespace swec
