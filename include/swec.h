@@ -74,6 +74,7 @@ typedef enum swec_status {
 
 typedef struct swec_encoder swec_encoder;
 typedef struct swec_ec_volume swec_ec_volume; /* a mounted EC volume (swec_ec_volume_open, below) */
+typedef struct swec_needle_check swec_needle_check; /* one record's Needle.ReadBytes check (below) */
 
 /* ---- library ------------------------------------------------------------------------------ */
 const char *swec_version(void);
@@ -332,6 +333,33 @@ int swec_ec_volume_locate_needle_damage(swec_ec_volume *vol, int radius, swec_da
                                         swec_damage_range *ranges, int ranges_cap, int *n_ranges,
                                         swec_needle_damage *needles, int needles_cap, int *n_needles,
                                         uint64_t unowned[2], int *ok);
+/* Repair through the mounted volume: swec_ec_volume_locate_needle_damage and swec_repair_ec_damage in one pass 1, then
+ * every needle the repair touched checked again on the GPU.
+ *   - Arguments and errors are those of swec_ec_volume_locate_needle_damage, in its order and before any device work or
+ *     any open for writing, with one more needle rule: checks may be NULL only when needles_cap is 0.
+ *   - report, ranges, needles, *n_needles and unowned are byte for byte what swec_ec_volume_locate_needle_damage returns
+ *     for the same set before the call; the report is also the one swec_repair_ec_damage returns, so shard_bytes[i] =
+ *     the bytes corrected in shard i.
+ *   - The writes are those of swec_repair_ec_damage's pass 2: only the blamed shards are opened for writing, each gets
+ *     back only its own flagged pages (O_DIRECT when "file_direct_io" bit 1 is set), every modified file is
+ *     fdatasync'ed before the call returns, and uncorrectable columns are left byte for byte as they were.  The bytes go
+ *     to the inodes the handle reads, each blamed shard's read-only descriptor opened again for writing through
+ *     /proc/self/fd; when that is refused the call fails with SWEC_ERR_IO before anything is written.  Each byte is
+ *     written once, so running the call again finishes a repair cut short.
+ *   - After the writes are durable, every needle with a non-zero count (all of them, not only the first needles_cap) is
+ *     read from the repaired files and checked like swec_ec_volume_scrub_needles checks a record (size, layout,
+ *     CRC32-C) on the GPU of the handle's device.  checks[i] = the check of needles[i], with needle_id, offset and
+ *     size filled in; a record that runs past the end of its shard is SWEC_NEEDLE_OUTSIDE_IMAGE.
+ *   - *ok = 1 iff no uncorrectable column remains and every re-checked needle is SWEC_NEEDLE_OK.  The needle CRC is the
+ *     one check independent of the code, so a column MISCORRECTED beyond the guarantee (more than m-t wrong shards,
+ *     reported as corrected) that holds live data shows here as a needle that is not SWEC_NEEDLE_OK, and *ok = 0.
+ *   - A clean set stops after pass 1: nothing is opened for writing, nothing is re-checked, *n_needles = 0, *ok = 1.
+ * Calls on one handle serialise, so the handle's reads see the files before or after the call, and after it return the
+ * corrected bytes.                                                                                                   */
+int swec_ec_volume_repair_needle_damage(swec_ec_volume *vol, int radius, swec_damage_report *report,
+                                        swec_damage_range *ranges, int ranges_cap, int *n_ranges,
+                                        swec_needle_damage *needles, swec_needle_check *checks, int needles_cap,
+                                        int *n_needles, uint64_t unowned[2], int *ok);
 /* Device level: shards[k+m] in HBM (only read), the image of a .dat of dat_size bytes striped as
  * swec_encode_volume_device does with large_block / small_block.  records[n_records] holds needle_id, offset and size
  * of every live record, sized as needle version 3; its out fields are filled for every entry, zero counts included
@@ -517,7 +545,7 @@ typedef enum swec_needle_status {
     SWEC_NEEDLE_BAD_CRC = 3,        /* CRC32-C of Data != the stored checksum                             */
     SWEC_NEEDLE_OUTSIDE_IMAGE = 4   /* the record does not fit inside the image: not read at all          */
 } swec_needle_status;
-typedef struct swec_needle_check {
+struct swec_needle_check {
     uint64_t needle_id;   /* in  (reported back only)                                                       */
     int64_t offset;       /* in  byte offset of the record in the image                                     */
     int32_t size;         /* in  Size of the index entry                                                    */
@@ -529,7 +557,7 @@ typedef struct swec_needle_check {
     int32_t legacy_crc;   /* out 1 when crc_want is the pre-3.09 CRC.Value() form of crc_got (crc.go:25-27):  */
                           /*     ReadBytes still reports the record, but it is old, not corrupt             */
     int32_t reserved;
-} swec_needle_check;
+};
 /* Check n records of a volume image (.dat bytes, superblock included) resident in HBM, each the way
  * Needle.ReadBytes(record, 0, size, version) does, stopping at a record's first failure.  `dat` is a device pointer;
  * checks[] is host memory.  A record that does not end inside dat_size is SWEC_NEEDLE_OUTSIDE_IMAGE and is never

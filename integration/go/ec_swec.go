@@ -496,6 +496,43 @@ func (v *swecEcVolume) LocateNeedleDamage(radius int, maxNeedles int) (needles [
 	return needles, total, unowned, nil
 }
 
+// swecNeedleRepair is a needle RepairNeedleDamage touched, and how it reads back from the repaired files: Status 0 means
+// Needle.ReadBytes accepts it (size, layout and CRC32-C); any other status (1 size mismatch, 2 out of range, 3 bad CRC,
+// 4 past the end of its shard) means the needle has to come from a replica or a backup.
+type swecNeedleRepair struct {
+	swecNeedleDamage
+	Status  int32
+	CrcGot  uint32
+	CrcWant uint32
+}
+
+// RepairNeedleDamage is LocateNeedleDamage and swecRepairEcDamage in one pass over the shard files the volume reads,
+// under the volume's lock, then a CRC check of every needle the repair touched.  ok is false when an uncorrectable
+// column remains or a touched needle does not read back: that is how a column miscorrected beyond the guarantee of the
+// code (more than m-t wrong shards) shows.  needles, total and unowned are what LocateNeedleDamage reported before.
+func (v *swecEcVolume) RepairNeedleDamage(radius int, maxNeedles int) (needles []swecNeedleRepair, total int, unowned [2]uint64, ok bool, err error) {
+	var report C.swec_damage_report
+	var nRanges, nNeedles, cOk C.int
+	var cUnowned [2]C.uint64_t
+	buf := make([]C.swec_needle_damage, maxNeedles+1)
+	checks := make([]C.swec_needle_check, maxNeedles+1)
+	if err := swecCall(func() C.int {
+		return C.swec_ec_volume_repair_needle_damage(v.h, C.int(radius), &report, nil, 0, &nRanges, &buf[0], &checks[0],
+			C.int(maxNeedles), &nNeedles, &cUnowned[0], &cOk)
+	}); err != nil {
+		return nil, 0, unowned, false, fmt.Errorf("repair needle damage: %w", err)
+	}
+	total = int(nNeedles)
+	for i := 0; i < total && i < maxNeedles; i++ {
+		d, c := buf[i], checks[i]
+		needles = append(needles, swecNeedleRepair{swecNeedleDamage{uint64(d.needle_id), int64(d.offset), int32(d.size),
+			uint32(d.shard_mask), uint64(d.damaged_bytes), uint64(d.uncorrectable_bytes)}, int32(c.status),
+			uint32(c.crc_got), uint32(c.crc_want)})
+	}
+	unowned = [2]uint64{uint64(cUnowned[0]), uint64(cUnowned[1])}
+	return needles, total, unowned, cOk == 1, nil
+}
+
 // swecLocateEcDamage is the parity side of a scrub of a volume whose shards are all local, run before ec.rebuild: it
 // names the shard FILES that are wrong, where verify_ec_shards (seaweed-volume/src/storage/erasure_coding/
 // ec_encoder.rs:240-258) can only name the parity shards that disagree.  broken is ready to become EcShardInfos (delete

@@ -121,6 +121,10 @@ PROTOTYPES = {
     "swec_ec_volume_locate_needle_damage": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(DamageReport), C.POINTER(DamageRange),
                                                       C.c_int, C.POINTER(C.c_int), C.POINTER(NeedleDamage), C.c_int,
                                                       C.POINTER(C.c_int), C.POINTER(C.c_uint64), C.POINTER(C.c_int)]),
+    "swec_ec_volume_repair_needle_damage": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(DamageReport), C.POINTER(DamageRange),
+                                                      C.c_int, C.POINTER(C.c_int), C.POINTER(NeedleDamage),
+                                                      C.POINTER(NeedleCheck), C.c_int, C.POINTER(C.c_int),
+                                                      C.POINTER(C.c_uint64), C.POINTER(C.c_int)]),
     "swec_locate_needle_damage_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int64, C.c_int64, C.c_int64,
                                                    C.c_int, C.POINTER(NeedleDamage), C.c_int, C.POINTER(DamageReport),
                                                    C.POINTER(DamageRange), C.c_int, C.POINTER(C.c_int),

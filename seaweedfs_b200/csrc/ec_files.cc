@@ -577,6 +577,48 @@ int submit_flagged(FilePipeline& pipe, const std::vector<swec_damage_range>& run
     return pipe.finish();
 }
 
+// The writes of the repairs' pass 2: each blamed shard gets back only its own pages of pass 1's `runs`, through out[i]
+// (out_d[i]: its O_DIRECT twin, -1 = none), which the caller opens for the blamed shards alone.
+class PageWrites {
+  public:
+    std::vector<int> out, out_d;
+
+    PageWrites(const std::vector<swec_damage_range>& runs, int total)
+        : out(size_t(total), -1), out_d(size_t(total), -1), runs_(runs), next_(size_t(total), 0), stop_(size_t(total), 0) {
+        // each shard's slice of `runs`, which lists them shard by shard in ascending offset; an empty one: not blamed
+        for (size_t r = runs.size(); r-- > 0;)
+            if (runs[r].shard_id >= 0) {
+                const size_t id = size_t(runs[r].shard_id);
+                if (!stop_[id]) stop_[id] = r + 1;
+                next_[id] = r;
+            }
+    }
+    bool blamed(int i) const { return stop_[size_t(i)] > 0; }
+
+    // the writes of the next item, which submit_flagged hands over in ascending shard offset
+    void add(Item& it) {
+        const int64_t o = it.shard_off, end = o + int64_t(it.len);
+        for (size_t i = 0; i < out.size(); i++)
+            for (size_t& r = next_[i]; r < stop_[i]; r++) {  // shard i's own pages in the item
+                const int64_t lo = std::max(runs_[r].offset, o), hi = std::min(runs_[r].offset + runs_[r].length, end);
+                if (lo >= end) break;
+                it.writes.push_back({int(i), out[i], lo, size_t(lo - o), size_t(hi - lo), out_d[i]});
+                if (hi < runs_[r].offset + runs_[r].length) break;  // the run goes on in the next item
+            }
+    }
+
+    // every modified file made durable; `base` + the shard's extension names a failing one
+    int sync(const std::string& base) const {
+        for (size_t i = 0; i < out.size(); i++)
+            if (out[i] >= 0 && fdatasync(out[i]) != 0) return io_fail("fdatasync " + base + shard_ext(int(i)));
+        return SWEC_OK;
+    }
+
+  private:
+    const std::vector<swec_damage_range>& runs_;
+    std::vector<size_t> next_, stop_;
+};
+
 // Pass 2 of swec_repair_ec_damage.  `runs` are every page run pass 1 found, of the blamed shards and of the
 // uncorrectable columns.  Only the columns of those pages go through the pipeline again, with a correcting locator, and
 // the report and ranges are collected from that.  Each blamed shard gets back only its own pages, in the file where it
@@ -585,24 +627,16 @@ int repair_pages(swec_encoder* enc, const Matrix& rows, const std::string& b, co
                  const std::vector<int>& in, int64_t size, int radius, const std::vector<swec_damage_range>& runs,
                  swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges) {
     const int total = int(in.size());
-    // each shard's slice of `runs`, which lists them shard by shard in ascending offset; an empty one: not blamed
-    std::vector<size_t> next(static_cast<size_t>(total), 0), stop(static_cast<size_t>(total), 0);
-    for (size_t r = runs.size(); r-- > 0;)
-        if (runs[r].shard_id >= 0) {
-            const size_t id = size_t(runs[r].shard_id);
-            if (!stop[id]) stop[id] = r + 1;
-            next[id] = r;
-        }
+    PageWrites writes(runs, total);
     FdSet fds;
     const long direct = g_opt_file_direct_io.load();
-    std::vector<int> in_d(static_cast<size_t>(total), -1), out(static_cast<size_t>(total), -1),
-        out_d(static_cast<size_t>(total), -1);
+    std::vector<int> in_d(static_cast<size_t>(total), -1);
     for (int i = 0; i < total; i++) {
         const std::string path = find_shard_file(b, dirs, ndirs, i);
         in_d[size_t(i)] = fds.keep(open_direct(path, O_RDONLY, direct & 1));
-        if (!stop[size_t(i)]) continue;
-        if ((out[size_t(i)] = fds.keep(open(path.c_str(), O_RDWR))) < 0) return io_fail("open " + path);
-        out_d[size_t(i)] = fds.keep(open_direct(path, O_RDWR, direct & 2));
+        if (!writes.blamed(i)) continue;
+        if ((writes.out[size_t(i)] = fds.keep(open(path.c_str(), O_RDWR))) < 0) return io_fail("open " + path);
+        writes.out_d[size_t(i)] = fds.keep(open_direct(path, O_RDWR, direct & 2));
     }
     const size_t chunk = file_chunk(size);
     DamageLocator locator;
@@ -610,19 +644,8 @@ int repair_pages(swec_encoder* enc, const Matrix& rows, const std::string& b, co
     int rc = pipe.start();
     if (rc) return rc;
     if ((rc = locator.init(rows, size, radius, enc->stream, /*correct=*/true))) return rc;
-    const auto writes = [&](Item& it) {
-        const int64_t o = it.shard_off, end = o + int64_t(it.len);
-        for (int i = 0; i < total; i++)
-            for (size_t& r = next[size_t(i)]; r < stop[size_t(i)]; r++) {  // shard i's own pages in the item
-                const int64_t lo = std::max(runs[r].offset, o), hi = std::min(runs[r].offset + runs[r].length, end);
-                if (lo >= end) break;
-                it.writes.push_back({i, out[size_t(i)], lo, size_t(lo - o), size_t(hi - lo), out_d[size_t(i)]});
-                if (hi < runs[r].offset + runs[r].length) break;  // the run goes on in the next item
-            }
-    };
-    if ((rc = submit_flagged(pipe, runs, chunk, in, in_d, writes))) return rc;
-    for (int i = 0; i < total; i++)
-        if (out[size_t(i)] >= 0 && fdatasync(out[size_t(i)]) != 0) return io_fail("fdatasync " + b + shard_ext(i));
+    if ((rc = submit_flagged(pipe, runs, chunk, in, in_d, [&](Item& it) { writes.add(it); }))) return rc;
+    if ((rc = writes.sync(b))) return rc;
     return locator.collect(report, ranges, ranges_cap, n_ranges);
 }
 
@@ -899,15 +922,28 @@ int decode_dat(swec_encoder* enc, const std::vector<int>& in, const std::vector<
 namespace swec {
 
 // Pass 2 per item: the slot's data shards saved, the correcting locate, the corrected data re-encoded into the computed
-// rows (the locate is done with them), then the attribution.  Nothing comes back to the host and nothing is written.
+// rows (the locate is done with them), then the attribution.  Without `repair` nothing comes back to the host and
+// nothing is written.  With it, the writes of swec_repair_ec_damage's pass 2 go to the inodes behind `in`: each blamed
+// shard's descriptor is opened again for writing through /proc/self/fd before anything is read again, and the call
+// fails there, with nothing written, when that is refused.
 int needle_damage_files(swec_encoder* enc, const std::vector<int>& in, int64_t size, int radius, const StripeMap& map,
-                        int version, std::vector<swec_needle_damage>* recs, swec_damage_report* report,
+                        int version, bool repair, std::vector<swec_needle_damage>* recs, swec_damage_report* report,
                         swec_damage_range* ranges, int ranges_cap, int* n_ranges, uint64_t unowned[2]) {
     const Matrix rows = parity_rows(enc);
     std::vector<swec_damage_range> runs;
     int rc = locate_pass(enc, rows, in, size, radius, report, ranges, ranges_cap, n_ranges, &runs);
     if (rc || report->damaged_columns == 0) return rc;
     const int k = enc->k;
+    PageWrites writes(runs, int(in.size()));
+    FdSet fds;
+    const long direct = g_opt_file_direct_io.load();
+    for (int i = 0; repair && i < int(in.size()); i++) {
+        if (!writes.blamed(i)) continue;
+        const std::string self = "/proc/self/fd/" + std::to_string(in[size_t(i)]);
+        if ((writes.out[size_t(i)] = fds.keep(open(self.c_str(), O_RDWR))) < 0)
+            return io_fail("open shard " + shard_ext(i) + " for writing through " + self);
+        writes.out_d[size_t(i)] = fds.keep(open_direct(self, O_RDWR, direct & 2));
+    }
     const size_t chunk = file_chunk(size);
     DamageLocator locator;
     NeedleDamage nd;
@@ -928,7 +964,9 @@ int needle_damage_files(swec_encoder* enc, const std::vector<int>& in, int64_t s
     if ((rc = locator.init(rows, size, radius, enc->stream, /*correct=*/true))) return rc;
     if ((rc = nd.init(k, enc->m, map, recs->data(), int(recs->size()), version, int(pipe.slot_count()), chunk, enc->stream)))
         return rc;
-    if ((rc = submit_flagged(pipe, runs, chunk, in, std::vector<int>(in.size(), -1), nullptr))) return rc;
+    const std::function<void(Item&)> add = [&](Item& it) { writes.add(it); };
+    if ((rc = submit_flagged(pipe, runs, chunk, in, std::vector<int>(in.size(), -1), repair ? add : nullptr))) return rc;
+    if ((rc = writes.sync(""))) return rc;
     return nd.collect(recs->data(), unowned);
 }
 

@@ -486,6 +486,7 @@ class NeedleScrub {
     }
 
     std::vector<std::pair<size_t, std::string>> failed;  // (finding, text) of every record that failed its check
+    std::vector<swec_needle_check>* results = nullptr;   // when set: (*results)[finding] = every record's check
 
   private:
     static constexpr size_t kSlotData = size_t(16) << 20;  // record bytes per slot
@@ -536,6 +537,7 @@ class NeedleScrub {
     }
 
     void note(const swec_needle_check& c, size_t finding) {
+        if (results) (*results)[finding] = c;
         std::string err;
         char buf[160];
         switch (c.status) {
@@ -670,6 +672,103 @@ int scrub_walk(swec_ec_volume* v, NeedleScrub* needles, int64_t* entries, uint32
     return SWEC_OK;
 }
 
+// The repair's re-check: every record of `named` (all its shards local) read from the shard files and checked the way
+// scrub_needles checks a record.  (*out)[j] is the check of named[j], with its needle_id, offset and size; a record
+// that runs past the end of its shard is SWEC_NEEDLE_OUTSIDE_IMAGE and is not checked.
+int recheck_needles(swec_ec_volume* v, const std::vector<swec_needle_damage>& named, std::vector<swec_needle_check>* out) {
+    out->assign(named.size(), swec_needle_check{});
+    NeedleScrub scrub(v->device, v->version, 0);
+    scrub.results = out;
+    std::vector<Chunk> chunks;
+    int rc;
+    for (size_t j = 0; j < named.size(); j++) {
+        const swec_needle_damage& r = named[j];
+        const int64_t want = needle_actual_size(r.size, v->version);
+        uint8_t* record = nullptr;
+        if ((rc = locate_chunks(v->shard_dat_size, v->k, r.offset, want, &chunks)) || (rc = scrub.reserve(size_t(want), &record)))
+            return rc;
+        int64_t pos = 0;
+        bool whole = true;
+        for (const auto& [sid, soff, bytes] : chunks) {
+            whole = whole && pread(v->shard_fd[size_t(sid)], record + pos, size_t(bytes), off_t(soff)) == ssize_t(bytes);
+            pos += bytes;
+        }
+        if (!whole) (*out)[j].status = SWEC_NEEDLE_OUTSIDE_IMAGE;
+        else if ((rc = scrub.commit(r.needle_id, r.size, size_t(want), j))) return rc;
+    }
+    if ((rc = scrub.finish())) return rc;
+    for (size_t j = 0; j < named.size(); j++) {
+        (*out)[j].needle_id = named[j].needle_id;
+        (*out)[j].offset = named[j].offset;
+        (*out)[j].size = named[j].size;
+    }
+    return SWEC_OK;
+}
+
+// Both needle damage calls on the handle (include/swec.h): every check before any device work, the live records as the
+// reads see them, then pass 1 and, with damage, pass 2 (needle_damage_files).  With `checks` (the repair), pass 2 also
+// writes the corrections, and every named needle is re-checked from the repaired files.
+int handle_needle_damage(swec_ec_volume* v, int radius, swec_damage_report* report, swec_damage_range* ranges,
+                         int ranges_cap, int* n_ranges, swec_needle_damage* needles, bool repair, swec_needle_check* checks,
+                         int needles_cap, int* n_needles, uint64_t unowned[2], int* ok) {
+    int rc = check_needle_damage_args(needles_cap, needles, unowned, 0, nullptr);
+    if (rc) return rc;
+    if (repair && needles_cap > 0 && !checks)
+        return fail(SWEC_ERR_INVALID_ARG, "checks must be non-NULL when needles_cap is > 0");
+    if (!v || !n_needles || !ok) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
+    std::lock_guard<std::mutex> lock(v->mu);
+    if ((rc = check_locate_args(v->m, radius, report, ranges, ranges_cap))) return rc;
+    *ok = 0;
+    *n_needles = 0;
+    unowned[0] = unowned[1] = 0;
+    const int total = v->k + v->m;
+    for (int i = 0; i < total; i++)
+        if (v->shard_fd[size_t(i)] < 0)
+            return fail(SWEC_ERR_TOO_FEW_SHARDS, std::string(repair ? "repairing" : "locating") +
+                                                     " needle damage needs all shards; missing " + shard_ext(i));
+    int64_t size = -1;
+    for (int i = 0; i < total; i++)
+        if ((rc = check_length(v->shard_fd[size_t(i)], &size))) return rc;
+    if (v->device < 0) return fail(SWEC_ERR_NO_DEVICE, "no CUDA device: the volume was opened with device < 0");
+    // live records: .ecx entries that are not deleted, minus the journalled ids (FindNeedleFromEcx, ec_volume.go:419-429)
+    v->refresh_journal();
+    std::vector<swec_needle_damage> recs;
+    for (int64_t e = 0; e < v->entries(); e++) {
+        const IndexEntry x = v->entry(e);
+        if (size_deleted(x.size) || v->journalled(x.key)) continue;
+        swec_needle_damage r{};
+        r.needle_id = x.key;
+        r.offset = x.offset;
+        r.size = x.size;
+        recs.push_back(r);
+    }
+    if (!v->enc && (rc = swec_encoder_new(v->k, v->m, v->device, &v->enc))) return rc;
+    const StripeMap map = StripeMap::locate(v->shard_dat_size, v->k, kLargeBlockSize, kSmallBlockSize);
+    if ((rc = needle_damage_files(v->enc, v->shard_fd, size, radius, map, v->version, repair, &recs, report, ranges,
+                                  ranges_cap, n_ranges, unowned)))
+        return rc;
+    std::stable_sort(recs.begin(), recs.end(),
+                     [](const swec_needle_damage& a, const swec_needle_damage& b) { return a.needle_id < b.needle_id; });
+    recs.erase(std::remove_if(recs.begin(), recs.end(),
+                              [](const swec_needle_damage& r) { return !r.damaged_bytes && !r.uncorrectable_bytes; }),
+               recs.end());
+    for (int j = 0; j < needles_cap && j < int(recs.size()); j++) needles[j] = recs[size_t(j)];
+    *n_needles = int(recs.size());
+    if (!repair) {
+        *ok = report->damaged_columns == 0 ? 1 : 0;
+        return SWEC_OK;
+    }
+    std::vector<swec_needle_check> rechecked;
+    if ((rc = recheck_needles(v, recs, &rechecked))) return rc;
+    bool all_ok = report->uncorrectable_columns == 0;
+    for (size_t j = 0; j < rechecked.size(); j++) {
+        all_ok = all_ok && rechecked[j].status == SWEC_NEEDLE_OK;
+        if (int(j) < needles_cap) checks[j] = rechecked[j];
+    }
+    *ok = all_ok ? 1 : 0;
+    return SWEC_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -704,55 +803,19 @@ int swec_ec_volume_info(swec_ec_volume* v, int* data_shards, int* parity_shards,
     return SWEC_OK;
 }
 
-// Which needles the located damage hits, on the handle's own descriptors (include/swec.h): every check before any
-// device work, the live records as the reads see them, then pass 1 and, with damage, pass 2 (needle_damage_files).
 int swec_ec_volume_locate_needle_damage(swec_ec_volume* v, int radius, swec_damage_report* report, swec_damage_range* ranges,
                                         int ranges_cap, int* n_ranges, swec_needle_damage* needles, int needles_cap,
                                         int* n_needles, uint64_t unowned[2], int* ok) {
-    int rc = check_needle_damage_args(needles_cap, needles, unowned, 0, nullptr);
-    if (rc) return rc;
-    if (!v || !n_needles || !ok) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
-    std::lock_guard<std::mutex> lock(v->mu);
-    if ((rc = check_locate_args(v->m, radius, report, ranges, ranges_cap))) return rc;
-    *ok = 0;
-    *n_needles = 0;
-    unowned[0] = unowned[1] = 0;
-    const int total = v->k + v->m;
-    for (int i = 0; i < total; i++)
-        if (v->shard_fd[size_t(i)] < 0)
-            return fail(SWEC_ERR_TOO_FEW_SHARDS, "locating needle damage needs all shards; missing " + shard_ext(i));
-    int64_t size = -1;
-    for (int i = 0; i < total; i++)
-        if ((rc = check_length(v->shard_fd[size_t(i)], &size))) return rc;
-    if (v->device < 0) return fail(SWEC_ERR_NO_DEVICE, "no CUDA device: the volume was opened with device < 0");
-    // live records: .ecx entries that are not deleted, minus the journalled ids (FindNeedleFromEcx, ec_volume.go:419-429)
-    v->refresh_journal();
-    std::vector<swec_needle_damage> recs;
-    for (int64_t e = 0; e < v->entries(); e++) {
-        const IndexEntry x = v->entry(e);
-        if (size_deleted(x.size) || v->journalled(x.key)) continue;
-        swec_needle_damage r{};
-        r.needle_id = x.key;
-        r.offset = x.offset;
-        r.size = x.size;
-        recs.push_back(r);
-    }
-    if (!v->enc && (rc = swec_encoder_new(v->k, v->m, v->device, &v->enc))) return rc;
-    const StripeMap map = StripeMap::locate(v->shard_dat_size, v->k, kLargeBlockSize, kSmallBlockSize);
-    if ((rc = needle_damage_files(v->enc, v->shard_fd, size, radius, map, v->version, &recs, report, ranges, ranges_cap,
-                                  n_ranges, unowned)))
-        return rc;
-    std::stable_sort(recs.begin(), recs.end(),
-                     [](const swec_needle_damage& a, const swec_needle_damage& b) { return a.needle_id < b.needle_id; });
-    int hit = 0;
-    for (const swec_needle_damage& r : recs) {
-        if (!r.damaged_bytes && !r.uncorrectable_bytes) continue;
-        if (hit < needles_cap) needles[hit] = r;
-        hit++;
-    }
-    *n_needles = hit;
-    *ok = report->damaged_columns == 0 ? 1 : 0;
-    return SWEC_OK;
+    return handle_needle_damage(v, radius, report, ranges, ranges_cap, n_ranges, needles, false, nullptr, needles_cap,
+                                n_needles, unowned, ok);
+}
+
+int swec_ec_volume_repair_needle_damage(swec_ec_volume* v, int radius, swec_damage_report* report, swec_damage_range* ranges,
+                                        int ranges_cap, int* n_ranges, swec_needle_damage* needles,
+                                        swec_needle_check* checks, int needles_cap, int* n_needles, uint64_t unowned[2],
+                                        int* ok) {
+    return handle_needle_damage(v, radius, report, ranges, ranges_cap, n_ranges, needles, true, checks, needles_cap,
+                                n_needles, unowned, ok);
 }
 
 // FileAndDeleteCount (ec_volume.go:330-349): entries of the sealed .ecx, and distinct journalled ids.

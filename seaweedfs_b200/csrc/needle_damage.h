@@ -54,12 +54,12 @@ class NeedleDamage {
     DeviceBuffer saved_;     // slots x k x piece bytes
 };
 
-// swec_ec_volume_locate_needle_damage's file work (ec_files.cc) on the k+m local shard files `in`, all `size` bytes:
+// The file work of the handle's needle damage calls (ec_files.cc) on the k+m local shard files `in`, all `size` bytes:
 // pass 1 is the locate pass of swec_locate_ec_damage; when it finds damage, pass 2 reads the flagged pages again, as
 // the repair does, through a NeedleDamage over `recs` mapped by `map`.  recs' counts and unowned are left zero on a
-// clean set.
+// clean set.  `repair`: pass 2 also writes what swec_repair_ec_damage's pass 2 writes, to the files behind `in`.
 int needle_damage_files(swec_encoder* enc, const std::vector<int>& in, int64_t size, int radius, const StripeMap& map,
-                        int version, std::vector<swec_needle_damage>* recs, swec_damage_report* report,
+                        int version, bool repair, std::vector<swec_needle_damage>* recs, swec_damage_report* report,
                         swec_damage_range* ranges, int ranges_cap, int* n_ranges, uint64_t unowned[2]);
 
 }  // namespace swec

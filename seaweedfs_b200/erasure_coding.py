@@ -590,6 +590,30 @@ class EcVolume:
 
     LocateNeedleDamage = locate_needle_damage
 
+    def repair_needle_damage(self, radius: int = 1, max_ranges: int = 4096, max_needles: int = 1 << 16) -> dict:
+        """locate_needle_damage and repair_ec_damage in one pass over the volume's shards, written to the files the
+        handle reads, then every named needle checked again from the repaired files like scrub_needles checks it
+        (swec_ec_volume_repair_needle_damage).  Returns the locate_needle_damage dict, as it was before the call; each
+        needle also carries its check: status (0 ok, 1 size mismatch, 2 out of range, 3 bad crc, 4 outside image),
+        range_index, data_size, crc_got, crc_want and legacy_crc.  "ok" is True iff no uncorrectable column remains and
+        every named needle (not only the first max_needles) checks ok: a column miscorrected beyond the guarantee of
+        the code shows as a needle that does not."""
+        from ._native import NeedleCheck
+        report, ranges, n, ok = DamageReport(), (DamageRange * max(1, max_ranges))(), C.c_int(0), C.c_int(0)
+        needles, n_needles, unowned = (NeedleDamage * max(1, max_needles))(), C.c_int(0), (C.c_uint64 * 2)()
+        checks = (NeedleCheck * max(1, max_needles))()
+        check(lib().swec_ec_volume_repair_needle_damage(self._h, radius, C.byref(report), ranges, max_ranges, C.byref(n),
+                                                        needles, checks, max_needles, C.byref(n_needles), unowned,
+                                                        C.byref(ok)))
+        shown = min(n_needles.value, max_needles)
+        named = [{**d, "status": int(c.status), "range_index": int(c.range_index), "data_size": int(c.data_size),
+                  "crc_got": int(c.crc_got), "crc_want": int(c.crc_want), "legacy_crc": int(c.legacy_crc)}
+                 for d, c in zip(_needle_damage(needles[:shown]), checks[:shown])]
+        return {"ok": bool(ok.value), **_damage_result(report, ranges, n.value, max_ranges), "needles": named,
+                "n_needles": n_needles.value, "unowned": [int(unowned[0]), int(unowned[1])]}
+
+    RepairNeedleDamage = repair_needle_damage
+
     def close(self) -> None:
         h, self._h = getattr(self, "_h", None), None
         if h and callable(lib):
