@@ -661,6 +661,8 @@ int swec_encode_volume_device(swec_encoder* e, const void* dat_v, int64_t dat_si
         return fail(SWEC_ERR_INVALID_ARG, "bad argument");
     const uint8_t* dat = static_cast<const uint8_t*>(dat_v);
     const int k = e->k, m = e->m;
+    for (int p = 0; p < m; p++)
+        if (!parity[p]) return fail(SWEC_ERR_INVALID_ARG, "NULL parity shard");
     std::lock_guard<std::mutex> lock(e->mu);
     int rc = e->ensure_device();
     if (rc) return rc;
@@ -676,7 +678,9 @@ int swec_encode_volume_device(swec_encoder* e, const void* dat_v, int64_t dat_si
     auto region = [&](const uint8_t* base, int64_t block, int64_t nrows, int64_t poff) -> int {
         const uint8_t* ins[SWEC_MAX_SHARDS];
         uint8_t* outs[SWEC_MAX_SHARDS];
-        const bool vec_ok = horner && block % 16 == 0 && (reinterpret_cast<uintptr_t>(base) & 15) == 0;
+        // the blocked kernels read and write whole 16-byte vectors: every block and every parity stream must be aligned
+        bool vec_ok = horner && block % 16 == 0 && (reinterpret_cast<uintptr_t>(base) & 15) == 0;
+        for (int p = 0; p < m && vec_ok; p++) vec_ok = ((reinterpret_cast<uintptr_t>(parity[p]) + uint64_t(poff)) & 15) == 0;
         if (vec_ok || nrows == 1) {
             for (int i = 0; i < k; i++) ins[i] = base + int64_t(i) * block;
             for (int p = 0; p < m; p++) outs[p] = static_cast<uint8_t*>(parity[p]) + poff;
