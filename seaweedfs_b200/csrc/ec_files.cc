@@ -645,6 +645,7 @@ int repair_pages(swec_encoder* enc, const Matrix& rows, const std::string& b, co
     if (rc) return rc;
     if ((rc = locator.init(rows, size, radius, enc->stream, /*correct=*/true))) return rc;
     if ((rc = submit_flagged(pipe, runs, chunk, in, in_d, [&](Item& it) { writes.add(it); }))) return rc;
+    pipe.report("repair_ec_damage");
     if ((rc = writes.sync(b))) return rc;
     return locator.collect(report, ranges, ranges_cap, n_ranges);
 }
@@ -966,6 +967,7 @@ int needle_damage_files(swec_encoder* enc, const std::vector<int>& in, int64_t s
         return rc;
     const std::function<void(Item&)> add = [&](Item& it) { writes.add(it); };
     if ((rc = submit_flagged(pipe, runs, chunk, in, std::vector<int>(in.size(), -1), repair ? add : nullptr))) return rc;
+    pipe.report(repair ? "repair_needle_damage" : "locate_needle_damage");
     if ((rc = writes.sync(""))) return rc;
     return nd.collect(recs->data(), unowned);
 }
