@@ -22,6 +22,9 @@
  *   swec_repair_ec_damage       (no counterpart) corrects the located bytes in place instead of rebuilding whole shards
  *   swec_rebuild_ec_files_checked  rebuildEcFiles reading every present shard (ec_encoder.go:342-357), which corrects
  *                               damage in the shards it rebuilds from instead of copying it into the rebuilt ones
+ *   swec_page_sketch_file,      (no counterpart) ScrubEcVolume FULL checks only needle CRCs over the network
+ *   swec_locate_sketch_damage   (weed/storage/store_ec_scrub.go); these check parity of a balanced volume from
+ *                               8 bytes per 4 KiB page of every shard
  *   swec_reconstruct_batch      batched ReconstructData   weed/storage/store_ec.go:482-560 (one call per interval today)
  *   swec_write_dat_file         WriteDatFile              weed/storage/erasure_coding/ec_decoder.go:176-223
  *   swec_ec_shards_generate     VolumeEcShardsGenerate (file work)   weed/server/volume_grpc_erasure_coding.go:43-146
@@ -408,6 +411,64 @@ int swec_reconstruct_checked_device(swec_encoder *enc, void *const *shards, cons
 int swec_write_dat_file(const char *base_file_name, int64_t dat_file_size,
                         const char *const *shard_file_names, int data_shards,
                         int64_t large_block, int64_t small_block);
+/* ---- locate damage across servers from per-page shard sketches -------------------------------------------------------
+ * The locate calls above need all k+m shards on one machine; a balanced EC volume has them on different servers.  Each
+ * server instead sketches its own shard into 8 bytes per 4 KiB page (0.2 % of the shard), and the coordinator decodes
+ * the sketches.  Definition (version SWEC_PAGE_SKETCH_VERSION; sketches from different versions must never be mixed):
+ *   - page g of a shard is the bytes [4096 g, min(4096 (g+1), len)); a shard has ceil(len / 4096) pages;
+ *   - the weight word of shard offset x is w(x) = splitmix64(seed + (x+1)·0x9E3779B97F4A7C15), word x of the
+ *     swec_synth_fill_device stream; w_l(x) is its byte l (little-endian), l = 0..7;
+ *   - byte l of sketch[g] (a uint64_t, little-endian) = XOR over x in page g of w_l(x) ⊗ c[x], over GF(2^8)/0x11D.
+ * Properties:
+ *   - Linearity: σ(a⊗c ⊕ b⊗c') = a⊗σ(c) ⊕ b⊗σ(c').  So for every page g and byte l, the k+m sketch bytes of a clean
+ *     set are a codeword of the same RS(k,m), and damage e_i in shard i on page g is the error σ_l(e_i) in position i
+ *     of sketch column (g, l).
+ *   - Misses: for a non-zero e_i, σ_l(e_i) is zero with probability 1/256 over the seed, so a damaged shard-page is
+ *     missed (all 8 bytes zero) with probability about 2^-64.  This assumes splitmix64's output behaves as uniform, a
+ *     property of the generator that is argued, not measured.  The coordinator must draw a fresh seed for every scrub:
+ *     damage is independent of a random seed, not of a known one.                                                  */
+#define SWEC_PAGE_SKETCH_VERSION 1
+/* The sketches of len bytes of one shard in device memory, whose first byte is shard offset first_column (a multiple
+ * of 4096, so that a long shard can be sketched in pieces that concatenate).  sketches: device memory for ceil(len/4096)
+ * words, 8-byte aligned; the shard may have any alignment.  len 0 writes nothing.  Asynchronous on `stream` (a
+ * cudaStream_t; NULL = the default stream).  SWEC_ERR_INVALID_ARG for a NULL pointer with len > 0, an unaligned
+ * sketches pointer or first_column; SWEC_ERR_NO_DEVICE for device < 0.                                            */
+int swec_page_sketch_device(int device, const void *shard, size_t len, uint64_t first_column, uint64_t seed,
+                            uint64_t *sketches, void *stream);
+/* The sketches of one shard file, read through the file pipeline's staging ring (O_DIRECT when "file_direct_io" bit 0
+ * is set) and sketched on the GPU `device`.  The file is only read.  *shard_len = the file's length, *n_pages = its
+ * pages; only the first sketches_cap sketches are written (sketches may be NULL when sketches_cap is 0).  Errors:
+ * SWEC_ERR_INVALID_ARG (NULL path, shard_len or n_pages, negative sketches_cap), SWEC_ERR_IO (open, stat or read
+ * failed), then SWEC_ERR_NO_DEVICE.  An empty file has no pages and needs no GPU.                                 */
+int swec_page_sketch_file(const char *shard_file, int device, uint64_t seed, uint64_t *sketches, int64_t sketches_cap,
+                          int64_t *shard_len, int64_t *n_pages);
+/* A page the sketches flag: blamed on the shards of blamed_mask (bit i = shard i), or uncorrectable (mask 0).        */
+typedef struct swec_sketch_page {
+    int64_t page;          /* shard offset / 4096                                                                  */
+    uint32_t blamed_mask;
+    int32_t uncorrectable; /* 1: no pattern of <= radius shards explains the page                                  */
+} swec_sketch_page;
+/* Which pages of which shards are damaged, from the k+m shards' sketches (host arrays of ceil(shard_len/4096) words,
+ * all taken with one seed).  The parity sketches are recomputed from the data sketches with the encoder's own encode
+ * path and compared with the stored ones; every page with a non-zero sketch syndrome is decoded column by column
+ * (each of its 8 bytes is one column) with the locate calls' decoder, and the columns' blame is merged.
+ *   - radius 0 (detect only), 1 or 2, with 2·radius <= m.  Every page with a non-zero syndrome is flagged.
+ *   - The result is PER PAGE, not per column.  Let D be the shards whose bytes on the page differ from the codeword
+ *     and t the radius.  |D| <= t: exactly D is blamed.  t < |D| <= m-t: the page is uncorrectable.  Each statement
+ *     fails only with probability <= |D|·2^-64 over the seed.  |D| > m-t: the page is flagged (same miss bound) but
+ *     its blame can be wrong, the limit of the code as for the locate calls.  Two shards damaged in DIFFERENT columns
+ *     of one page count as |D| = 2: at radius 1 the page is uncorrectable, although swec_locate_ec_damage would blame
+ *     both shards column by column.  Fetching such a page from all k+m shards and running swec_correct_damage_device
+ *     on it resolves it (INTEGRATION.md).
+ *   - pages[] receives the flagged pages in ascending page order, the first pages_cap of them; *n_flagged = how many
+ *     there are.  shard_pages[i] (SWEC_MAX_SHARDS entries, may be NULL) = pages blamed on shard i.  *ok = 1 iff no
+ *     page is flagged.
+ * Errors, all before any device work: SWEC_ERR_INVALID_ARG (NULL enc, sketches, n_flagged or ok, negative shard_len or
+ * pages_cap, pages NULL with pages_cap > 0, a radius out of range); then SWEC_ERR_TOO_FEW_SHARDS for a NULL sketch (a
+ * lost shard must be rebuilt first); then SWEC_ERR_NO_DEVICE for an encoder without a device.  Synchronous.      */
+int swec_locate_sketch_damage(swec_encoder *enc, const uint64_t *const *sketches, int64_t shard_len, int radius,
+                              swec_sketch_page *pages, int64_t pages_cap, int64_t *n_flagged,
+                              uint64_t *shard_pages, int *ok);
 /* ---- checked decode: errors and erasures before the parity is dropped -----------------------------------------------
  * ec.decode deletes every shard, parity included, once the .dat is written (weed/shell/command_ec_decode.go:156-181),
  * so it is the last point at which damage in the data shards can be corrected.  swec_write_dat_file copies the data

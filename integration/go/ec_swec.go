@@ -16,6 +16,7 @@ import "C"
 import (
 	"fmt"
 	"io"
+	"os"
 	"runtime"
 	"strings"
 	"sync/atomic"
@@ -566,6 +567,79 @@ func swecLocateEcDamage(baseFileName string, ctx *ECContext, additionalDirs []st
 			uint64(report.uncorrectable_columns), int64(report.first_uncorrectable), int64(report.last_uncorrectable)))
 	}
 	return broken, details, nil
+}
+
+// swecPageSketchFile answers the shard holder's side of a distributed parity scrub (a VolumeEcShardSketch RPC): the
+// page sketches of one local shard file, 8 bytes per 4 KiB page, under the coordinator's seed.  The caller must check
+// that the coordinator asked for SWEC_PAGE_SKETCH_VERSION.  The file is only read.
+func swecPageSketchFile(shardFileName string, seed uint64) (sketches []uint64, shardSize int64, err error) {
+	cs := C.CString(shardFileName)
+	defer C.free(unsafe.Pointer(cs))
+	st, err := os.Stat(shardFileName)
+	if err != nil {
+		return nil, 0, err
+	}
+	for capPages := (st.Size() + 4095) / 4096; ; {
+		buf := make([]uint64, capPages+1) // +1: never a zero-length slice to take the address of
+		var length, nPages C.int64_t
+		if err := swecCall(func() C.int {
+			return C.swec_page_sketch_file(cs, swecPickDevice(), C.uint64_t(seed), (*C.uint64_t)(unsafe.Pointer(&buf[0])),
+				C.int64_t(capPages), &length, &nPages)
+		}); err != nil {
+			return nil, 0, fmt.Errorf("page sketch %s: %w", shardFileName, err)
+		}
+		if int64(nPages) <= capPages {
+			return buf[:nPages], int64(length), nil
+		}
+		capPages = int64(nPages) // the file grew since the stat
+	}
+}
+
+// swecSketchPage is one page the coordinator must fetch: blamed on the shards of Blamed (bit i = shard i), or
+// Uncorrectable (fetch it from all k+m shards and run swec_correct_damage_device on them).
+type swecSketchPage struct {
+	Page          int64
+	Blamed        uint32
+	Uncorrectable bool
+}
+
+// swecLocateSketchDamage is the coordinator's side (the ScrubEcVolume FULL handler or ec.scrub): the pages of a balanced
+// volume that are damaged, from every shard holder's sketches and shard size, all taken with one fresh seed.  Unequal
+// sizes are the ErrShardSize of a rebuild; a shard whose holder did not answer must be rebuilt first.  Radius 1 blames a
+// page on one shard; a page damaged in two shards comes back Uncorrectable even when no column of it is (INTEGRATION.md).
+func swecLocateSketchDamage(enc *swecEncoder, sketches [][]uint64, shardSizes []int64) (pages []swecSketchPage, err error) {
+	for _, s := range shardSizes[1:] {
+		if s != shardSizes[0] {
+			return nil, fmt.Errorf("ec shard size expected %d actual %d", shardSizes[0], s)
+		}
+	}
+	nPages := (shardSizes[0] + 4095) / 4096
+	var p runtime.Pinner
+	defer p.Unpin()
+	ptrs := (*[C.SWEC_MAX_SHARDS]*C.uint64_t)(C.calloc(C.SWEC_MAX_SHARDS, C.size_t(unsafe.Sizeof(uintptr(0)))))
+	defer C.free(unsafe.Pointer(ptrs))
+	for i, s := range sketches {
+		if int64(len(s)) != nPages {
+			return nil, fmt.Errorf("ec shard %d: %d sketches for %d pages", i, len(s), nPages)
+		}
+		if nPages > 0 {
+			p.Pin(&s[0])
+			ptrs[i] = (*C.uint64_t)(unsafe.Pointer(&s[0]))
+		}
+	}
+	out := make([]C.swec_sketch_page, nPages+1)
+	var nFlagged C.int64_t
+	var ok C.int
+	if err := swecCall(func() C.int {
+		return C.swec_locate_sketch_damage(enc.h, &ptrs[0], C.int64_t(shardSizes[0]), 1, &out[0], C.int64_t(nPages),
+			&nFlagged, nil, &ok)
+	}); err != nil {
+		return nil, fmt.Errorf("locate sketch damage: %w", err)
+	}
+	for _, q := range out[:nFlagged] {
+		pages = append(pages, swecSketchPage{int64(q.page), uint32(q.blamed_mask), q.uncorrectable != 0})
+	}
+	return pages, nil
 }
 
 // swecRepairEcDamage is swecLocateEcDamage, which also corrects the located bytes in the shard files: only the damaged

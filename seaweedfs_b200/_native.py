@@ -64,6 +64,10 @@ class NeedleDamage(C.Structure):
                 ("damaged_bytes", C.c_uint64), ("uncorrectable_bytes", C.c_uint64)]
 
 
+class SketchPage(C.Structure):
+    _fields_ = [("page", C.c_int64), ("blamed_mask", C.c_uint32), ("uncorrectable", C.c_int32)]
+
+
 NEEDLE_STATUS = {0: "ok", 1: "size mismatch", 2: "out of range", 3: "bad crc", 4: "outside image"}
 
 
@@ -138,6 +142,12 @@ PROTOTYPES = {
     "swec_decode_data_checked_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int,
                                                   C.POINTER(DamageReport), C.POINTER(DamageRange), C.c_int,
                                                   C.POINTER(C.c_int), C.c_void_p]),
+    "swec_page_sketch_device": (C.c_int, [C.c_int, C.c_void_p, C.c_size_t, C.c_uint64, C.c_uint64, C.c_void_p,
+                                          C.c_void_p]),
+    "swec_page_sketch_file": (C.c_int, [C.c_char_p, C.c_int, C.c_uint64, C.c_void_p, C.c_int64, C.POINTER(C.c_int64),
+                                        C.POINTER(C.c_int64)]),
+    "swec_locate_sketch_damage": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.POINTER(SketchPage),
+                                            C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_uint64), C.POINTER(C.c_int)]),
     "swec_write_dat_file": (C.c_int, [C.c_char_p, C.c_int64, C.c_void_p, C.c_int, C.c_int64, C.c_int64]),
     "swec_write_dat_file_checked": (C.c_int, [C.c_char_p, C.c_int64, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_int64,
                                               C.c_int, C.c_int, C.POINTER(DamageReport), C.POINTER(DamageRange), C.c_int,

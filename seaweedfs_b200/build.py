@@ -22,10 +22,10 @@ GEN = os.path.join(CSRC, "generated")
 LIB = os.path.join(HERE, "libswec.so")
 ROOT = os.path.dirname(HERE)
 
-SOURCES = ["kernels.cu", "aot_recon.cu", "needles.cu", "damage.cu", "needle_damage.cu", "engine.cc", "host_seam.cc", "ec_files.cc", "ec_index.cc", "ec_volume.cc", "volume_format.cc", "staging.cc",
+SOURCES = ["kernels.cu", "aot_recon.cu", "needles.cu", "damage.cu", "needle_damage.cu", "sketch.cu", "engine.cc", "host_seam.cc", "ec_files.cc", "ec_index.cc", "ec_volume.cc", "volume_format.cc", "staging.cc",
            "jit.cc", "codegen.cc", "gf256.cc"]
 HEADERS = ["apply_params.h", "device_common.cuh", "tma_fetch.cuh", "kernels.h", "engine.h", "host_seam.h", "gf256.h", "codegen.h", "io_pool.h", "mini_json.h",
-           "volume_format.h", "needle_format.h", "needles.h", "damage.h", "needle_damage.h", "stripe_map.h", "staging.h", os.path.join(ROOT, "include", "swec.h")]
+           "volume_format.h", "needle_format.h", "needles.h", "damage.h", "needle_damage.h", "sketch.h", "locate_decode.cuh", "stripe_map.h", "staging.h", os.path.join(ROOT, "include", "swec.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC,-Wall,-Wno-unused-function", "-cudart", "static"]
 

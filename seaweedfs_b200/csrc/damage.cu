@@ -30,6 +30,7 @@
 //                        missing data shards and the check shards only, and it also XORs each located error value of an
 //                        information position that holds a data shard into that shard's own byte, so every data byte of
 //                        a column decoded within the radius is the true one.  Present parity shards are never written.
+// The column decoder (decode_column) lives in locate_decode.cuh, which the page decode of the sketch calls shares.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -40,6 +41,7 @@
 #include "damage.h"
 #include "device_common.cuh"
 #include "engine.h"
+#include "locate_decode.cuh"
 
 namespace swec {
 
@@ -52,14 +54,6 @@ constexpr u8 kLogZero = 0xff;               // log R entry of a zero coefficient
 
 enum : int { kLocate = 0, kCorrect = 1, kRebuild = 2, kDecode = 3 };  // the instantiations of swec_locate_kernel
 
-struct LocateTables {
-    u8 log[256];
-    u8 exp[512];         // two periods of 2^i: a sum of two logs needs no reduction
-    u8 logp[32 * 32];    // log P[i][j] at i*32 + j
-    u8 logdet[32 * 32];  // log det [P0a P0b; P1a P1b] at a*32 + b (a != b data shards)
-};
-constexpr int kTableWords = int(sizeof(LocateTables) / 4);
-static_assert(sizeof(LocateTables) % 16 == 0, "tables are copied in words");
 
 // kRebuild and kDecode only, in shared memory of its own so that the other instantiations copy no more than before
 struct RebuildTables {
@@ -135,98 +129,6 @@ __device__ __forceinline__ void record(const LocateParams& p, Run* run, int set,
     }
     run[i].cnt++;
     run[i].last = off;
-}
-
-__device__ __forceinline__ u8 gmul(const LocateTables& t, int log_c, u8 v) { return v ? t.exp[log_c + t.log[v]] : 0; }
-
-// rows other than `skip` of s (logs in L, all non-zero) are one multiple of column j of P; r is the log of that
-// multiple, the error value of data shard j
-__device__ __forceinline__ bool multiple_of_column(const LocateTables& t, const u8* L, int m, int j, int skip, int& r) {
-    r = -1;
-    for (int i = 0; i < m; i++) {
-        if (i == skip) continue;
-        int d = int(L[i]) - int(t.logp[i * 32 + j]);
-        if (d < 0) d += 255;
-        if (r < 0) r = d;
-        else if (d != r) return false;
-    }
-    return true;
-}
-
-// Shards that explain the non-zero syndrome s within the radius, ascending in *a, *b; returns how many (0: none does).
-// VALUES: also their error values in *ea, *eb, the bytes that XORed into the shards turn the column into a codeword.
-template <bool VALUES>
-__device__ int decode_column(const LocateTables& t, const u8* s, int k, int m, int radius, int* a, int* b, u8* ea, u8* eb) {
-    u8 L[SWEC_MAX_SHARDS];
-    u32 nz = 0;
-    for (int i = 0; i < m; i++) {
-        L[i] = t.log[s[i]];
-        if (s[i]) nz |= 1u << i;
-    }
-    const int w = __popc(nz);
-    if (w == 1) {
-        *a = k + __ffs(nz) - 1;
-        if (VALUES) *ea = s[*a - k];
-        return 1;
-    }
-    if (w == m)  // every entry of an MDS P is non-zero
-        for (int j = 0; j < k; j++) {
-            int r;
-            if (multiple_of_column(t, L, m, j, -1, r)) {
-                *a = j;
-                if (VALUES) *ea = t.exp[r];
-                return 1;
-            }
-        }
-    if (radius < 2) return 0;
-    if (w == 2) {
-        *a = k + __ffs(nz) - 1;
-        *b = k + __ffs(nz & (nz - 1)) - 1;
-        if (VALUES) {
-            *ea = s[*a - k];
-            *eb = s[*b - k];
-        }
-        return 2;
-    }
-    if (w < m - 1) return 0;  // a data shard in the pattern makes at least m-1 components non-zero
-    for (int q = 0; q < m; q++) {
-        if (w == m - 1 && ((nz >> q) & 1)) continue;  // the zero component can only be the parity shard's
-        for (int j = 0; j < k; j++) {
-            int r;
-            if (multiple_of_column(t, L, m, j, q, r)) {
-                *a = j;
-                *b = k + q;
-                if (VALUES) {  // s_q = P[q][j]·e_j ^ e_q
-                    *ea = t.exp[r];
-                    *eb = s[q] ^ t.exp[r + t.logp[q * 32 + j]];
-                }
-                return 2;
-            }
-        }
-    }
-    for (int x = 0; x + 1 < k; x++)
-        for (int y = x + 1; y < k; y++) {
-            // [P0x P0y; P1x P1y]·[ex; ey] = [s0; s1]
-            const u8 nx = gmul(t, t.logp[32 + y], s[0]) ^ gmul(t, t.logp[y], s[1]);
-            const u8 ny = gmul(t, t.logp[32 + x], s[0]) ^ gmul(t, t.logp[x], s[1]);
-            if (!nx || !ny) continue;
-            const int ld = t.logdet[x * 32 + y];
-            int lx = int(t.log[nx]) - ld, ly = int(t.log[ny]) - ld;
-            if (lx < 0) lx += 255;
-            if (ly < 0) ly += 255;
-            bool ok = true;
-            for (int i = 2; i < m && ok; i++) ok = (t.exp[lx + t.logp[i * 32 + x]] ^ t.exp[ly + t.logp[i * 32 + y]]) == s[i];
-            if (ok) {
-                *a = x;
-                *b = y;
-                if (VALUES) {
-                    *ea = t.exp[lx];
-                    *eb = t.exp[ly];
-                }
-                return 2;
-            }
-        }
-    return 0;
 }
 
 // kRebuild: the error value e of position j carried into byte x of every rebuilt stream (nothing for a check position)
@@ -391,18 +293,6 @@ void launch_locate(int m, const LocateParams& p, u64 n, cudaStream_t s) {
     swec_locate_kernel<MT, MODE><<<locate_grid<MT, MODE>(n), 256, 0, s>>>(p);
 }
 
-// logs of the field's non-zero bytes (to base 2), and two periods of powers of 2
-void log_exp_tables(u8* log, u8* exp) {
-    unsigned x = 1;
-    for (int i = 0; i < 255; i++) {
-        exp[i] = u8(x);
-        log[x] = u8(i);
-        x <<= 1;
-        if (x & 0x100) x ^= kFieldPoly;
-    }
-    for (int i = 255; i < 512; i++) exp[i] = exp[i - 255];
-}
-
 }  // namespace
 
 int check_locate_args(int m, int radius, const swec_damage_report* report, const swec_damage_range* ranges,
@@ -475,15 +365,7 @@ int DamageLocator::init(const Matrix& parity, int64_t shard_len, int radius, cud
     ids_.resize(size_t(k_ + m_));
     for (int i = 0; i < k_ + m_; i++) ids_[size_t(i)] = i;
     LocateTables t;
-    memset(&t, 0, sizeof t);
-    log_exp_tables(t.log, t.exp);
-    const GF& gf = GF::get();
-    for (int i = 0; i < m_; i++)
-        for (int j = 0; j < k_; j++) t.logp[i * 32 + j] = t.log[parity.at(i, j)];
-    for (int a = 0; a < k_ && m_ >= 2; a++)
-        for (int b = 0; b < k_; b++)
-            if (a != b)
-                t.logdet[a * 32 + b] = t.log[gf.mul[parity.at(0, a)][parity.at(1, b)] ^ gf.mul[parity.at(0, b)][parity.at(1, a)]];
+    locate_tables(parity, &t);
     const int64_t pages = (shard_len + (int64_t(1) << kPageShift) - 1) >> kPageShift;
     page_words_ = std::max<size_t>(1, size_t((pages + 31) / 32));
     const size_t page_bytes = size_t(k_ + m_ + 1) * page_words_ * 4;

@@ -31,6 +31,7 @@
 #include "engine.h"
 #include "io_pool.h"
 #include "needle_damage.h"
+#include "sketch.h"
 #include "volume_format.h"
 
 namespace swec {
@@ -1111,6 +1112,49 @@ int swec_verify_ec_files(const char* base, const char* const* dirs, int ndirs, i
         all_ok = all_ok && bad[size_t(p)] == 0;
     }
     *ok = all_ok ? 1 : 0;
+    return SWEC_OK;
+}
+
+int swec_page_sketch_file(const char* path, int device, uint64_t seed, uint64_t* sketches, int64_t sketches_cap,
+                          int64_t* shard_len, int64_t* n_pages) {
+    if (!path || !shard_len || !n_pages || sketches_cap < 0 || (sketches_cap > 0 && !sketches))
+        return fail(SWEC_ERR_INVALID_ARG, "NULL argument or negative sketches_cap");
+    FdSet fds;
+    const int fd = fds.keep(open(path, O_RDONLY));
+    if (fd < 0) return io_fail(std::string("open ") + path);
+    struct stat st;
+    if (fstat(fd, &st) != 0) return io_fail(std::string("stat ") + path);
+    const int64_t size = int64_t(st.st_size), pages = (size + 4095) / 4096;
+    if (size > 0) {
+        // one stream read per slot and no matrix: the step sketches it; items start on page boundaries
+        CallEncoder enc;
+        int rc = new_call_encoder(1, 1, device, &enc);
+        if (rc) return rc;
+        const int dfd = fds.keep(open_direct(path, O_RDONLY, g_opt_file_direct_io.load() & 1));
+        if ((rc = enc->ensure_device())) return rc;
+        DeviceBuffer dev;  // declared before the pipeline: freed after its shutdown has drained every slot
+        SWEC_CUDA(dev.alloc(size_t(pages) * 8));
+        const size_t chunk = (file_chunk(size) + 4095) & ~size_t(4095);
+        FilePipeline pipe(enc.get(), Matrix(0, 0), chunk, 1, [&](uint8_t* const*, uint8_t* const* shards, size_t len,
+                                                                 int64_t base, int, cudaStream_t s) -> int {
+            SWEC_CUDA(launch_page_sketch(shards[0], len, u64(base), seed, dev.as<u64>() + base / 4096, s));
+            return SWEC_OK;
+        });
+        if ((rc = pipe.start())) return rc;
+        for (int64_t o = 0; o < size; o += int64_t(chunk)) {
+            Item it;
+            it.len = size_t(std::min<int64_t>(int64_t(chunk), size - o));
+            it.shard_off = o;
+            it.reads.push_back({0, fd, o, 0, it.len, dfd});
+            if (pipe.submit(std::move(it))) break;
+        }
+        if ((rc = pipe.finish())) return rc;
+        pipe.report("page_sketch");
+        if (const int64_t n = std::min(sketches_cap, pages))
+            SWEC_CUDA(cudaMemcpy(sketches, dev.as<u64>(), size_t(n) * 8, cudaMemcpyDeviceToHost));
+    }
+    *shard_len = size;
+    *n_pages = pages;
     return SWEC_OK;
 }
 

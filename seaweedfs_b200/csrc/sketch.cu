@@ -1,0 +1,265 @@
+// seaweedfs_b200/csrc/sketch.cu — page sketches of shards, and damage located from the sketches of a whole set.
+//
+//   swec_page_sketch_kernel   one warp per 4 KiB page, grid-stride.  Bit-sliced: a lane keeps eight words T_b, T_b the
+//                             XOR of the weight words w(x) of its columns whose byte has bit b set, so each column costs
+//                             one splitmix64 and eight masked XORs.  The lane's share of the page is then
+//                             ⊕_b 2^b ⊗ T_b (Horner over b with a multiply-by-2 on all 8 bytes at once), and the warp
+//                             XORs its 32 shares with shuffles.  A whole page of an aligned shard is read as 8 coalesced
+//                             16-byte loads per lane; the partial last page and unaligned shards go byte by byte.
+//   swec_sketch_pages_kernel  the page decode of swec_locate_sketch_damage: one thread per page, the 8 bytes of its
+//                             sketch syndromes decoded as 8 columns by the locate kernels' decoder (locate_decode.cuh),
+//                             and their blame merged per page.
+#include <cuda_runtime.h>
+
+#include <algorithm>
+#include <cstring>
+#include <string>
+#include <vector>
+
+#include "device_common.cuh"
+#include "engine.h"
+#include "locate_decode.cuh"
+#include "sketch.h"
+
+namespace swec {
+
+namespace {
+
+constexpr u64 kPage = 4096;
+constexpr u64 kGolden = 0x9E3779B97F4A7C15ull;  // splitmix64's increment: w(x) = mix(seed + (x+1)·kGolden)
+
+__device__ __forceinline__ u64 mix(u64 z) {
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+
+// column with byte c and weight word w into the slices
+__device__ __forceinline__ void take(u64 (&t)[8], u64 w, u32 c) {
+#pragma unroll
+    for (int b = 0; b < 8; b++) t[b] ^= w & (0ull - u64((c >> b) & 1u));
+}
+
+// 2 ⊗ every byte of a (GF(2^8)/0x11D)
+__device__ __forceinline__ u64 xtime8(u64 a) {
+    return ((a & 0x7f7f7f7f7f7f7f7full) << 1) ^ (((a >> 7) & 0x0101010101010101ull) * 0x1d);
+}
+
+__global__ void __launch_bounds__(256) swec_page_sketch_kernel(const u8* __restrict__ src, u64 n, u64 first_column,
+                                                               u64 seed, u64* __restrict__ out) {
+    const u64 pages = (n + kPage - 1) / kPage;
+    const u32 lane = threadIdx.x & 31;
+    const u64 warps = (u64)gridDim.x * (blockDim.x >> 5);
+    const bool vec = (reinterpret_cast<unsigned long long>(src) & 15) == 0;
+    for (u64 g = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 5; g < pages; g += warps) {
+        const u64 p0 = g * kPage;
+        const u64 len = min(kPage, n - p0);
+        const u64 z0 = seed + (first_column + p0 + 1) * kGolden;  // before mix: the weight of the page's first column
+        u64 t[8];
+#pragma unroll
+        for (int b = 0; b < 8; b++) t[b] = 0;
+        if (vec && len == kPage) {
+            uint4 d[8];
+#pragma unroll
+            for (int j = 0; j < 8; j++) d[j] = swec_ldg_stream(src + p0 + (u64(lane + 32 * j) << 4));
+#pragma unroll
+            for (int j = 0; j < 8; j++) {
+                u64 z = z0 + u64((lane + 32 * j) << 4) * kGolden;
+                const u32 w[4] = {d[j].x, d[j].y, d[j].z, d[j].w};
+#pragma unroll
+                for (int c = 0; c < 16; c++, z += kGolden) take(t, mix(z), w[c >> 2] >> (8 * (c & 3)));
+            }
+        } else {
+            for (u32 x = lane; x < len; x += 32) take(t, mix(z0 + u64(x) * kGolden), src[p0 + x]);
+        }
+        u64 r = t[7];
+#pragma unroll
+        for (int b = 6; b >= 0; b--) r = xtime8(r) ^ t[b];
+#pragma unroll
+        for (int s = 16; s > 0; s >>= 1) r ^= __shfl_xor_sync(0xffffffffu, r, s);
+        if (lane == 0) out[g] = r;
+    }
+}
+
+struct SketchPageParams {
+    const u64* comp[SWEC_MAX_SHARDS];    // parity sketches recomputed from the data sketches
+    const u64* stored[SWEC_MAX_SHARDS];  // parity sketches as the parity shards' holders sent them
+    u64 pages;
+    int k, m, radius;
+    const u32* tables;            // LocateTables
+    swec_sketch_page* flagged;    // one entry per flagged page, in no particular order
+    unsigned long long* count;    // entries written
+};
+
+// Page decode, one thread per page, grid-stride.  Byte l of the m sketch syndromes of page g is the syndrome of sketch
+// column (g, l): each non-zero column is decoded as the locate kernel decodes a byte column, and the page is blamed on
+// the union of its columns' blame, or uncorrectable when a column is or the union exceeds the radius.  Radius 0
+// decodes nothing.  Clean pages cost the loads.
+__global__ void __launch_bounds__(256) swec_sketch_pages_kernel(const __grid_constant__ SketchPageParams p) {
+    __shared__ __align__(16) u32 words[kTableWords];
+    for (int i = threadIdx.x; i < kTableWords; i += blockDim.x) words[i] = p.tables[i];
+    __syncthreads();
+    const LocateTables& t = *reinterpret_cast<const LocateTables*>(words);
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 g = (u64)blockIdx.x * blockDim.x + threadIdx.x; g < p.pages; g += stride) {
+        u64 any = 0;
+        for (int i = 0; i < p.m; i++) any |= p.comp[i][g] ^ p.stored[i][g];
+        if (!any) continue;
+        u32 mask = 0;
+        bool bad = false;
+        for (int l = 0; l < 8 && !bad; l++) {
+            u8 s[SWEC_MAX_SHARDS];
+            u8 nz = 0;
+            for (int i = 0; i < p.m; i++) {
+                s[i] = u8((p.comp[i][g] ^ p.stored[i][g]) >> (8 * l));
+                nz |= s[i];
+            }
+            if (!nz) continue;
+            int a = -1, b = -1;
+            u8 ea = 0, eb = 0;
+            const int found = p.radius == 0 ? 0 : decode_column<false>(t, s, p.k, p.m, p.radius, &a, &b, &ea, &eb);
+            bad = !found;
+            if (found >= 1) mask |= 1u << a;
+            if (found == 2) mask |= 1u << b;
+        }
+        bad = bad || __popc(mask) > p.radius;
+        const unsigned long long at = atomicAdd(p.count, 1ull);
+        p.flagged[at].page = int64_t(g);
+        p.flagged[at].blamed_mask = bad ? 0u : mask;
+        p.flagged[at].uncorrectable = bad ? 1 : 0;
+    }
+}
+
+// The page decode: comp[p] and stored[p] are the recomputed and the stored sketches of parity shard p, `pages` words
+// each, in device memory.  Every page whose syndrome is not zero goes into *flagged, in ascending page order.
+// Synchronises `s`.
+int locate_sketch_pages(const Matrix& parity, const uint8_t* const* comp, const uint8_t* const* stored, int64_t pages,
+                        int radius, cudaStream_t s, std::vector<swec_sketch_page>* flagged) {
+    LocateTables t;
+    locate_tables(parity, &t);
+    DeviceBuffer tables;
+    SWEC_CUDA(tables.upload(&t, 1, s));
+    StreamScratch out(s);
+    SWEC_CUDA(out.alloc(sizeof(unsigned long long) + size_t(pages) * sizeof(swec_sketch_page)));
+    SketchPageParams p;
+    memset(&p, 0, sizeof p);
+    for (int i = 0; i < parity.rows; i++) {
+        p.comp[i] = reinterpret_cast<const u64*>(comp[i]);
+        p.stored[i] = reinterpret_cast<const u64*>(stored[i]);
+    }
+    p.pages = u64(pages);
+    p.k = parity.cols;
+    p.m = parity.rows;
+    p.radius = radius;
+    p.tables = tables.as<u32>();
+    p.count = out.as<unsigned long long>();
+    p.flagged = reinterpret_cast<swec_sketch_page*>(p.count + 1);
+    SWEC_CUDA(cudaMemsetAsync(p.count, 0, sizeof *p.count, s));
+    static const int per_sm = [] {
+        int c = 0;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, swec_sketch_pages_kernel, 256, 0) != cudaSuccess) {
+            cudaGetLastError();
+            c = 4;
+        }
+        return std::max(1, c);
+    }();
+    swec_sketch_pages_kernel<<<grid_for(u64(pages), 256, per_sm), 256, 0, s>>>(p);
+    SWEC_CUDA(launched());
+    unsigned long long n = 0;
+    SWEC_CUDA(cudaMemcpyAsync(&n, p.count, sizeof n, cudaMemcpyDeviceToHost, s));
+    SWEC_CUDA(cudaStreamSynchronize(s));
+    flagged->resize(size_t(n));
+    if (n) {
+        SWEC_CUDA(cudaMemcpyAsync(flagged->data(), p.flagged, size_t(n) * sizeof(swec_sketch_page), cudaMemcpyDeviceToHost, s));
+        SWEC_CUDA(cudaStreamSynchronize(s));
+    }
+    std::sort(flagged->begin(), flagged->end(),
+              [](const swec_sketch_page& a, const swec_sketch_page& b) { return a.page < b.page; });
+    return SWEC_OK;
+}
+
+}  // namespace
+
+cudaError_t launch_page_sketch(const void* shard, u64 n, u64 first_column, u64 seed, u64* sketches, cudaStream_t s) {
+    if (n == 0) return cudaSuccess;
+    static const int per_sm = [] {  // resident CTAs per SM, the same on every device of this architecture
+        int c = 0;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, swec_page_sketch_kernel, 256, 0) != cudaSuccess) {
+            cudaGetLastError();
+            c = 4;
+        }
+        return std::max(1, c);
+    }();
+    const u64 pages = (n + kPage - 1) / kPage;
+    swec_page_sketch_kernel<<<grid_for(pages, 8, per_sm), 256, 0, s>>>(static_cast<const u8*>(shard), n, first_column,
+                                                                       seed, sketches);
+    return launched();
+}
+
+}  // namespace swec
+
+using namespace swec;
+
+extern "C" {
+
+int swec_page_sketch_device(int device, const void* shard, size_t len, uint64_t first_column, uint64_t seed,
+                            uint64_t* sketches, void* stream) {
+    if (len > 0 && (!shard || !sketches)) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
+    if (first_column % kPage) return fail(SWEC_ERR_INVALID_ARG, "first_column must be a multiple of 4096");
+    if (reinterpret_cast<uintptr_t>(sketches) & 7) return fail(SWEC_ERR_INVALID_ARG, "sketches must be 8-byte aligned");
+    if (device < 0) return fail(SWEC_ERR_NO_DEVICE, "device < 0; no CPU fallback exists");
+    if (len == 0) return SWEC_OK;
+    SWEC_CUDA(cudaSetDevice(device));
+    SWEC_CUDA(launch_page_sketch(shard, len, first_column, seed, reinterpret_cast<u64*>(sketches),
+                                 static_cast<cudaStream_t>(stream)));
+    return SWEC_OK;
+}
+
+int swec_locate_sketch_damage(swec_encoder* e, const uint64_t* const* sketches, int64_t shard_len, int radius,
+                              swec_sketch_page* pages, int64_t pages_cap, int64_t* n_flagged, uint64_t* shard_pages,
+                              int* ok) {
+    if (!e || !sketches || !n_flagged || !ok) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
+    if (shard_len < 0) return fail(SWEC_ERR_INVALID_ARG, "shard_len must be >= 0");
+    if (pages_cap < 0 || (pages_cap > 0 && !pages))
+        return fail(SWEC_ERR_INVALID_ARG, "pages_cap must be >= 0, and pages non-NULL when it is > 0");
+    if (radius < 0 || radius > 2) return fail(SWEC_ERR_INVALID_ARG, "radius must be 0, 1 or 2");
+    const int k = e->k, m = e->m;
+    if (2 * radius > m)
+        return fail(SWEC_ERR_INVALID_ARG, "radius " + std::to_string(radius) + " needs at least " +
+                                              std::to_string(2 * radius) + " parity shards, the code has " + std::to_string(m));
+    for (int i = 0; i < k + m; i++)
+        if (!sketches[i])
+            return fail(SWEC_ERR_TOO_FEW_SHARDS, "no sketch of shard " + std::to_string(i) + ": rebuild it first");
+    std::lock_guard<std::mutex> lock(e->mu);
+    int rc = e->ensure_device();
+    if (rc) return rc;
+    cudaStream_t s = e->stream;
+    const int64_t n_pages = (shard_len + int64_t(kPage) - 1) / int64_t(kPage);
+    const size_t bytes = size_t(n_pages) * 8;
+    std::vector<swec_sketch_page> flagged;
+    if (n_pages > 0) {
+        // the k+m sketches as uploaded, then the m recomputed parity sketches
+        StreamScratch buf(s);
+        SWEC_CUDA(buf.alloc(size_t(k + 2 * m) * bytes));
+        uint8_t* at[SWEC_MAX_SHARDS];
+        uint8_t* comp[SWEC_MAX_SHARDS];
+        for (int i = 0; i < k + m; i++) {
+            at[i] = buf.as<uint8_t>() + size_t(i) * bytes;
+            SWEC_CUDA(cudaMemcpyAsync(at[i], sketches[i], bytes, cudaMemcpyHostToDevice, s));
+        }
+        for (int p = 0; p < m; p++) comp[p] = buf.as<uint8_t>() + size_t(k + m + p) * bytes;
+        // sketches are linear: the parity rows applied to the data sketches give the clean parity sketches
+        if ((rc = e->apply(parity_rows(e), at, comp, bytes, Layout{}, s))) return rc;
+        if ((rc = locate_sketch_pages(parity_rows(e), comp, at + k, n_pages, radius, s, &flagged))) return rc;
+    }
+    if (shard_pages) memset(shard_pages, 0, SWEC_MAX_SHARDS * sizeof *shard_pages);
+    for (size_t i = 0; i < flagged.size(); i++) {
+        if (int64_t(i) < pages_cap) pages[i] = flagged[i];
+        for (uint32_t b = flagged[i].blamed_mask; b && shard_pages; b &= b - 1) shard_pages[__builtin_ctz(b)]++;
+    }
+    *n_flagged = int64_t(flagged.size());
+    *ok = flagged.empty() ? 1 : 0;
+    return SWEC_OK;
+}
+
+}  // extern "C"

@@ -18,8 +18,8 @@ from dataclasses import dataclass
 
 import numpy as np
 
-from ._native import (STATUS, DamageRange, DamageReport, Interval, NeedleDamage, NeedleRead, ReconstructItem, SwecError,
-                      check, lib)
+from ._native import (STATUS, DamageRange, DamageReport, Interval, NeedleDamage, NeedleRead, ReconstructItem, SketchPage,
+                      SwecError, check, lib)
 
 DataShardsCount = 10                               # ec_encoder.go:20
 ParityShardsCount = 4                              # ec_encoder.go:21
@@ -238,6 +238,43 @@ class Encoder:
                                                     C.byref(report), ranges, max_ranges, C.byref(n), stream))
         return _damage_result(report, ranges, n.value, max_ranges)
 
+    def page_sketch_device(self, shard_ptr: int, shard_len: int, sketches_ptr: int, seed: int, first_column: int = 0,
+                           stream: int = 0) -> None:
+        """The page sketches (include/swec.h, SWEC_PAGE_SKETCH_VERSION) of shard_len bytes of one shard in device
+        memory, whose first byte is shard offset first_column (a multiple of 4096), into ceil(shard_len / 4096) words
+        at sketches_ptr on this encoder's device (swec_page_sketch_device).  Asynchronous on `stream`."""
+        check(lib().swec_page_sketch_device(self.device, shard_ptr, shard_len, first_column, seed, sketches_ptr, stream))
+
+    def locate_sketch_damage(self, sketches, shard_len, radius: int = 1) -> dict:
+        """Which pages of which shards are damaged, from the k+m shards' page sketches, all taken with one seed
+        (swec_locate_sketch_damage).  sketches: k+m uint64 arrays (None: a lost shard, SWEC_ERR_TOO_FEW_SHARDS).
+        shard_len: the shard length, or the k+m lengths the holders reported, which must be equal (ErrShardSize).
+        Returns ok, "pages" = [(page, blamed shard mask, uncorrectable)] in ascending page order, "n_flagged" and
+        "shard_pages" = {shard id: pages blamed on it}.  The result is per page, not per column (include/swec.h)."""
+        if not isinstance(shard_len, int):
+            lengths = {int(n) for n in shard_len}
+            if len(lengths) != 1:
+                raise SwecError(-6, "shards are of different sizes (ErrShardSize)")
+            shard_len = lengths.pop()
+        if len(sketches) != self.total_shards:
+            raise SwecError(-1, f"need {self.total_shards} sketches, got {len(sketches)}")
+        n_pages = (shard_len + 4095) // 4096
+        keep = []
+        for s in sketches:
+            if s is not None:
+                s = np.ascontiguousarray(s, dtype=np.uint64)
+                if s.shape != (n_pages,):
+                    raise SwecError(-1, f"a sketch array must hold {n_pages} words, got {s.shape}")
+            keep.append(s)
+        ptrs = _ptrs(keep)
+        pages = (SketchPage * max(1, n_pages))()
+        n, per_shard, ok = C.c_int64(0), (C.c_uint64 * MaxShardCount)(), C.c_int(0)
+        check(lib().swec_locate_sketch_damage(self._h, ptrs, shard_len, radius, pages, n_pages, C.byref(n), per_shard,
+                                              C.byref(ok)))
+        return {"ok": bool(ok.value), "n_flagged": int(n.value),
+                "pages": [(int(p.page), int(p.blamed_mask), bool(p.uncorrectable)) for p in pages[:n.value]],
+                "shard_pages": {i: int(per_shard[i]) for i in range(MaxShardCount) if per_shard[i]}}
+
     def synchronize(self, stream: int = 0) -> None:
         check(lib().swec_stream_synchronize(self._h, stream))
 
@@ -342,6 +379,21 @@ def verify_ec_files(base_file_name: str, additional_dirs: list[str] | None = Non
     check(lib().swec_verify_ec_files(base_file_name.encode(), arr, len(dirs), k, m, dev, bad, C.byref(ok)))
     nm = ctx.ParityShards if ctx else ParityShardsCount
     return bool(ok.value), list(bad[:nm])
+
+
+def page_sketch_file(path: str, seed: int, device: int = 0) -> tuple[np.ndarray, int]:
+    """The page sketches of one shard file (swec_page_sketch_file): (uint64 array of ceil(len / 4096) words, len).  The
+    file is only read; "file_direct_io" bit 0 reads it with O_DIRECT."""
+    import os
+    cap = (os.stat(path).st_size + 4095) // 4096
+    while True:
+        out = np.zeros(max(1, cap), dtype=np.uint64)
+        shard_len, n = C.c_int64(0), C.c_int64(0)
+        check(lib().swec_page_sketch_file(path.encode(), device, seed, out.ctypes.data, cap, C.byref(shard_len),
+                                          C.byref(n)))
+        if n.value <= cap:   # else the file grew since the stat: again with room for every page
+            return out[:n.value], int(shard_len.value)
+        cap = n.value
 
 
 def _damage_result(report, ranges, n_ranges: int, max_ranges: int) -> dict:
