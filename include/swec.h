@@ -25,6 +25,9 @@
  *   swec_page_sketch_file,      (no counterpart) ScrubEcVolume FULL checks only needle CRCs over the network
  *   swec_locate_sketch_damage   (weed/storage/store_ec_scrub.go); these check parity of a balanced volume from
  *                               8 bytes per 4 KiB page of every shard
+ *   swec_locate_sketch_damage_checked  ec.rebuild of a balanced volume (weed/shell/command_ec_rebuild.go) copies every
+ *                               present shard to one rebuilder; this locates their damage from sketches first, with
+ *                               the lost shards as erasures, and predicts the sketch of every rebuilt shard
  *   swec_reconstruct_batch      batched ReconstructData   weed/storage/store_ec.go:482-560 (one call per interval today)
  *   swec_write_dat_file         WriteDatFile              weed/storage/erasure_coding/ec_decoder.go:176-223
  *   swec_ec_shards_generate     VolumeEcShardsGenerate (file work)   weed/server/volume_grpc_erasure_coding.go:43-146
@@ -469,6 +472,32 @@ typedef struct swec_sketch_page {
 int swec_locate_sketch_damage(swec_encoder *enc, const uint64_t *const *sketches, int64_t shard_len, int radius,
                               swec_sketch_page *pages, int64_t pages_cap, int64_t *n_flagged,
                               uint64_t *shard_pages, int *ok);
+/* swec_locate_sketch_damage for a set with lost shards: errors and erasures over the sketches, as the checked rebuild
+ * decodes the shards.  sketches[i] == NULL marks a lost shard.  The first k present shards are the information set and
+ * the other c = (present shards) - k are its check shards; the radius used is t = min(radius, floor(c/2)), radius 0, 1
+ * or 2 (no 2·radius <= m rule).  The check sketches recomputed from the information sketches are compared with the
+ * stored ones, and every page with a non-zero sketch syndrome is decoded column by column and merged per page, with
+ * positions mapped back to shard ids; a lost shard is never blamed.
+ *   - The guarantee is the per-page one of swec_locate_sketch_damage with m replaced by c: for the set D of present
+ *     shards that differ from the codeword on a page, |D| <= t blames exactly D, t < |D| <= c-t makes the page
+ *     uncorrectable, and beyond that the page is flagged but its blame can be wrong.  Each statement fails only with
+ *     probability <= |D|·2^-64 over the seed.  Radius 0 flags every damaged page as uncorrectable.
+ *   - pages, pages_cap, *n_flagged and shard_pages are those of swec_locate_sketch_damage.  *ok = 1 iff c >= 1 and no
+ *     page is flagged.  c = 0 (exactly k present): nothing can be checked, *n_flagged = 0 and *ok = 0.
+ *   - rebuilt_sketches (may be NULL): k+m pointers, of which the entries of present shards are ignored and a lost
+ *     shard's may be NULL.  A non-NULL entry of lost shard r receives its ceil(shard_len/4096) words, R[r]·(information
+ *     sketches) with R = G[lost]·G[I]^-1: on unflagged pages and pages blamed within the radius, with the located errors
+ *     of information shards taken out, so the sketch of the TRUE shard r; on uncorrectable pages, of the information
+ *     sketches as found, so the sketch of what swec_rebuild_ec_files writes there (no partial correction).  With c = 0
+ *     they are plain R·(information sketches).  Sketch the rebuilt shard with the same seed and compare outside the
+ *     uncorrectable pages: this checks the rebuild against the other holders' data, not the rebuilder's.
+ *   - With every sketch present and 2·radius <= m, the result is that of swec_locate_sketch_damage.
+ * Errors, all before any device work: SWEC_ERR_INVALID_ARG (NULL enc, sketches, n_flagged or ok, negative shard_len or
+ * pages_cap, pages NULL with pages_cap > 0, a radius other than 0, 1 or 2); then SWEC_ERR_TOO_FEW_SHARDS for fewer
+ * than k sketches; then SWEC_ERR_NO_DEVICE for an encoder without a device.  Synchronous.                          */
+int swec_locate_sketch_damage_checked(swec_encoder *enc, const uint64_t *const *sketches, int64_t shard_len,
+                                      int radius, swec_sketch_page *pages, int64_t pages_cap, int64_t *n_flagged,
+                                      uint64_t *shard_pages, uint64_t *const *rebuilt_sketches, int *ok);
 /* ---- checked decode: errors and erasures before the parity is dropped -----------------------------------------------
  * ec.decode deletes every shard, parity included, once the .dat is written (weed/shell/command_ec_decode.go:156-181),
  * so it is the last point at which damage in the data shards can be corrected.  swec_write_dat_file copies the data

@@ -642,6 +642,67 @@ func swecLocateSketchDamage(enc *swecEncoder, sketches [][]uint64, shardSizes []
 	return pages, nil
 }
 
+// swecLocateSketchDamageChecked is swecLocateSketchDamage for a volume with lost shards (a nil sketch; its shardSizes
+// entry is ignored), before ec.rebuild.  The first k present shards are checked against the other c present ones at
+// radius min(1, c/2); with c = 0 nothing is checked and no page comes back.  Repair the blamed pages at their holders
+// first (a page blamed on B has k present shards outside B), then rebuild.  rebuilt[id] is the sketch lost shard id must
+// have afterwards: sketch the rebuilt file with the same seed and compare it outside the Uncorrectable pages, where the
+// prediction is what the plain rebuild writes from the shards as found (INTEGRATION.md).
+func swecLocateSketchDamageChecked(enc *swecEncoder, sketches [][]uint64, shardSizes []int64) (pages []swecSketchPage, rebuilt map[int][]uint64, err error) {
+	size := int64(-1)
+	for i, s := range sketches {
+		if s == nil {
+			continue
+		}
+		if size < 0 {
+			size = shardSizes[i]
+		} else if shardSizes[i] != size {
+			return nil, nil, fmt.Errorf("ec shard size expected %d actual %d", size, shardSizes[i])
+		}
+	}
+	if size < 0 {
+		size = 0 // no shard present: the call reports too few shards
+	}
+	nPages := (size + 4095) / 4096
+	var p runtime.Pinner
+	defer p.Unpin()
+	ptrs := (*[C.SWEC_MAX_SHARDS]*C.uint64_t)(C.calloc(C.SWEC_MAX_SHARDS, C.size_t(unsafe.Sizeof(uintptr(0)))))
+	defer C.free(unsafe.Pointer(ptrs))
+	outs := (*[C.SWEC_MAX_SHARDS]*C.uint64_t)(C.calloc(C.SWEC_MAX_SHARDS, C.size_t(unsafe.Sizeof(uintptr(0)))))
+	defer C.free(unsafe.Pointer(outs))
+	rebuilt = map[int][]uint64{}
+	for i, s := range sketches {
+		if s == nil {
+			r := make([]uint64, nPages+1) // +1: never a zero-length slice to take the address of
+			p.Pin(&r[0])
+			outs[i] = (*C.uint64_t)(unsafe.Pointer(&r[0]))
+			rebuilt[i] = r[:nPages]
+			continue
+		}
+		if int64(len(s)) != nPages {
+			return nil, nil, fmt.Errorf("ec shard %d: %d sketches for %d pages", i, len(s), nPages)
+		}
+		if nPages == 0 {
+			s = make([]uint64, 1) // present, with no pages: NULL would mark it lost
+		}
+		p.Pin(&s[0])
+		ptrs[i] = (*C.uint64_t)(unsafe.Pointer(&s[0]))
+	}
+	out := make([]C.swec_sketch_page, nPages+1)
+	var nFlagged C.int64_t
+	var ok C.int
+	if err := swecCall(func() C.int {
+		return C.swec_locate_sketch_damage_checked(enc.h, &ptrs[0], C.int64_t(size), 1, &out[0], C.int64_t(nPages),
+			&nFlagged, nil, &outs[0], &ok)
+	}); err != nil {
+		return nil, nil, fmt.Errorf("locate sketch damage (checked): %w", err)
+	}
+	for _, q := range out[:nFlagged] {
+		pages = append(pages, swecSketchPage{int64(q.page), uint32(q.blamed_mask), q.uncorrectable != 0})
+	}
+	return pages, rebuilt, nil
+}
+
 // swecRepairEcDamage is swecLocateEcDamage, which also corrects the located bytes in the shard files: only the damaged
 // pages of the damaged shards are rewritten, so scattered bit rot in more than ParityShards shards is still repaired,
 // where deleting and rebuilding that many shards is impossible.  repaired are the shards written; details say where.

@@ -148,6 +148,9 @@ PROTOTYPES = {
                                         C.POINTER(C.c_int64)]),
     "swec_locate_sketch_damage": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.POINTER(SketchPage),
                                             C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_uint64), C.POINTER(C.c_int)]),
+    "swec_locate_sketch_damage_checked": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.POINTER(SketchPage),
+                                                    C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_uint64), C.c_void_p,
+                                                    C.POINTER(C.c_int)]),
     "swec_write_dat_file": (C.c_int, [C.c_char_p, C.c_int64, C.c_void_p, C.c_int, C.c_int64, C.c_int64]),
     "swec_write_dat_file_checked": (C.c_int, [C.c_char_p, C.c_int64, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_int64,
                                               C.c_int, C.c_int, C.POINTER(DamageReport), C.POINTER(DamageRange), C.c_int,

@@ -6,9 +6,10 @@
 //                             ⊕_b 2^b ⊗ T_b (Horner over b with a multiply-by-2 on all 8 bytes at once), and the warp
 //                             XORs its 32 shares with shuffles.  A whole page of an aligned shard is read as 8 coalesced
 //                             16-byte loads per lane; the partial last page and unaligned shards go byte by byte.
-//   swec_sketch_pages_kernel  the page decode of swec_locate_sketch_damage: one thread per page, the 8 bytes of its
-//                             sketch syndromes decoded as 8 columns by the locate kernels' decoder (locate_decode.cuh),
-//                             and their blame merged per page.
+//   swec_sketch_pages_kernel  the page decode of both sketch calls, over the errors-and-erasures plan of the present
+//                             shards (damage.h): one thread per page, the 8 bytes of its sketch syndromes decoded as 8
+//                             columns by the locate kernels' decoder (locate_decode.cuh), their blame merged per page,
+//                             and the located errors of information shards taken out of the lost shards' sketches.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -16,6 +17,7 @@
 #include <string>
 #include <vector>
 
+#include "damage.h"
 #include "device_common.cuh"
 #include "engine.h"
 #include "locate_decode.cuh"
@@ -81,100 +83,197 @@ __global__ void __launch_bounds__(256) swec_page_sketch_kernel(const u8* __restr
     }
 }
 
+constexpr u8 kLogZero = 0xff;  // log R entry of a zero coefficient (logs of non-zero bytes are < 255)
+constexpr int kLogRWords = 32 * 32 / 4;  // log R[r][j] at byte r*32 + j, after the LocateTables
+
 struct SketchPageParams {
-    const u64* comp[SWEC_MAX_SHARDS];    // parity sketches recomputed from the data sketches
-    const u64* stored[SWEC_MAX_SHARDS];  // parity sketches as the parity shards' holders sent them
+    const u64* comp[SWEC_MAX_SHARDS];    // check sketches recomputed from the information sketches
+    const u64* stored[SWEC_MAX_SHARDS];  // check sketches as their holders sent them
+    u64* rebuilt[SWEC_MAX_SHARDS];       // R·(information sketches) of every lost shard, corrected in place
+    u8 ids[SWEC_MAX_SHARDS];             // shard id of every position: information 0..k-1, checks k..k+c-1
     u64 pages;
-    int k, m, radius;
-    const u32* tables;            // LocateTables
-    swec_sketch_page* flagged;    // one entry per flagged page, in no particular order
-    unsigned long long* count;    // entries written
+    int k, c, f, radius;                 // information, check and lost shards; the radius, at most c/2
+    const u32* tables;                   // LocateTables of the check rows P', then log R (f > 0)
+    swec_sketch_page* flagged;           // one entry per flagged page, in no particular order
+    unsigned long long* count;           // entries written
 };
 
-// Page decode, one thread per page, grid-stride.  Byte l of the m sketch syndromes of page g is the syndrome of sketch
+// R[r][j]·e, the image in lost shard r of error value e at information position j (0 for any other position)
+__device__ __forceinline__ u8 carried(const LocateTables& t, const u8* logr, int r, u32 j, u8 e, int k) {
+    if (j >= u32(k) || !e) return 0;
+    const u8 lr = logr[r * 32 + int(j)];
+    return lr == kLogZero ? 0 : t.exp[lr + t.log[e]];
+}
+
+// Page decode, one thread per page, grid-stride.  Byte l of the c sketch syndromes of page g is the syndrome of sketch
 // column (g, l): each non-zero column is decoded as the locate kernel decodes a byte column, and the page is blamed on
 // the union of its columns' blame, or uncorrectable when a column is or the union exceeds the radius.  Radius 0
-// decodes nothing.  Clean pages cost the loads.
+// decodes nothing.  The positions and error values of the 8 columns are kept a byte each in four words, and only a
+// page decoded within the radius XORs the images of its information errors into byte l of every lost shard's sketch
+// word; an uncorrectable page keeps R·(information sketches as found).  Clean pages cost the loads.
 __global__ void __launch_bounds__(256) swec_sketch_pages_kernel(const __grid_constant__ SketchPageParams p) {
-    __shared__ __align__(16) u32 words[kTableWords];
-    for (int i = threadIdx.x; i < kTableWords; i += blockDim.x) words[i] = p.tables[i];
+    __shared__ __align__(16) u32 words[kTableWords + kLogRWords];
+    const int n_words = kTableWords + (p.f > 0 ? kLogRWords : 0);
+    for (int i = threadIdx.x; i < n_words; i += blockDim.x) words[i] = p.tables[i];
     __syncthreads();
     const LocateTables& t = *reinterpret_cast<const LocateTables*>(words);
+    const u8* logr = reinterpret_cast<const u8*>(words + kTableWords);
     const u64 stride = (u64)gridDim.x * blockDim.x;
     for (u64 g = (u64)blockIdx.x * blockDim.x + threadIdx.x; g < p.pages; g += stride) {
         u64 any = 0;
-        for (int i = 0; i < p.m; i++) any |= p.comp[i][g] ^ p.stored[i][g];
+        for (int i = 0; i < p.c; i++) any |= p.comp[i][g] ^ p.stored[i][g];
         if (!any) continue;
-        u32 mask = 0;
+        u32 mask = 0;                      // blamed positions
         bool bad = false;
+        u64 pa = ~0ull, pb = ~0ull;        // byte l: the positions column l is blamed on, 0xff for none
+        u64 va = 0, vb = 0;                // byte l: their error values
         for (int l = 0; l < 8 && !bad; l++) {
             u8 s[SWEC_MAX_SHARDS];
             u8 nz = 0;
-            for (int i = 0; i < p.m; i++) {
+            for (int i = 0; i < p.c; i++) {
                 s[i] = u8((p.comp[i][g] ^ p.stored[i][g]) >> (8 * l));
                 nz |= s[i];
             }
             if (!nz) continue;
             int a = -1, b = -1;
             u8 ea = 0, eb = 0;
-            const int found = p.radius == 0 ? 0 : decode_column<false>(t, s, p.k, p.m, p.radius, &a, &b, &ea, &eb);
+            const int found = p.radius == 0 ? 0 : decode_column<true>(t, s, p.k, p.c, p.radius, &a, &b, &ea, &eb);
             bad = !found;
-            if (found >= 1) mask |= 1u << a;
-            if (found == 2) mask |= 1u << b;
+            if (found >= 1) {
+                mask |= 1u << a;
+                pa ^= u64(0xff ^ a) << (8 * l);
+                va |= u64(ea) << (8 * l);
+            }
+            if (found == 2) {
+                mask |= 1u << b;
+                pb ^= u64(0xff ^ b) << (8 * l);
+                vb |= u64(eb) << (8 * l);
+            }
         }
         bad = bad || __popc(mask) > p.radius;
+        u32 blamed = 0;  // the shard ids of the blamed positions
+        for (u32 x = bad ? 0u : mask; x; x &= x - 1) blamed |= 1u << p.ids[__ffs(x) - 1];
         const unsigned long long at = atomicAdd(p.count, 1ull);
         p.flagged[at].page = int64_t(g);
-        p.flagged[at].blamed_mask = bad ? 0u : mask;
+        p.flagged[at].blamed_mask = blamed;
         p.flagged[at].uncorrectable = bad ? 1 : 0;
+        if (bad) continue;
+        for (int r = 0; r < p.f; r++) {
+            u64 fix = 0;
+            for (int l = 0; l < 8; l++) {
+                const int sh = 8 * l;
+                const u8 x = carried(t, logr, r, u32(pa >> sh) & 0xff, u8(va >> sh), p.k) ^
+                             carried(t, logr, r, u32(pb >> sh) & 0xff, u8(vb >> sh), p.k);
+                fix |= u64(x) << sh;
+            }
+            p.rebuilt[r][g] ^= fix;
+        }
     }
 }
 
-// The page decode: comp[p] and stored[p] are the recomputed and the stored sketches of parity shard p, `pages` words
-// each, in device memory.  Every page whose syndrome is not zero goes into *flagged, in ascending page order.
-// Synchronises `s`.
-int locate_sketch_pages(const Matrix& parity, const uint8_t* const* comp, const uint8_t* const* stored, int64_t pages,
-                        int radius, cudaStream_t s, std::vector<swec_sketch_page>* flagged) {
-    LocateTables t;
-    locate_tables(parity, &t);
-    DeviceBuffer tables;
-    SWEC_CUDA(tables.upload(&t, 1, s));
-    StreamScratch out(s);
-    SWEC_CUDA(out.alloc(sizeof(unsigned long long) + size_t(pages) * sizeof(swec_sketch_page)));
-    SketchPageParams p;
-    memset(&p, 0, sizeof p);
-    for (int i = 0; i < parity.rows; i++) {
-        p.comp[i] = reinterpret_cast<const u64*>(comp[i]);
-        p.stored[i] = reinterpret_cast<const u64*>(stored[i]);
+// Both sketch calls: sketches[id] are the host sketches of the present shards (n_pages words each), decoded over
+// `plan` at radius t <= c/2.  One apply of plan.fused to the uploaded information sketches gives the check sketches
+// and R·(information sketches) of every lost shard; the page decode (c >= 1) compares the check sketches with the
+// stored ones and corrects the lost shards' sketches.  The flagged pages come back in ascending page order, and the
+// sketch of lost shard id into out[id] where out and out[id] are non-NULL.  Synchronous on the encoder's stream.
+int sketch_pages(swec_encoder* e, const CheckedPlan& plan, const uint64_t* const* sketches, int64_t n_pages, int t,
+                 uint64_t* const* out, std::vector<swec_sketch_page>* flagged) {
+    const int k = e->k, c = plan.c(), nout = int(plan.outs.size()), f = int(plan.rebuilt_rows.size());
+    flagged->clear();
+    if (n_pages == 0) return SWEC_OK;
+    cudaStream_t s = e->stream;
+    const size_t bytes = size_t(n_pages) * 8, pitch = (bytes + 15) & ~size_t(15);  // 16-byte rows: the vector path
+    // the k information and c check sketches as uploaded, then the nout rows the apply computes
+    StreamScratch buf(s);
+    SWEC_CUDA(buf.alloc(size_t(k + c + nout) * pitch));
+    auto row = [&](int i) { return buf.as<uint8_t>() + size_t(i) * pitch; };
+    uint8_t* at[SWEC_MAX_SHARDS];
+    uint8_t* comp[SWEC_MAX_SHARDS];
+    for (int i = 0; i < k + c; i++) {
+        at[i] = row(i);
+        SWEC_CUDA(cudaMemcpyAsync(at[i], sketches[i < k ? plan.info[size_t(i)] : plan.check(i - k)], bytes,
+                                  cudaMemcpyHostToDevice, s));
     }
-    p.pages = u64(pages);
-    p.k = parity.cols;
-    p.m = parity.rows;
-    p.radius = radius;
-    p.tables = tables.as<u32>();
-    p.count = out.as<unsigned long long>();
-    p.flagged = reinterpret_cast<swec_sketch_page*>(p.count + 1);
-    SWEC_CUDA(cudaMemsetAsync(p.count, 0, sizeof *p.count, s));
-    static const int per_sm = [] {
-        int c = 0;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, swec_sketch_pages_kernel, 256, 0) != cudaSuccess) {
-            cudaGetLastError();
-            c = 4;
+    for (int o = 0; o < nout; o++) comp[o] = row(k + c + o);
+    // sketches are linear: the plan's rows applied to the information sketches give every other shard's clean sketch
+    if (int rc = e->apply(plan.fused, at, comp, bytes, Layout{}, s)) return rc;
+    if (c > 0) {
+        std::vector<u8> host(sizeof(LocateTables) + size_t(kLogRWords) * 4, kLogZero);
+        LocateTables& lt = *reinterpret_cast<LocateTables*>(host.data());
+        Matrix pc(c, k);
+        for (int i = 0; i < c; i++)
+            for (int j = 0; j < k; j++) pc.at(i, j) = plan.fused.at(plan.check_rows[size_t(i)], j);
+        locate_tables(pc, &lt);
+        u8* logr = host.data() + sizeof(LocateTables);
+        for (int r = 0; r < f; r++)
+            for (int j = 0; j < k; j++)
+                if (const u8 v = plan.fused.at(plan.rebuilt_rows[size_t(r)], j)) logr[r * 32 + j] = lt.log[v];
+        DeviceBuffer tables;
+        SWEC_CUDA(tables.upload(host.data(), host.size(), s));
+        StreamScratch res(s);
+        SWEC_CUDA(res.alloc(sizeof(unsigned long long) + size_t(n_pages) * sizeof(swec_sketch_page)));
+        SketchPageParams p;
+        memset(&p, 0, sizeof p);
+        for (int i = 0; i < c; i++) {
+            p.comp[i] = reinterpret_cast<const u64*>(comp[plan.check_rows[size_t(i)]]);
+            p.stored[i] = reinterpret_cast<const u64*>(at[k + i]);
+            p.ids[k + i] = u8(plan.check(i));
         }
-        return std::max(1, c);
-    }();
-    swec_sketch_pages_kernel<<<grid_for(u64(pages), 256, per_sm), 256, 0, s>>>(p);
-    SWEC_CUDA(launched());
-    unsigned long long n = 0;
-    SWEC_CUDA(cudaMemcpyAsync(&n, p.count, sizeof n, cudaMemcpyDeviceToHost, s));
-    SWEC_CUDA(cudaStreamSynchronize(s));
-    flagged->resize(size_t(n));
-    if (n) {
-        SWEC_CUDA(cudaMemcpyAsync(flagged->data(), p.flagged, size_t(n) * sizeof(swec_sketch_page), cudaMemcpyDeviceToHost, s));
+        for (int j = 0; j < k; j++) p.ids[j] = u8(plan.info[size_t(j)]);
+        for (int r = 0; r < f; r++) p.rebuilt[r] = reinterpret_cast<u64*>(comp[plan.rebuilt_rows[size_t(r)]]);
+        p.pages = u64(n_pages);
+        p.k = k;
+        p.c = c;
+        p.f = f;
+        p.radius = t;
+        p.tables = tables.as<u32>();
+        p.count = res.as<unsigned long long>();
+        p.flagged = reinterpret_cast<swec_sketch_page*>(p.count + 1);
+        SWEC_CUDA(cudaMemsetAsync(p.count, 0, sizeof *p.count, s));
+        static const int per_sm = [] {
+            int n = 0;
+            if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, swec_sketch_pages_kernel, 256, 0) != cudaSuccess) {
+                cudaGetLastError();
+                n = 4;
+            }
+            return std::max(1, n);
+        }();
+        swec_sketch_pages_kernel<<<grid_for(u64(n_pages), 256, per_sm), 256, 0, s>>>(p);
+        SWEC_CUDA(launched());
+        unsigned long long n = 0;
+        SWEC_CUDA(cudaMemcpyAsync(&n, p.count, sizeof n, cudaMemcpyDeviceToHost, s));
         SWEC_CUDA(cudaStreamSynchronize(s));
+        flagged->resize(size_t(n));
+        if (n)
+            SWEC_CUDA(cudaMemcpyAsync(flagged->data(), p.flagged, size_t(n) * sizeof(swec_sketch_page),
+                                      cudaMemcpyDeviceToHost, s));
     }
+    for (int r = 0; r < f && out; r++)
+        if (uint64_t* dst = out[plan.rebuilt(r)])
+            SWEC_CUDA(cudaMemcpyAsync(dst, comp[plan.rebuilt_rows[size_t(r)]], bytes, cudaMemcpyDeviceToHost, s));
+    SWEC_CUDA(cudaStreamSynchronize(s));
     std::sort(flagged->begin(), flagged->end(),
               [](const swec_sketch_page& a, const swec_sketch_page& b) { return a.page < b.page; });
+    return SWEC_OK;
+}
+
+// The tail of both sketch calls, after their argument rules: the decode over `plan`, then the caller's outputs.
+int locate_sketches(swec_encoder* e, const CheckedPlan& plan, const uint64_t* const* sketches, int64_t shard_len,
+                    int radius, swec_sketch_page* pages, int64_t pages_cap, int64_t* n_flagged, uint64_t* shard_pages,
+                    uint64_t* const* rebuilt, int* ok) {
+    std::lock_guard<std::mutex> lock(e->mu);
+    if (int rc = e->ensure_device()) return rc;
+    const int64_t n_pages = (shard_len + int64_t(kPage) - 1) / int64_t(kPage);
+    std::vector<swec_sketch_page> flagged;
+    // the punctured code has distance c+1: radius t needs 2t <= c
+    if (int rc = sketch_pages(e, plan, sketches, n_pages, std::min(radius, plan.c() / 2), rebuilt, &flagged)) return rc;
+    if (shard_pages) memset(shard_pages, 0, SWEC_MAX_SHARDS * sizeof *shard_pages);
+    for (size_t i = 0; i < flagged.size(); i++) {
+        if (int64_t(i) < pages_cap) pages[i] = flagged[i];
+        for (uint32_t b = flagged[i].blamed_mask; b && shard_pages; b &= b - 1) shard_pages[__builtin_ctz(b)]++;
+    }
+    *n_flagged = int64_t(flagged.size());
+    *ok = plan.c() >= 1 && flagged.empty() ? 1 : 0;
     return SWEC_OK;
 }
 
@@ -230,36 +329,28 @@ int swec_locate_sketch_damage(swec_encoder* e, const uint64_t* const* sketches, 
     for (int i = 0; i < k + m; i++)
         if (!sketches[i])
             return fail(SWEC_ERR_TOO_FEW_SHARDS, "no sketch of shard " + std::to_string(i) + ": rebuild it first");
-    std::lock_guard<std::mutex> lock(e->mu);
-    int rc = e->ensure_device();
-    if (rc) return rc;
-    cudaStream_t s = e->stream;
-    const int64_t n_pages = (shard_len + int64_t(kPage) - 1) / int64_t(kPage);
-    const size_t bytes = size_t(n_pages) * 8;
-    std::vector<swec_sketch_page> flagged;
-    if (n_pages > 0) {
-        // the k+m sketches as uploaded, then the m recomputed parity sketches
-        StreamScratch buf(s);
-        SWEC_CUDA(buf.alloc(size_t(k + 2 * m) * bytes));
-        uint8_t* at[SWEC_MAX_SHARDS];
-        uint8_t* comp[SWEC_MAX_SHARDS];
-        for (int i = 0; i < k + m; i++) {
-            at[i] = buf.as<uint8_t>() + size_t(i) * bytes;
-            SWEC_CUDA(cudaMemcpyAsync(at[i], sketches[i], bytes, cudaMemcpyHostToDevice, s));
-        }
-        for (int p = 0; p < m; p++) comp[p] = buf.as<uint8_t>() + size_t(k + m + p) * bytes;
-        // sketches are linear: the parity rows applied to the data sketches give the clean parity sketches
-        if ((rc = e->apply(parity_rows(e), at, comp, bytes, Layout{}, s))) return rc;
-        if ((rc = locate_sketch_pages(parity_rows(e), comp, at + k, n_pages, radius, s, &flagged))) return rc;
-    }
-    if (shard_pages) memset(shard_pages, 0, SWEC_MAX_SHARDS * sizeof *shard_pages);
-    for (size_t i = 0; i < flagged.size(); i++) {
-        if (int64_t(i) < pages_cap) pages[i] = flagged[i];
-        for (uint32_t b = flagged[i].blamed_mask; b && shard_pages; b &= b - 1) shard_pages[__builtin_ctz(b)]++;
-    }
-    *n_flagged = int64_t(flagged.size());
-    *ok = flagged.empty() ? 1 : 0;
-    return SWEC_OK;
+    // every shard present: the data shards are the information set, fused is the parity rows, the checks are parity
+    const std::vector<uint8_t> all(size_t(k + m), 1);
+    CheckedPlan plan;
+    plan.build(e->gen, k, all.data(), false);
+    return locate_sketches(e, plan, sketches, shard_len, radius, pages, pages_cap, n_flagged, shard_pages, nullptr, ok);
+}
+
+int swec_locate_sketch_damage_checked(swec_encoder* e, const uint64_t* const* sketches, int64_t shard_len, int radius,
+                                      swec_sketch_page* pages, int64_t pages_cap, int64_t* n_flagged,
+                                      uint64_t* shard_pages, uint64_t* const* rebuilt_sketches, int* ok) {
+    if (!e || !sketches || !n_flagged || !ok) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
+    if (shard_len < 0) return fail(SWEC_ERR_INVALID_ARG, "shard_len must be >= 0");
+    if (pages_cap < 0 || (pages_cap > 0 && !pages))
+        return fail(SWEC_ERR_INVALID_ARG, "pages_cap must be >= 0, and pages non-NULL when it is > 0");
+    if (radius < 0 || radius > 2) return fail(SWEC_ERR_INVALID_ARG, "radius must be 0, 1 or 2");
+    std::vector<uint8_t> present(size_t(e->k + e->m));
+    for (size_t i = 0; i < present.size(); i++) present[i] = sketches[i] != nullptr;
+    CheckedPlan plan;
+    if (!plan.build(e->gen, e->k, present.data(), false))
+        return fail(SWEC_ERR_TOO_FEW_SHARDS, "fewer than data_shards sketches present");
+    return locate_sketches(e, plan, sketches, shard_len, radius, pages, pages_cap, n_flagged, shard_pages,
+                           rebuilt_sketches, ok);
 }
 
 }  // extern "C"

@@ -251,6 +251,39 @@ class Encoder:
         shard_len: the shard length, or the k+m lengths the holders reported, which must be equal (ErrShardSize).
         Returns ok, "pages" = [(page, blamed shard mask, uncorrectable)] in ascending page order, "n_flagged" and
         "shard_pages" = {shard id: pages blamed on it}.  The result is per page, not per column (include/swec.h)."""
+        shard_len, n_pages, ptrs, _ = self._sketch_args(sketches, shard_len)
+        pages = (SketchPage * max(1, n_pages))()
+        n, per_shard, ok = C.c_int64(0), (C.c_uint64 * MaxShardCount)(), C.c_int(0)
+        check(lib().swec_locate_sketch_damage(self._h, ptrs, shard_len, radius, pages, n_pages, C.byref(n), per_shard,
+                                              C.byref(ok)))
+        return _sketch_result(ok, n, pages, per_shard)
+
+    def locate_sketch_damage_checked(self, sketches, shard_len, radius: int = 1) -> dict:
+        """locate_sketch_damage for a set with lost shards (swec_locate_sketch_damage_checked): None marks a lost shard,
+        and the first k present shards are checked against the other c present ones at radius min(radius, c // 2).
+        shard_len: as for locate_sketch_damage, the lengths the present shards' holders reported (None entries are
+        skipped).  Returns the keys of locate_sketch_damage, plus "checks" = c and "rebuilt" = {lost shard id: uint64
+        array}, the sketch that shard must have once rebuilt: of the true shard outside uncorrectable pages, and of what
+        the plain rebuild writes on them.  With c = 0 nothing is checked and "ok" is False (include/swec.h)."""
+        if not isinstance(shard_len, int):
+            shard_len = [n for n in shard_len if n is not None]
+        shard_len, n_pages, ptrs, keep = self._sketch_args(sketches, shard_len)
+        present = sum(s is not None for s in keep)
+        rebuilt = {i: np.zeros(n_pages, dtype=np.uint64) for i, s in enumerate(keep) if s is None}
+        outs = (C.c_void_p * self.total_shards)(*[rebuilt[i].ctypes.data if i in rebuilt else None
+                                                  for i in range(self.total_shards)])
+        pages = (SketchPage * max(1, n_pages))()
+        n, per_shard, ok = C.c_int64(0), (C.c_uint64 * MaxShardCount)(), C.c_int(0)
+        check(lib().swec_locate_sketch_damage_checked(self._h, ptrs, shard_len, radius, pages, n_pages, C.byref(n),
+                                                      per_shard, outs, C.byref(ok)))
+        res = _sketch_result(ok, n, pages, per_shard)
+        res["checks"] = max(0, present - self.data_shards)
+        res["rebuilt"] = rebuilt
+        return res
+
+    def _sketch_args(self, sketches, shard_len):
+        """(shard_len, pages, pointer array, arrays kept alive) of the sketch calls; shard_len may be a list of equal
+        lengths (ErrShardSize otherwise)."""
         if not isinstance(shard_len, int):
             lengths = {int(n) for n in shard_len}
             if len(lengths) != 1:
@@ -266,14 +299,7 @@ class Encoder:
                 if s.shape != (n_pages,):
                     raise SwecError(-1, f"a sketch array must hold {n_pages} words, got {s.shape}")
             keep.append(s)
-        ptrs = _ptrs(keep)
-        pages = (SketchPage * max(1, n_pages))()
-        n, per_shard, ok = C.c_int64(0), (C.c_uint64 * MaxShardCount)(), C.c_int(0)
-        check(lib().swec_locate_sketch_damage(self._h, ptrs, shard_len, radius, pages, n_pages, C.byref(n), per_shard,
-                                              C.byref(ok)))
-        return {"ok": bool(ok.value), "n_flagged": int(n.value),
-                "pages": [(int(p.page), int(p.blamed_mask), bool(p.uncorrectable)) for p in pages[:n.value]],
-                "shard_pages": {i: int(per_shard[i]) for i in range(MaxShardCount) if per_shard[i]}}
+        return shard_len, n_pages, _ptrs(keep), keep
 
     def synchronize(self, stream: int = 0) -> None:
         check(lib().swec_stream_synchronize(self._h, stream))
@@ -394,6 +420,12 @@ def page_sketch_file(path: str, seed: int, device: int = 0) -> tuple[np.ndarray,
         if n.value <= cap:   # else the file grew since the stat: again with room for every page
             return out[:n.value], int(shard_len.value)
         cap = n.value
+
+
+def _sketch_result(ok, n, pages, per_shard) -> dict:
+    return {"ok": bool(ok.value), "n_flagged": int(n.value),
+            "pages": [(int(p.page), int(p.blamed_mask), bool(p.uncorrectable)) for p in pages[:n.value]],
+            "shard_pages": {i: int(per_shard[i]) for i in range(MaxShardCount) if per_shard[i]}}
 
 
 def _damage_result(report, ranges, n_ranges: int, max_ranges: int) -> dict:
