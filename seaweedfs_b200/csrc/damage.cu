@@ -50,14 +50,13 @@ namespace {
 constexpr int kSets = SWEC_MAX_SHARDS + 1;  // one counter set per shard, and one for uncorrectable columns (set k+m)
 constexpr int kCounters = 3 * kSets + 1;    // bytes[kSets], first[kSets], last[kSets], damaged columns
 constexpr int kPageShift = 12;              // 4 KiB pages
-constexpr u8 kLogZero = 0xff;               // log R entry of a zero coefficient (logs of non-zero bytes are < 255)
 
 enum : int { kLocate = 0, kCorrect = 1, kRebuild = 2, kDecode = 3 };  // the instantiations of swec_locate_kernel
 
 
 // kRebuild and kDecode only, in shared memory of its own so that the other instantiations copy no more than before
 struct RebuildTables {
-    u8 logr[32 * 32];  // log R[r][j] at r*32 + j, kLogZero for a zero entry
+    u8 logr[kLogRBytes];  // CheckedPlan::rebuilt_logs
 };
 constexpr int kRebuildWords = int(sizeof(RebuildTables) / 4);
 
@@ -295,31 +294,27 @@ void launch_locate(int m, const LocateParams& p, u64 n, cudaStream_t s) {
 
 }  // namespace
 
-int check_locate_args(int m, int radius, const swec_damage_report* report, const swec_damage_range* ranges,
-                      int ranges_cap) {
+int DamageOut::check() const {
     if (!report) return fail(SWEC_ERR_INVALID_ARG, "report is NULL");
-    if (ranges_cap < 0 || (ranges_cap > 0 && !ranges))
+    if (cap < 0 || (cap > 0 && !ranges))
         return fail(SWEC_ERR_INVALID_ARG, "ranges_cap must be >= 0, and ranges non-NULL when it is > 0");
-    if (radius != 1 && radius != 2) return fail(SWEC_ERR_INVALID_ARG, "radius must be 1 or 2");
-    if (m < 2 * radius)
-        return fail(SWEC_ERR_INVALID_ARG, "radius " + std::to_string(radius) + " needs at least " +
-                                              std::to_string(2 * radius) + " parity shards, the code has " + std::to_string(m));
     return SWEC_OK;
 }
 
-int check_rebuild_args(int radius, const swec_damage_report* report, const swec_damage_range* ranges, int ranges_cap) {
-    if (!report) return fail(SWEC_ERR_INVALID_ARG, "report is NULL");
-    if (ranges_cap < 0 || (ranges_cap > 0 && !ranges))
-        return fail(SWEC_ERR_INVALID_ARG, "ranges_cap must be >= 0, and ranges non-NULL when it is > 0");
-    if (radius < 0 || radius > 2) return fail(SWEC_ERR_INVALID_ARG, "radius must be 0, 1 or 2");
-    return SWEC_OK;
-}
-
-void unchecked_report(swec_damage_report* report, int* n_ranges) {
+void DamageOut::unchecked() const {
     memset(report, 0, sizeof *report);
     report->first_uncorrectable = report->last_uncorrectable = -1;
     for (int i = 0; i < SWEC_MAX_SHARDS; i++) report->shard_first[i] = report->shard_last[i] = -1;
     if (n_ranges) *n_ranges = 0;
+}
+
+int check_radius(int radius, int lowest, int m) {
+    if (radius < lowest || radius > 2)
+        return fail(SWEC_ERR_INVALID_ARG, lowest ? "radius must be 1 or 2" : "radius must be 0, 1 or 2");
+    if (m < 2 * radius)
+        return fail(SWEC_ERR_INVALID_ARG, "radius " + std::to_string(radius) + " needs at least " +
+                                              std::to_string(2 * radius) + " parity shards, the code has " + std::to_string(m));
+    return SWEC_OK;
 }
 
 bool CheckedPlan::build(const Matrix& gen, int k, const uint8_t* present, bool decode) {
@@ -345,6 +340,13 @@ bool CheckedPlan::build(const Matrix& gen, int k, const uint8_t* present, bool d
     return true;
 }
 
+CheckedPlan CheckedPlan::all_present(const Matrix& gen, int k) {
+    const std::vector<uint8_t> all(size_t(gen.rows), 1);
+    CheckedPlan plan;
+    plan.build(gen, k, all.data(), false);
+    return plan;
+}
+
 int CheckedPlan::position(int id) const {
     const int k = int(info.size()), c = this->c();
     for (int j = 0; j < k; j++)
@@ -354,6 +356,23 @@ int CheckedPlan::position(int id) const {
     for (size_t o = 0; o < outs.size(); o++)
         if (outs[o] == id) return k + c + int(o);
     return -1;
+}
+
+Matrix CheckedPlan::checks() const {
+    const int k = fused.cols;
+    Matrix pc(c(), k);
+    for (int i = 0; i < c(); i++)
+        for (int j = 0; j < k; j++) pc.at(i, j) = fused.at(check_rows[size_t(i)], j);
+    return pc;
+}
+
+void CheckedPlan::rebuilt_logs(uint8_t* logr) const {
+    u8 log[256], exp[512];
+    log_exp_tables(log, exp);
+    memset(logr, kLogZero, kLogRBytes);
+    for (size_t r = 0; r < rebuilt_rows.size(); r++)
+        for (int j = 0; j < fused.cols; j++)
+            if (const u8 v = fused.at(rebuilt_rows[r], j)) logr[r * 32 + size_t(j)] = log[v];
 }
 
 int DamageLocator::init(const Matrix& parity, int64_t shard_len, int radius, cudaStream_t s, bool correct) {
@@ -380,26 +399,15 @@ int DamageLocator::init(const Matrix& parity, int64_t shard_len, int radius, cud
 }
 
 int DamageLocator::init_rebuild(const CheckedPlan& plan, int64_t shard_len, int radius, cudaStream_t s) {
-    const Matrix& fused = plan.fused;
-    const int k = fused.cols, c = plan.c();
-    Matrix pc(c, k);
-    for (int i = 0; i < c; i++)
-        for (int j = 0; j < k; j++) pc.at(i, j) = fused.at(plan.check_rows[size_t(i)], j);
-    // the punctured code has distance c+1: radius t needs 2t <= c
-    if (int rc = init(pc, shard_len, std::min(radius, c / 2), s)) return rc;
+    if (int rc = init(plan.checks(), shard_len, plan.radius(radius), s)) return rc;
     rebuild_ = true;
     decode_ = plan.decode;
     check_rows_ = plan.check_rows;
     out_rows_ = plan.rebuilt_rows;
-    for (int j = 0; j < k; j++) ids_[size_t(j)] = plan.info[size_t(j)];
-    for (int i = 0; i < c; i++) ids_[size_t(k + i)] = plan.check(i);
-    u8 log[256], exp[512];
-    log_exp_tables(log, exp);
+    for (int j = 0; j < k_; j++) ids_[size_t(j)] = plan.info[size_t(j)];
+    for (int i = 0; i < m_; i++) ids_[size_t(k_ + i)] = plan.check(i);
     RebuildTables rt;
-    memset(&rt, kLogZero, sizeof rt);
-    for (size_t r = 0; r < out_rows_.size(); r++)
-        for (int j = 0; j < k; j++)
-            if (const u8 v = fused.at(out_rows_[r], j)) rt.logr[r * 32 + size_t(j)] = log[v];
+    plan.rebuilt_logs(rt.logr);
     SWEC_CUDA(rtables_.upload(&rt, 1, s));
     return SWEC_OK;
 }
@@ -438,14 +446,14 @@ int DamageLocator::launch(uint8_t* const* computed, uint8_t* const* shards, size
     return SWEC_OK;
 }
 
-int DamageLocator::collect(swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges,
-                           std::vector<swec_damage_range>* all) {
+int DamageLocator::collect(const DamageOut& out, std::vector<swec_damage_range>* all) {
     const int n = k_ + m_;
     std::vector<unsigned long long> c;
     std::vector<uint32_t> bits;  // n + 1 page bitmaps
     SWEC_CUDA(counters_.read(&c));
     SWEC_CUDA(pages_.read(&bits));
-    unchecked_report(report, nullptr);
+    swec_damage_report* report = out.report;
+    out.unchecked();
     report->columns = uint64_t(shard_len_);
     report->damaged_columns = c[3 * kSets];
     report->uncorrectable_columns = c[size_t(n)];
@@ -481,13 +489,13 @@ int DamageLocator::collect(swec_damage_report* report, swec_damage_range* ranges
             r.reserved = 0;
             r.offset = pg << kPageShift;
             r.length = std::min(end << kPageShift, shard_len_) - r.offset;
-            if (total < ranges_cap) ranges[total] = r;
+            if (total < out.cap) out.ranges[total] = r;
             if (all) all->push_back(r);
             total++;
             pg = end;
         }
     }
-    if (n_ranges) *n_ranges = total;
+    if (out.n_ranges) *out.n_ranges = total;
     return SWEC_OK;
 }
 

@@ -4,6 +4,8 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <algorithm>
+#include <climits>
 #include <cstddef>
 #include <cstdint>
 #include <vector>
@@ -14,15 +16,23 @@
 
 namespace swec {
 
-// The argument rules every entry point shares: radius 1 needs m >= 2 and radius 2 needs m >= 4, a report is required,
-// ranges_cap must not be negative and ranges may only be NULL when ranges_cap is 0.
-int check_locate_args(int m, int radius, const swec_damage_report* report, const swec_damage_range* ranges,
-                      int ranges_cap);
-// The checked rebuild's rules: those of check_locate_args without the parity count, and radius 0, 1 or 2 (clamped to
-// what the present shards allow by DamageLocator::init_rebuild).
-int check_rebuild_args(int radius, const swec_damage_report* report, const swec_damage_range* ranges, int ranges_cap);
-// The report of a set where nothing could be checked: no columns, no shards, no ranges (n_ranges may be NULL).
-void unchecked_report(swec_damage_report* report, int* n_ranges);
+// The report out-parameters of every damage call: the report, the first `cap` page ranges and their total.
+struct DamageOut {
+    swec_damage_report* report;
+    swec_damage_range* ranges;
+    int cap;
+    int* n_ranges;         // may be NULL
+    bool checked = false;  // the checked file calls: set once the report comes from a locator (c >= 1)
+
+    // a report is required, cap must not be negative and ranges may only be NULL when cap is 0
+    int check() const;
+    // the report of a set where nothing could be checked: no columns, no shards, no ranges
+    void unchecked() const;
+};
+
+// The radius rule: `lowest` (0 or 1) up to 2, and radius t needs 2t <= m parity shards (the default m sets no bound:
+// the checked calls clamp the radius to what their present shards allow, CheckedPlan::radius).
+int check_radius(int radius, int lowest, int m = INT_MAX);
 
 // Errors and erasures over a presence mask: the first k present shards are the information set, and one apply of
 // `fused` computes every other shard in `outs` from it; the present ones are the check shards, the missing ones are
@@ -36,12 +46,21 @@ struct CheckedPlan {
     bool decode = false;            // ec.decode: only the missing data shards are rebuilt
 
     bool build(const Matrix& gen, int k, const uint8_t* present, bool decode);  // false: fewer than k present
+    // every shard present: the data shards are the information set, fused is the parity rows, the checks are parity
+    static CheckedPlan all_present(const Matrix& gen, int k);
     int c() const { return int(check_rows.size()); }
     int check(int i) const { return outs[size_t(check_rows[size_t(i)])]; }      // shard id of check shard i
     int rebuilt(int r) const { return outs[size_t(rebuilt_rows[size_t(r)])]; }  // shard id of rebuilt shard r
     // The locator's position of shard `id`, which the file pipeline's slot streams and the device loop's shard arrays
     // share: information shard j at j, check shard i at k+i, computed row o at k+c+o; -1 for any other shard.
     int position(int id) const;
+
+    // What the locate kernel and the sketch page decode both read of the code punctured to the information and check
+    // shards, which has distance c+1:
+    Matrix checks() const;  // P', the c x k rows of `fused` that compute the check shards
+    // log R[r][j] of rebuilt row r at byte r*32 + j of kLogRBytes, kLogZero for a zero entry (locate_decode.cuh)
+    void rebuilt_logs(uint8_t* logr) const;
+    int radius(int t) const { return std::min(t, c() / 2); }  // radius t needs 2t <= c
 };
 
 // Accumulates, over any number of launches, the shards blamed for every byte column of a shard set whose syndrome
@@ -69,10 +88,9 @@ class DamageLocator {
     // their positions; only the rebuilt rows in `computed` are written, after the apply that made them.
     // Decode mode also writes shards[j] of the information shards that are data shards.
     int launch(uint8_t* const* computed, uint8_t* const* shards, size_t n, int64_t base, cudaStream_t s);
-    // After every launch has completed: the report, the page ranges (first ranges_cap of them) and their total; `all`
+    // After every launch has completed: the report, the page ranges (the first out.cap of them) and their total; `all`
     // (may be NULL) receives every range.
-    int collect(swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges,
-                std::vector<swec_damage_range>* all = nullptr);
+    int collect(const DamageOut& out, std::vector<swec_damage_range>* all = nullptr);
 
   private:
     int k_ = 0, m_ = 0, radius_ = 1;  // m_: check positions (c in rebuild mode)

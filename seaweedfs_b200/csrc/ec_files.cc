@@ -626,7 +626,7 @@ class PageWrites {
 // was found, made durable before the call returns.
 int repair_pages(swec_encoder* enc, const Matrix& rows, const std::string& b, const char* const* dirs, int ndirs,
                  const std::vector<int>& in, int64_t size, int radius, const std::vector<swec_damage_range>& runs,
-                 swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges) {
+                 const DamageOut& out) {
     const int total = int(in.size());
     PageWrites writes(runs, total);
     FdSet fds;
@@ -648,15 +648,14 @@ int repair_pages(swec_encoder* enc, const Matrix& rows, const std::string& b, co
     if ((rc = submit_flagged(pipe, runs, chunk, in, in_d, [&](Item& it) { writes.add(it); }))) return rc;
     pipe.report("repair_ec_damage");
     if ((rc = writes.sync(b))) return rc;
-    return locator.collect(report, ranges, ranges_cap, n_ranges);
+    return locator.collect(out);
 }
 
 // Pass 1 of the damage calls, swec_locate_ec_damage itself: every column of the k+m shard files `in`, all `size` bytes,
 // through a pipeline that reads the m parity shards too and runs the locator on each slot.  `runs` (may be NULL)
 // receives every page run, for pass 2.
 int locate_pass(swec_encoder* enc, const Matrix& rows, const std::vector<int>& in, int64_t size, int radius,
-                swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges,
-                std::vector<swec_damage_range>* runs) {
+                const DamageOut& out, std::vector<swec_damage_range>* runs) {
     const size_t chunk = file_chunk(size);
     DamageLocator locator;
     FilePipeline pipe(enc, rows, chunk, rows.rows, locate_step(locator));
@@ -664,20 +663,20 @@ int locate_pass(swec_encoder* enc, const Matrix& rows, const std::vector<int>& i
     if (rc) return rc;
     rc = locator.init(rows, size, radius, enc->stream);
     if (rc == SWEC_OK) rc = scrub_columns(pipe, in, size, chunk);
-    if (rc == SWEC_OK) rc = locator.collect(report, ranges, ranges_cap, n_ranges, runs);
+    if (rc == SWEC_OK) rc = locator.collect(out, runs);
     return rc;
 }  // the pipeline parks its staging ring for pass 2
 
 // swec_locate_ec_damage, and with `repair` swec_repair_ec_damage, whose pass 1 is the locate call itself: a set without
 // damage is never opened for writing.
 int damage_files(const char* base, const char* const* dirs, int ndirs, int k, int m, int device, int radius, bool repair,
-                 swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges, int* ok) {
+                 const DamageOut& out, int* ok) {
     if (!base || !ok || (ndirs > 0 && !dirs)) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
     *ok = 0;
     const std::string b(base);
     if (k == 0) ec_ratio(b, &k, &m);
-    int rc = check_locate_args(m, radius, report, ranges, ranges_cap);
-    if (rc) return rc;
+    int rc;
+    if ((rc = out.check()) || (rc = check_radius(radius, 1, m))) return rc;
     CallEncoder enc;
     if ((rc = new_call_encoder(k, m, device, &enc))) return rc;
     FdSet fds;
@@ -686,24 +685,13 @@ int damage_files(const char* base, const char* const* dirs, int ndirs, int k, in
     if ((rc = open_all_shards(b, dirs, ndirs, k + m, &fds, &in, &size))) return rc;
     const Matrix rows = parity_rows(enc.get());
     std::vector<swec_damage_range> runs;
-    if ((rc = locate_pass(enc.get(), rows, in, size, radius, report, ranges, ranges_cap, n_ranges, repair ? &runs : nullptr)))
+    if ((rc = locate_pass(enc.get(), rows, in, size, radius, out, repair ? &runs : nullptr))) return rc;
+    if (repair && out.report->damaged_columns &&
+        (rc = repair_pages(enc.get(), rows, b, dirs, ndirs, in, size, radius, runs, out)))
         return rc;
-    if (repair && report->damaged_columns &&
-        (rc = repair_pages(enc.get(), rows, b, dirs, ndirs, in, size, radius, runs, report, ranges, ranges_cap, n_ranges)))
-        return rc;
-    *ok = (repair ? report->uncorrectable_columns : report->damaged_columns) == 0 ? 1 : 0;
+    *ok = (repair ? out.report->uncorrectable_columns : out.report->damaged_columns) == 0 ? 1 : 0;
     return SWEC_OK;
 }
-
-// What the checked rebuild adds to swec_rebuild_ec_files: the radius and where the report goes.
-struct Checked {
-    int radius;
-    swec_damage_report* report;
-    swec_damage_range* ranges;
-    int ranges_cap;
-    int* n_ranges;
-    bool checked = false;  // set once the report comes from a locator (c >= 1)
-};
 
 // Submits an item whose length is set, at shard offset `col`: the caller adds what else the item needs.
 using SubmitFn = std::function<int(Item&& it, int64_t col)>;
@@ -756,7 +744,7 @@ int walk_items(const StripeGeometry& g, size_t chunk, int64_t tail_width, const 
 // the stored ones and corrects the errors it locates in the information set.  With c = 0 (exactly k shards present)
 // the set is rebuilt and the report says nothing was checked.
 int checked_pipeline(swec_encoder* enc, const CheckedPlan& plan, const std::vector<int>& in, const std::vector<int>& in_d,
-                     int64_t cols, const std::vector<int>& reserve, int64_t reserve_size, Checked* chk,
+                     int64_t cols, const std::vector<int>& reserve, int64_t reserve_size, int radius, DamageOut* chk,
                      const std::function<int(size_t chunk, const SubmitFn& submit)>& walk) {
     const int k = enc->k, c = plan.c();
     const size_t chunk = file_chunk(cols);
@@ -764,7 +752,7 @@ int checked_pipeline(swec_encoder* enc, const CheckedPlan& plan, const std::vect
     FilePipeline pipe(enc, plan.fused, chunk, c, c > 0 ? locate_step(locator) : FilePipeline::Step{});
     int rc = pipe.start();
     if (rc) return rc;
-    if (c > 0 && (rc = locator.init_rebuild(plan, cols, chk->radius, enc->stream))) return rc;
+    if (c > 0 && (rc = locator.init_rebuild(plan, cols, radius, enc->stream))) return rc;
     if (!reserve.empty()) reserve_extents(reserve, reserve_size);
     walk(chunk, [&](Item&& it, int64_t col) {
         it.shard_off = col;
@@ -776,10 +764,10 @@ int checked_pipeline(swec_encoder* enc, const CheckedPlan& plan, const std::vect
     });  // a failed submit ends the walk, and finish() returns its error
     if ((rc = pipe.finish())) return rc;
     if (c == 0) {
-        unchecked_report(chk->report, chk->n_ranges);
+        chk->unchecked();
         return SWEC_OK;
     }
-    if ((rc = locator.collect(chk->report, chk->ranges, chk->ranges_cap, chk->n_ranges))) return rc;
+    if ((rc = locator.collect(*chk))) return rc;
     chk->checked = true;
     return SWEC_OK;
 }
@@ -788,10 +776,10 @@ int checked_pipeline(swec_encoder* enc, const CheckedPlan& plan, const std::vect
 // the rebuilt shards are written to `out` (in ascending id of the missing shards).
 int rebuild_checked(swec_encoder* enc, const std::vector<int>& in, const std::vector<int>& in_d,
                     const std::vector<uint8_t>& present, const std::vector<int>& out, const std::vector<int>& out_d,
-                    int64_t todo, Checked* chk) {
+                    int64_t todo, int radius, DamageOut* chk) {
     CheckedPlan plan;
     if (!plan.build(enc->gen, enc->k, present.data(), /*decode=*/false)) return fail(SWEC_ERR_TOO_FEW_SHARDS, "not enough shards");
-    return checked_pipeline(enc, plan, in, in_d, todo, out, todo, chk, [&](size_t chunk, const SubmitFn& submit) {
+    return checked_pipeline(enc, plan, in, in_d, todo, out, todo, radius, chk, [&](size_t chunk, const SubmitFn& submit) {
         int rc = SWEC_OK;
         for (int64_t o = 0; rc == SWEC_OK && o < todo; o += int64_t(chunk)) {
             Item it;
@@ -804,11 +792,11 @@ int rebuild_checked(swec_encoder* enc, const std::vector<int>& in, const std::ve
     });
 }
 
-// swec_rebuild_ec_files, and with `chk` swec_rebuild_ec_files_checked: the same files, checks, errors and order.  The
+// swec_rebuild_ec_files, and with `chk` swec_rebuild_ec_files_checked at `radius`: the same files, checks, errors and order.  The
 // checked rebuild reads every present shard, not only the first k, and corrects the damage it locates in the first k
 // before it reaches the rebuilt shards.
 int rebuild_files(const char* base, const char* const* dirs, int ndirs, int k, int m, int device, uint32_t* rebuilt,
-                  int* n_rebuilt, Checked* chk) {
+                  int* n_rebuilt, int radius, DamageOut* chk) {
     if (!base || !rebuilt || !n_rebuilt || (ndirs > 0 && !dirs)) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
     *n_rebuilt = 0;
     const std::string b(base);
@@ -872,7 +860,7 @@ int rebuild_files(const char* base, const char* const* dirs, int ndirs, int k, i
     const int64_t todo = ragged ? size / mib * mib : size;
 
     if (chk) {
-        if ((rc = rebuild_checked(enc.get(), in, in_d, present, out, out_d, todo, chk))) return rc;
+        if ((rc = rebuild_checked(enc.get(), in, in_d, present, out, out_d, todo, radius, chk))) return rc;
     } else {
         std::vector<int> ins, outs_idx;  // outs_idx == missing: fused row r rebuilds the shard of out[r]
         Matrix fused;
@@ -902,7 +890,7 @@ int rebuild_files(const char* base, const char* const* dirs, int ndirs, int k, i
 // the k data streams into the .dat at the plan's offsets; shard s holds tail_bytes(s) of the tail row.
 int decode_dat(swec_encoder* enc, const std::vector<int>& in, const std::vector<int>& in_d,
                const std::vector<uint8_t>& present, int dat, int dat_d, const StripeGeometry& g, int64_t dat_size,
-               int64_t cols, Checked* chk) {
+               int64_t cols, int radius, DamageOut* chk) {
     const int k = enc->k;
     CheckedPlan plan;
     if (!plan.build(enc->gen, k, present.data(), /*decode=*/true)) return fail(SWEC_ERR_TOO_FEW_SHARDS, "not enough shards");
@@ -914,7 +902,7 @@ int decode_dat(swec_encoder* enc, const std::vector<int>& in, const std::vector<
             if (n > 0) it.writes.push_back({stream[size_t(s)], dat, row_dat + int64_t(s) * block + col, src, size_t(n), dat_d});
         }
     };
-    return checked_pipeline(enc, plan, in, in_d, cols, {dat}, dat_size, chk, [&](size_t chunk, const SubmitFn& submit) {
+    return checked_pipeline(enc, plan, in, in_d, cols, {dat}, dat_size, radius, chk, [&](size_t chunk, const SubmitFn& submit) {
         return walk_items(g, chunk, g.tail_bytes(0), unstripe, submit);
     });
 }
@@ -929,12 +917,12 @@ namespace swec {
 // shard's descriptor is opened again for writing through /proc/self/fd before anything is read again, and the call
 // fails there, with nothing written, when that is refused.
 int needle_damage_files(swec_encoder* enc, const std::vector<int>& in, int64_t size, int radius, const StripeMap& map,
-                        int version, bool repair, std::vector<swec_needle_damage>* recs, swec_damage_report* report,
-                        swec_damage_range* ranges, int ranges_cap, int* n_ranges, uint64_t unowned[2]) {
+                        int version, bool repair, std::vector<swec_needle_damage>* recs, const DamageOut& out,
+                        uint64_t unowned[2]) {
     const Matrix rows = parity_rows(enc);
     std::vector<swec_damage_range> runs;
-    int rc = locate_pass(enc, rows, in, size, radius, report, ranges, ranges_cap, n_ranges, &runs);
-    if (rc || report->damaged_columns == 0) return rc;
+    int rc = locate_pass(enc, rows, in, size, radius, out, &runs);
+    if (rc || out.report->damaged_columns == 0) return rc;
     const int k = enc->k;
     PageWrites writes(runs, int(in.size()));
     FdSet fds;
@@ -1058,7 +1046,7 @@ int swec_write_ec_files(const char* base, int device) {
 
 int swec_rebuild_ec_files(const char* base, const char* const* dirs, int ndirs, int k, int m, int device,
                           uint32_t* rebuilt, int* n_rebuilt) {
-    return rebuild_files(base, dirs, ndirs, k, m, device, rebuilt, n_rebuilt, nullptr);
+    return rebuild_files(base, dirs, ndirs, k, m, device, rebuilt, n_rebuilt, 0, nullptr);
 }
 
 int swec_rebuild_ec_files_checked(const char* base, const char* const* dirs, int ndirs, int k, int m, int device,
@@ -1067,9 +1055,10 @@ int swec_rebuild_ec_files_checked(const char* base, const char* const* dirs, int
     if (!base || !rebuilt || !n_rebuilt || !ok || (ndirs > 0 && !dirs)) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
     *ok = 0;
     *n_rebuilt = 0;
-    if (const int rc = check_rebuild_args(radius, report, ranges, ranges_cap)) return rc;
-    Checked chk{radius, report, ranges, ranges_cap, n_ranges};
-    const int rc = rebuild_files(base, dirs, ndirs, k, m, device, rebuilt, n_rebuilt, &chk);
+    DamageOut chk{report, ranges, ranges_cap, n_ranges};
+    int rc;
+    if ((rc = chk.check()) || (rc = check_radius(radius, 0))) return rc;
+    rc = rebuild_files(base, dirs, ndirs, k, m, device, rebuilt, n_rebuilt, radius, &chk);
     *ok = rc == SWEC_OK && chk.checked && report->uncorrectable_columns == 0 ? 1 : 0;
     return rc;
 }
@@ -1160,12 +1149,12 @@ int swec_page_sketch_file(const char* path, int device, uint64_t seed, uint64_t*
 
 int swec_locate_ec_damage(const char* base, const char* const* dirs, int ndirs, int k, int m, int device, int radius,
                           swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges, int* ok) {
-    return damage_files(base, dirs, ndirs, k, m, device, radius, false, report, ranges, ranges_cap, n_ranges, ok);
+    return damage_files(base, dirs, ndirs, k, m, device, radius, false, {report, ranges, ranges_cap, n_ranges}, ok);
 }
 
 int swec_repair_ec_damage(const char* base, const char* const* dirs, int ndirs, int k, int m, int device, int radius,
                           swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges, int* ok) {
-    return damage_files(base, dirs, ndirs, k, m, device, radius, true, report, ranges, ranges_cap, n_ranges, ok);
+    return damage_files(base, dirs, ndirs, k, m, device, radius, true, {report, ranges, ranges_cap, n_ranges}, ok);
 }
 
 int swec_write_dat_file(const char* base, int64_t dat_size, const char* const* shard_names, int k, int64_t large,
@@ -1248,8 +1237,9 @@ int swec_write_dat_file_checked(const char* base, int64_t dat_size, const char* 
     if (!base || !names || !ok || k <= 0 || m <= 0 || k + m > SWEC_MAX_SHARDS || large <= 0 || small <= 0 || dat_size < 0)
         return fail(SWEC_ERR_INVALID_ARG, "bad argument");
     *ok = 0;
-    int rc = check_rebuild_args(radius, report, ranges, ranges_cap);
-    if (rc) return rc;
+    DamageOut chk{report, ranges, ranges_cap, n_ranges};
+    int rc;
+    if ((rc = chk.check()) || (rc = check_radius(radius, 0))) return rc;
     const int total = k + m;
     FdSet fds;
     const long direct = g_opt_file_direct_io.load();
@@ -1276,7 +1266,7 @@ int swec_write_dat_file_checked(const char* base, int64_t dat_size, const char* 
     bool all_data = true;
     for (int s = 0; s < k; s++) all_data = all_data && present[size_t(s)];
     if (all_data && npresent == k) {  // the data shards alone: nothing to check, nothing to rebuild
-        unchecked_report(report, n_ranges);
+        chk.unchecked();
         return swec_write_dat_file(base, dat_size, names, k, large, small);
     }
     CallEncoder enc;
@@ -1293,8 +1283,8 @@ int swec_write_dat_file_checked(const char* base, int64_t dat_size, const char* 
     } undo{path};
     const int dat_d = fds.keep(open_direct(path, O_WRONLY, direct & 2));
     if (ftruncate(dat, off_t(dat_size)) != 0) return io_fail("size .dat");
-    Checked chk{radius, report, ranges, ranges_cap, n_ranges};
-    if ((rc = decode_dat(enc.get(), in, in_d, present, dat, dat_d, g, dat_size, g.tail_shard_offset() + g.tail_bytes(0), &chk)))
+    if ((rc = decode_dat(enc.get(), in, in_d, present, dat, dat_d, g, dat_size, g.tail_shard_offset() + g.tail_bytes(0), radius,
+                         &chk)))
         return rc;
     if (chk.checked && report->uncorrectable_columns)
         return fail(SWEC_ERR_UNCORRECTABLE, std::to_string(report->uncorrectable_columns) + " byte columns of " + std::string(base) +

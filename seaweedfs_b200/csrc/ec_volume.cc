@@ -149,7 +149,8 @@ int swec_ec_shards_to_volume_checked(const char* data_base, const char* index_ba
                                      int* ok) {
     if (!data_base || !ok || (n_additional_dirs > 0 && !additional_dirs)) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
     *ok = 0;
-    if (const int rc = check_rebuild_args(radius, report, ranges, ranges_cap)) return rc;
+    int rc;
+    if ((rc = DamageOut{report, ranges, ranges_cap, n_ranges}.check()) || (rc = check_radius(radius, 0))) return rc;
     const std::string db(data_base);
     int k, m;
     ec_ratio(db, &k, &m);
@@ -169,8 +170,7 @@ int swec_ec_shards_to_volume_checked(const char* data_base, const char* index_ba
     if (names[0].empty() && (version = read_volume_info(db, ib).version) <= 0)
         return fail(SWEC_ERR_TOO_FEW_SHARDS, "ec volume " + db + " has no .ec00 and no needle version in its .vif");
     int64_t size = 0;
-    int rc = decoded_dat_size(ib, names[0], int(version), &size);
-    if (rc) return rc;
+    if ((rc = decoded_dat_size(ib, names[0], int(version), &size))) return rc;
     std::vector<const char*> cnames;
     for (const auto& s : names) cnames.push_back(s.empty() ? nullptr : s.c_str());
     if ((rc = swec_write_dat_file_checked(db.c_str(), size, cnames.data(), k, m, kLargeBlockSize, kSmallBlockSize, device,
@@ -708,16 +708,15 @@ int recheck_needles(swec_ec_volume* v, const std::vector<swec_needle_damage>& na
 // Both needle damage calls on the handle (include/swec.h): every check before any device work, the live records as the
 // reads see them, then pass 1 and, with damage, pass 2 (needle_damage_files).  With `checks` (the repair), pass 2 also
 // writes the corrections, and every named needle is re-checked from the repaired files.
-int handle_needle_damage(swec_ec_volume* v, int radius, swec_damage_report* report, swec_damage_range* ranges,
-                         int ranges_cap, int* n_ranges, swec_needle_damage* needles, bool repair, swec_needle_check* checks,
-                         int needles_cap, int* n_needles, uint64_t unowned[2], int* ok) {
+int handle_needle_damage(swec_ec_volume* v, int radius, const DamageOut& out, swec_needle_damage* needles, bool repair,
+                         swec_needle_check* checks, int needles_cap, int* n_needles, uint64_t unowned[2], int* ok) {
     int rc = check_needle_damage_args(needles_cap, needles, unowned, 0, nullptr);
     if (rc) return rc;
     if (repair && needles_cap > 0 && !checks)
         return fail(SWEC_ERR_INVALID_ARG, "checks must be non-NULL when needles_cap is > 0");
     if (!v || !n_needles || !ok) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
     std::lock_guard<std::mutex> lock(v->mu);
-    if ((rc = check_locate_args(v->m, radius, report, ranges, ranges_cap))) return rc;
+    if ((rc = out.check()) || (rc = check_radius(radius, 1, v->m))) return rc;
     *ok = 0;
     *n_needles = 0;
     unowned[0] = unowned[1] = 0;
@@ -744,8 +743,7 @@ int handle_needle_damage(swec_ec_volume* v, int radius, swec_damage_report* repo
     }
     if (!v->enc && (rc = swec_encoder_new(v->k, v->m, v->device, &v->enc))) return rc;
     const StripeMap map = StripeMap::locate(v->shard_dat_size, v->k, kLargeBlockSize, kSmallBlockSize);
-    if ((rc = needle_damage_files(v->enc, v->shard_fd, size, radius, map, v->version, repair, &recs, report, ranges,
-                                  ranges_cap, n_ranges, unowned)))
+    if ((rc = needle_damage_files(v->enc, v->shard_fd, size, radius, map, v->version, repair, &recs, out, unowned)))
         return rc;
     std::stable_sort(recs.begin(), recs.end(),
                      [](const swec_needle_damage& a, const swec_needle_damage& b) { return a.needle_id < b.needle_id; });
@@ -755,12 +753,12 @@ int handle_needle_damage(swec_ec_volume* v, int radius, swec_damage_report* repo
     for (int j = 0; j < needles_cap && j < int(recs.size()); j++) needles[j] = recs[size_t(j)];
     *n_needles = int(recs.size());
     if (!repair) {
-        *ok = report->damaged_columns == 0 ? 1 : 0;
+        *ok = out.report->damaged_columns == 0 ? 1 : 0;
         return SWEC_OK;
     }
     std::vector<swec_needle_check> rechecked;
     if ((rc = recheck_needles(v, recs, &rechecked))) return rc;
-    bool all_ok = report->uncorrectable_columns == 0;
+    bool all_ok = out.report->uncorrectable_columns == 0;
     for (size_t j = 0; j < rechecked.size(); j++) {
         all_ok = all_ok && rechecked[j].status == SWEC_NEEDLE_OK;
         if (int(j) < needles_cap) checks[j] = rechecked[j];
@@ -806,7 +804,7 @@ int swec_ec_volume_info(swec_ec_volume* v, int* data_shards, int* parity_shards,
 int swec_ec_volume_locate_needle_damage(swec_ec_volume* v, int radius, swec_damage_report* report, swec_damage_range* ranges,
                                         int ranges_cap, int* n_ranges, swec_needle_damage* needles, int needles_cap,
                                         int* n_needles, uint64_t unowned[2], int* ok) {
-    return handle_needle_damage(v, radius, report, ranges, ranges_cap, n_ranges, needles, false, nullptr, needles_cap,
+    return handle_needle_damage(v, radius, {report, ranges, ranges_cap, n_ranges}, needles, false, nullptr, needles_cap,
                                 n_needles, unowned, ok);
 }
 
@@ -814,7 +812,7 @@ int swec_ec_volume_repair_needle_damage(swec_ec_volume* v, int radius, swec_dama
                                         int ranges_cap, int* n_ranges, swec_needle_damage* needles,
                                         swec_needle_check* checks, int needles_cap, int* n_needles, uint64_t unowned[2],
                                         int* ok) {
-    return handle_needle_damage(v, radius, report, ranges, ranges_cap, n_ranges, needles, true, checks, needles_cap,
+    return handle_needle_damage(v, radius, {report, ranges, ranges_cap, n_ranges}, needles, true, checks, needles_cap,
                                 n_needles, unowned, ok);
 }
 

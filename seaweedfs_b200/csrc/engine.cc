@@ -616,16 +616,13 @@ int swec_verify(swec_encoder* e, uint8_t* const* shards, size_t n, int* ok) {
 
 // ---- device-resident
 
-// `stream` is a plain cudaStream_t; NULL is CUDA's default stream, exactly as in the runtime API
-static cudaStream_t pick_stream(swec_encoder*, void* stream) { return static_cast<cudaStream_t>(stream); }
-
 int swec_encode_device(swec_encoder* e, const void* const* data, void* const* parity, size_t n, void* stream) {
     if (!e || !data || !parity) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
     std::lock_guard<std::mutex> lock(e->mu);
     int rc = e->ensure_device();
     if (rc) return rc;
     return e->apply(parity_rows(e), reinterpret_cast<const uint8_t* const*>(data),
-                    reinterpret_cast<uint8_t* const*>(parity), n, Layout{}, pick_stream(e, stream));
+                    reinterpret_cast<uint8_t* const*>(parity), n, Layout{}, static_cast<cudaStream_t>(stream));
 }
 
 int swec_reconstruct_device(swec_encoder* e, void* const* shards, const uint8_t* present, size_t n, int data_only,
@@ -639,7 +636,7 @@ int swec_reconstruct_device(swec_encoder* e, void* const* shards, const uint8_t*
     if ((rc = p.gather(reinterpret_cast<uint8_t* const*>(shards), ins, outs))) return rc;
     std::lock_guard<std::mutex> lock(e->mu);
     if ((rc = e->ensure_device())) return rc;
-    return e->apply(p.fused, ins, outs, n, Layout{}, pick_stream(e, stream));
+    return e->apply(p.fused, ins, outs, n, Layout{}, static_cast<cudaStream_t>(stream));
 }
 
 int swec_apply_device(swec_encoder* e, int r, int k, const uint8_t* rows, const void* const* in, void* const* out,
@@ -652,7 +649,7 @@ int swec_apply_device(swec_encoder* e, int r, int k, const uint8_t* rows, const 
     int rc = e->ensure_device();
     if (rc) return rc;
     return e->apply(m, reinterpret_cast<const uint8_t* const*>(in), reinterpret_cast<uint8_t* const*>(out), n,
-                    Layout{}, pick_stream(e, stream));
+                    Layout{}, static_cast<cudaStream_t>(stream));
 }
 
 int swec_encode_volume_device(swec_encoder* e, const void* dat_v, int64_t dat_size, int64_t large, int64_t small,
@@ -666,7 +663,7 @@ int swec_encode_volume_device(swec_encoder* e, const void* dat_v, int64_t dat_si
     std::lock_guard<std::mutex> lock(e->mu);
     int rc = e->ensure_device();
     if (rc) return rc;
-    cudaStream_t s = pick_stream(e, stream);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
     const Matrix rows = parity_rows(e);
     bool horner = is_rs10x4_parity(*e, rows);
     if (!horner && e->m <= SWEC_MAX_OUTPUTS && g_opt_jit_enabled.load() && jit_available()) {
@@ -721,7 +718,7 @@ int swec_extract_data_shard_device(swec_encoder* e, const void* dat_v, int64_t d
     std::lock_guard<std::mutex> lock(e->mu);
     int rc = e->ensure_device();
     if (rc) return rc;
-    cudaStream_t s = pick_stream(e, stream);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
     const StripeGeometry g(dat_size, e->k, large, small);
     if (g.large_rows)
         SWEC_CUDA(cudaMemcpy2DAsync(dst, size_t(large), dat + int64_t(shard_id) * large, size_t(g.large_row()), size_t(large),
@@ -749,7 +746,7 @@ int swec_write_dat_device(swec_encoder* e, const void* const* data_shards, int64
     std::lock_guard<std::mutex> lock(e->mu);
     int rc = e->ensure_device();
     if (rc) return rc;
-    cudaStream_t s = pick_stream(e, stream);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
     // WriteDatFile's loops (ec_decoder.go:197-219): `for datFileSize >= dataShards*LargeBlockSize` copies large blocks
     // round-robin, then small blocks until the size is used up — the last block short
     const StripeGeometry g(dat_size, k, large, small);
@@ -802,26 +799,22 @@ int locate_pieces(swec_encoder* e, const CheckedPlan& plan, uint8_t* const* sh, 
 }
 
 // swec_locate_damage_device, and with `correct` swec_correct_damage_device: the shards are written only then.
-int damage_device(swec_encoder* e, const void* const* shards, size_t n, int radius, bool correct,
-                  swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges, void* stream) {
+int damage_device(swec_encoder* e, const void* const* shards, size_t n, int radius, bool correct, const DamageOut& out,
+                  void* stream) {
     if (!e || !shards) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
-    int rc = check_locate_args(e->m, radius, report, ranges, ranges_cap);
-    if (rc) return rc;
-    const int k = e->k, m = e->m;
-    for (int i = 0; i < k + m; i++)
+    int rc;
+    if ((rc = out.check()) || (rc = check_radius(radius, 1, e->m))) return rc;
+    for (int i = 0; i < e->k + e->m; i++)
         if (!shards[i]) return fail(SWEC_ERR_INVALID_ARG, "NULL shard");
     uint8_t* const* sh = reinterpret_cast<uint8_t* const*>(const_cast<void* const*>(shards));
-    // every shard present: the data shards are the information set, fused is the parity rows, the checks are parity
-    const std::vector<uint8_t> all(static_cast<size_t>(k + m), 1);
-    CheckedPlan plan;
-    plan.build(e->gen, k, all.data(), false);
+    const CheckedPlan plan = CheckedPlan::all_present(e->gen, e->k);
     std::lock_guard<std::mutex> lock(e->mu);
     if ((rc = e->ensure_device())) return rc;
-    cudaStream_t s = pick_stream(e, stream);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
     DamageLocator locator;
     if ((rc = locator.init(plan.fused, int64_t(n), radius, s, correct))) return rc;
     if ((rc = locate_pieces(e, plan, sh, n, locator, s))) return rc;
-    return locator.collect(report, ranges, ranges_cap, n_ranges);
+    return locator.collect(out);
 }
 
 }  // namespace
@@ -830,12 +823,12 @@ extern "C" {
 
 int swec_locate_damage_device(swec_encoder* e, const void* const* shards, size_t n, int radius, swec_damage_report* report,
                               swec_damage_range* ranges, int ranges_cap, int* n_ranges, void* stream) {
-    return damage_device(e, shards, n, radius, false, report, ranges, ranges_cap, n_ranges, stream);
+    return damage_device(e, shards, n, radius, false, {report, ranges, ranges_cap, n_ranges}, stream);
 }
 
 int swec_correct_damage_device(swec_encoder* e, void* const* shards, size_t n, int radius, swec_damage_report* report,
                                swec_damage_range* ranges, int ranges_cap, int* n_ranges, void* stream) {
-    return damage_device(e, shards, n, radius, true, report, ranges, ranges_cap, n_ranges, stream);
+    return damage_device(e, shards, n, radius, true, {report, ranges, ranges_cap, n_ranges}, stream);
 }
 
 }  // extern "C"
@@ -849,10 +842,10 @@ namespace {
 // missing data shards and also corrects the present data shards in place; parity shards are only read, and a missing
 // one needs no buffer.
 int checked_device(swec_encoder* e, void* const* shards, const uint8_t* present, size_t n, int radius, bool decode,
-                   swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges, void* stream) {
+                   const DamageOut& out, void* stream) {
     if (!e || !shards || !present) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
-    int rc = check_rebuild_args(radius, report, ranges, ranges_cap);
-    if (rc) return rc;
+    int rc;
+    if ((rc = out.check()) || (rc = check_radius(radius, 0))) return rc;
     const int k = e->k, total = e->k + e->m;
     CheckedPlan plan;
     if (!plan.build(e->gen, k, present, decode)) return fail(SWEC_ERR_TOO_FEW_SHARDS, "fewer than data_shards shards present");
@@ -861,15 +854,15 @@ int checked_device(swec_encoder* e, void* const* shards, const uint8_t* present,
             return fail(SWEC_ERR_INVALID_ARG, present[i] ? "NULL shard" : "missing shard has no buffer");
     std::lock_guard<std::mutex> lock(e->mu);
     if ((rc = e->ensure_device())) return rc;
-    cudaStream_t s = pick_stream(e, stream);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
     DamageLocator locator;
     if (plan.c() > 0 && (rc = locator.init_rebuild(plan, int64_t(n), radius, s))) return rc;
     if ((rc = locate_pieces(e, plan, reinterpret_cast<uint8_t* const*>(shards), n, locator, s))) return rc;
     if (plan.c() == 0) {  // every present shard is an information shard: nothing to check
-        unchecked_report(report, n_ranges);
+        out.unchecked();
         return SWEC_OK;
     }
-    return locator.collect(report, ranges, ranges_cap, n_ranges);
+    return locator.collect(out);
 }
 
 }  // namespace
@@ -879,20 +872,20 @@ extern "C" {
 int swec_reconstruct_checked_device(swec_encoder* e, void* const* shards, const uint8_t* present, size_t n, int radius,
                                     swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges,
                                     void* stream) {
-    return checked_device(e, shards, present, n, radius, false, report, ranges, ranges_cap, n_ranges, stream);
+    return checked_device(e, shards, present, n, radius, false, {report, ranges, ranges_cap, n_ranges}, stream);
 }
 
 int swec_decode_data_checked_device(swec_encoder* e, void* const* shards, const uint8_t* present, size_t n, int radius,
                                     swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges,
                                     void* stream) {
-    return checked_device(e, shards, present, n, radius, true, report, ranges, ranges_cap, n_ranges, stream);
+    return checked_device(e, shards, present, n, radius, true, {report, ranges, ranges_cap, n_ranges}, stream);
 }
 
 int swec_stream_synchronize(swec_encoder* e, void* stream) {
     if (!e) return fail(SWEC_ERR_INVALID_ARG, "NULL encoder");
     int rc = e->ensure_device();
     if (rc) return rc;
-    SWEC_CUDA(cudaStreamSynchronize(pick_stream(e, stream)));
+    SWEC_CUDA(cudaStreamSynchronize(static_cast<cudaStream_t>(stream)));
     return SWEC_OK;
 }
 

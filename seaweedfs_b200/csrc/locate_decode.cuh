@@ -22,6 +22,12 @@ struct LocateTables {
 constexpr int kTableWords = int(sizeof(LocateTables) / 4);
 static_assert(sizeof(LocateTables) % 16 == 0, "tables are copied in words");
 
+// The log R table of the rebuilding decodes (CheckedPlan::rebuilt_logs): log R[r][j] of rebuilt row r and information
+// position j at byte r*32 + j, kLogZero for a zero entry (logs of non-zero bytes are < 255).
+constexpr u8 kLogZero = 0xff;
+constexpr int kLogRBytes = 32 * 32;
+constexpr int kLogRWords = kLogRBytes / 4;
+
 // logs of the field's non-zero bytes (to base 2), and two periods of powers of 2
 void log_exp_tables(u8* log, u8* exp) {
     unsigned x = 1;

@@ -177,7 +177,8 @@ int swec_locate_needle_damage_device(swec_encoder* e, const void* const* shards,
     int rc = check_needle_damage_args(0, nullptr, unowned, n_records, records);
     if (rc) return rc;
     if (!e || !shards) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
-    if ((rc = check_locate_args(e->m, radius, report, ranges, ranges_cap))) return rc;
+    const DamageOut out{report, ranges, ranges_cap, n_ranges};
+    if ((rc = out.check()) || (rc = check_radius(radius, 1, e->m))) return rc;
     if (dat_size < 0 || large <= 0 || small <= 0) return fail(SWEC_ERR_INVALID_ARG, "bad geometry");
     const int k = e->k, m = e->m;
     for (int i = 0; i < k + m; i++)
@@ -215,7 +216,7 @@ int swec_locate_needle_damage_device(swec_encoder* e, const void* const* shards,
         if ((rc = nd.launch(orig, work, comp, len, int64_t(off), 0, s))) return rc;
     }
     SWEC_CUDA(cudaStreamSynchronize(s));
-    if ((rc = locator.collect(report, ranges, ranges_cap, n_ranges))) return rc;
+    if ((rc = locator.collect(out))) return rc;
     return nd.collect(records, unowned);
 }
 

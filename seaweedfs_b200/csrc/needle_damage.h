@@ -13,6 +13,7 @@
 #include <vector>
 
 #include "../../include/swec.h"
+#include "damage.h"
 #include "engine.h"
 #include "stripe_map.h"
 
@@ -59,7 +60,7 @@ class NeedleDamage {
 // the repair does, through a NeedleDamage over `recs` mapped by `map`.  recs' counts and unowned are left zero on a
 // clean set.  `repair`: pass 2 also writes what swec_repair_ec_damage's pass 2 writes, to the files behind `in`.
 int needle_damage_files(swec_encoder* enc, const std::vector<int>& in, int64_t size, int radius, const StripeMap& map,
-                        int version, bool repair, std::vector<swec_needle_damage>* recs, swec_damage_report* report,
-                        swec_damage_range* ranges, int ranges_cap, int* n_ranges, uint64_t unowned[2]);
+                        int version, bool repair, std::vector<swec_needle_damage>* recs, const DamageOut& out,
+                        uint64_t unowned[2]);
 
 }  // namespace swec

@@ -83,9 +83,6 @@ __global__ void __launch_bounds__(256) swec_page_sketch_kernel(const u8* __restr
     }
 }
 
-constexpr u8 kLogZero = 0xff;  // log R entry of a zero coefficient (logs of non-zero bytes are < 255)
-constexpr int kLogRWords = 32 * 32 / 4;  // log R[r][j] at byte r*32 + j, after the LocateTables
-
 struct SketchPageParams {
     const u64* comp[SWEC_MAX_SHARDS];    // check sketches recomputed from the information sketches
     const u64* stored[SWEC_MAX_SHARDS];  // check sketches as their holders sent them
@@ -93,7 +90,7 @@ struct SketchPageParams {
     u8 ids[SWEC_MAX_SHARDS];             // shard id of every position: information 0..k-1, checks k..k+c-1
     u64 pages;
     int k, c, f, radius;                 // information, check and lost shards; the radius, at most c/2
-    const u32* tables;                   // LocateTables of the check rows P', then log R (f > 0)
+    const u32* tables;                   // LocateTables of the check rows P', then log R (kLogRWords, f > 0)
     swec_sketch_page* flagged;           // one entry per flagged page, in no particular order
     unsigned long long* count;           // entries written
 };
@@ -172,11 +169,11 @@ __global__ void __launch_bounds__(256) swec_sketch_pages_kernel(const __grid_con
 }
 
 // Both sketch calls: sketches[id] are the host sketches of the present shards (n_pages words each), decoded over
-// `plan` at radius t <= c/2.  One apply of plan.fused to the uploaded information sketches gives the check sketches
+// `plan` at plan.radius(radius).  One apply of plan.fused to the uploaded information sketches gives the check sketches
 // and R·(information sketches) of every lost shard; the page decode (c >= 1) compares the check sketches with the
 // stored ones and corrects the lost shards' sketches.  The flagged pages come back in ascending page order, and the
 // sketch of lost shard id into out[id] where out and out[id] are non-NULL.  Synchronous on the encoder's stream.
-int sketch_pages(swec_encoder* e, const CheckedPlan& plan, const uint64_t* const* sketches, int64_t n_pages, int t,
+int sketch_pages(swec_encoder* e, const CheckedPlan& plan, const uint64_t* const* sketches, int64_t n_pages, int radius,
                  uint64_t* const* out, std::vector<swec_sketch_page>* flagged) {
     const int k = e->k, c = plan.c(), nout = int(plan.outs.size()), f = int(plan.rebuilt_rows.size());
     flagged->clear();
@@ -198,16 +195,9 @@ int sketch_pages(swec_encoder* e, const CheckedPlan& plan, const uint64_t* const
     // sketches are linear: the plan's rows applied to the information sketches give every other shard's clean sketch
     if (int rc = e->apply(plan.fused, at, comp, bytes, Layout{}, s)) return rc;
     if (c > 0) {
-        std::vector<u8> host(sizeof(LocateTables) + size_t(kLogRWords) * 4, kLogZero);
-        LocateTables& lt = *reinterpret_cast<LocateTables*>(host.data());
-        Matrix pc(c, k);
-        for (int i = 0; i < c; i++)
-            for (int j = 0; j < k; j++) pc.at(i, j) = plan.fused.at(plan.check_rows[size_t(i)], j);
-        locate_tables(pc, &lt);
-        u8* logr = host.data() + sizeof(LocateTables);
-        for (int r = 0; r < f; r++)
-            for (int j = 0; j < k; j++)
-                if (const u8 v = plan.fused.at(plan.rebuilt_rows[size_t(r)], j)) logr[r * 32 + j] = lt.log[v];
+        std::vector<u8> host(sizeof(LocateTables) + kLogRBytes);
+        locate_tables(plan.checks(), reinterpret_cast<LocateTables*>(host.data()));
+        plan.rebuilt_logs(host.data() + sizeof(LocateTables));
         DeviceBuffer tables;
         SWEC_CUDA(tables.upload(host.data(), host.size(), s));
         StreamScratch res(s);
@@ -225,7 +215,7 @@ int sketch_pages(swec_encoder* e, const CheckedPlan& plan, const uint64_t* const
         p.k = k;
         p.c = c;
         p.f = f;
-        p.radius = t;
+        p.radius = plan.radius(radius);
         p.tables = tables.as<u32>();
         p.count = res.as<unsigned long long>();
         p.flagged = reinterpret_cast<swec_sketch_page*>(p.count + 1);
@@ -265,8 +255,7 @@ int locate_sketches(swec_encoder* e, const CheckedPlan& plan, const uint64_t* co
     if (int rc = e->ensure_device()) return rc;
     const int64_t n_pages = (shard_len + int64_t(kPage) - 1) / int64_t(kPage);
     std::vector<swec_sketch_page> flagged;
-    // the punctured code has distance c+1: radius t needs 2t <= c
-    if (int rc = sketch_pages(e, plan, sketches, n_pages, std::min(radius, plan.c() / 2), rebuilt, &flagged)) return rc;
+    if (int rc = sketch_pages(e, plan, sketches, n_pages, radius, rebuilt, &flagged)) return rc;
     if (shard_pages) memset(shard_pages, 0, SWEC_MAX_SHARDS * sizeof *shard_pages);
     for (size_t i = 0; i < flagged.size(); i++) {
         if (int64_t(i) < pages_cap) pages[i] = flagged[i];
@@ -321,19 +310,12 @@ int swec_locate_sketch_damage(swec_encoder* e, const uint64_t* const* sketches, 
     if (shard_len < 0) return fail(SWEC_ERR_INVALID_ARG, "shard_len must be >= 0");
     if (pages_cap < 0 || (pages_cap > 0 && !pages))
         return fail(SWEC_ERR_INVALID_ARG, "pages_cap must be >= 0, and pages non-NULL when it is > 0");
-    if (radius < 0 || radius > 2) return fail(SWEC_ERR_INVALID_ARG, "radius must be 0, 1 or 2");
-    const int k = e->k, m = e->m;
-    if (2 * radius > m)
-        return fail(SWEC_ERR_INVALID_ARG, "radius " + std::to_string(radius) + " needs at least " +
-                                              std::to_string(2 * radius) + " parity shards, the code has " + std::to_string(m));
-    for (int i = 0; i < k + m; i++)
+    if (int rc = check_radius(radius, 0, e->m)) return rc;
+    for (int i = 0; i < e->k + e->m; i++)
         if (!sketches[i])
             return fail(SWEC_ERR_TOO_FEW_SHARDS, "no sketch of shard " + std::to_string(i) + ": rebuild it first");
-    // every shard present: the data shards are the information set, fused is the parity rows, the checks are parity
-    const std::vector<uint8_t> all(size_t(k + m), 1);
-    CheckedPlan plan;
-    plan.build(e->gen, k, all.data(), false);
-    return locate_sketches(e, plan, sketches, shard_len, radius, pages, pages_cap, n_flagged, shard_pages, nullptr, ok);
+    return locate_sketches(e, CheckedPlan::all_present(e->gen, e->k), sketches, shard_len, radius, pages, pages_cap,
+                           n_flagged, shard_pages, nullptr, ok);
 }
 
 int swec_locate_sketch_damage_checked(swec_encoder* e, const uint64_t* const* sketches, int64_t shard_len, int radius,
@@ -343,7 +325,7 @@ int swec_locate_sketch_damage_checked(swec_encoder* e, const uint64_t* const* sk
     if (shard_len < 0) return fail(SWEC_ERR_INVALID_ARG, "shard_len must be >= 0");
     if (pages_cap < 0 || (pages_cap > 0 && !pages))
         return fail(SWEC_ERR_INVALID_ARG, "pages_cap must be >= 0, and pages non-NULL when it is > 0");
-    if (radius < 0 || radius > 2) return fail(SWEC_ERR_INVALID_ARG, "radius must be 0, 1 or 2");
+    if (int rc = check_radius(radius, 0)) return rc;
     std::vector<uint8_t> present(size_t(e->k + e->m));
     for (size_t i = 0; i < present.size(); i++) present[i] = sketches[i] != nullptr;
     CheckedPlan plan;

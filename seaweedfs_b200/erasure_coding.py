@@ -181,20 +181,18 @@ class Encoder:
                              stream: int = 0) -> dict:
         """Which shards of k+m shards in device memory are wrong, from the parity syndrome of every byte column
         (swec_locate_damage_device).  Same result as locate_ec_damage, without "ok"."""
-        report, ranges, n = DamageReport(), (DamageRange * max(1, max_ranges))(), C.c_int(0)
-        check(lib().swec_locate_damage_device(self._h, _ptrs(shard_ptrs), shard_len, radius, C.byref(report), ranges,
-                                              max_ranges, C.byref(n), stream))
-        return _damage_result(report, ranges, n.value, max_ranges)
+        out = _DamageOut(max_ranges)
+        check(lib().swec_locate_damage_device(self._h, _ptrs(shard_ptrs), shard_len, radius, *out.args, stream))
+        return out.result()
 
     def correct_damage_device(self, shard_ptrs, shard_len: int, radius: int = 1, max_ranges: int = 4096,
                               stream: int = 0) -> dict:
         """locate_damage_device, which also corrects the located bytes in place (swec_correct_damage_device).  Returns
         the report of the shards as they were; uncorrectable columns are left as they were.  Radius 2 can miscorrect a
         column with 3 or more wrong shards (include/swec.h)."""
-        report, ranges, n = DamageReport(), (DamageRange * max(1, max_ranges))(), C.c_int(0)
-        check(lib().swec_correct_damage_device(self._h, _ptrs(shard_ptrs), shard_len, radius, C.byref(report), ranges,
-                                               max_ranges, C.byref(n), stream))
-        return _damage_result(report, ranges, n.value, max_ranges)
+        out = _DamageOut(max_ranges)
+        check(lib().swec_correct_damage_device(self._h, _ptrs(shard_ptrs), shard_len, radius, *out.args, stream))
+        return out.result()
 
     def locate_needle_damage_device(self, shard_ptrs, shard_len: int, dat_size: int, records, radius: int = 1,
                                     large_block: int = ErasureCodingLargeBlockSize,
@@ -208,11 +206,10 @@ class Encoder:
         arr = (NeedleDamage * max(1, len(records)))()
         for r, (nid, off, size) in zip(arr, records):
             r.needle_id, r.offset, r.size = nid, off, size
-        report, ranges, n, unowned = DamageReport(), (DamageRange * max(1, max_ranges))(), C.c_int(0), (C.c_uint64 * 2)()
+        out, unowned = _DamageOut(max_ranges), (C.c_uint64 * 2)()
         check(lib().swec_locate_needle_damage_device(self._h, _ptrs(shard_ptrs), shard_len, dat_size, large_block,
-                                                     small_block, radius, arr, len(records), C.byref(report), ranges,
-                                                     max_ranges, C.byref(n), unowned, stream))
-        return {**_damage_result(report, ranges, n.value, max_ranges), "needles": _needle_damage(arr[:len(records)]),
+                                                     small_block, radius, arr, len(records), *out.args, unowned, stream))
+        return {**out.result(), "needles": _needle_damage(arr[:len(records)]),
                 "unowned": [int(unowned[0]), int(unowned[1])]}
 
     def reconstruct_checked_device(self, shard_ptrs, present, shard_len: int, radius: int = 1, max_ranges: int = 4096,
@@ -220,11 +217,10 @@ class Encoder:
         """reconstruct_device that reads every present shard and corrects the damage it locates in the first k present
         before it reaches the rebuilt shards (swec_reconstruct_checked_device).  Present shards are only read.  Returns
         the report of locate_damage_device over the present shards; radius 0 only detects (include/swec.h)."""
-        pres = np.ascontiguousarray(np.asarray(present, dtype=np.uint8))
-        report, ranges, n = DamageReport(), (DamageRange * max(1, max_ranges))(), C.c_int(0)
+        pres, out = np.ascontiguousarray(np.asarray(present, dtype=np.uint8)), _DamageOut(max_ranges)
         check(lib().swec_reconstruct_checked_device(self._h, _ptrs(shard_ptrs), pres.ctypes.data, shard_len, radius,
-                                                    C.byref(report), ranges, max_ranges, C.byref(n), stream))
-        return _damage_result(report, ranges, n.value, max_ranges)
+                                                    *out.args, stream))
+        return out.result()
 
     def decode_data_checked_device(self, shard_ptrs, present, shard_len: int, radius: int = 1, max_ranges: int = 4096,
                                    stream: int = 0) -> dict:
@@ -232,11 +228,10 @@ class Encoder:
         corrected in place and the missing data shards rebuilt, from any k present shards; parity shards are only read
         and a missing one may be None.  Returns the report of reconstruct_checked_device for the same shards; radius 0
         only detects (include/swec.h)."""
-        pres = np.ascontiguousarray(np.asarray(present, dtype=np.uint8))
-        report, ranges, n = DamageReport(), (DamageRange * max(1, max_ranges))(), C.c_int(0)
+        pres, out = np.ascontiguousarray(np.asarray(present, dtype=np.uint8)), _DamageOut(max_ranges)
         check(lib().swec_decode_data_checked_device(self._h, _ptrs(shard_ptrs), pres.ctypes.data, shard_len, radius,
-                                                    C.byref(report), ranges, max_ranges, C.byref(n), stream))
-        return _damage_result(report, ranges, n.value, max_ranges)
+                                                    *out.args, stream))
+        return out.result()
 
     def page_sketch_device(self, shard_ptr: int, shard_len: int, sketches_ptr: int, seed: int, first_column: int = 0,
                            stream: int = 0) -> None:
@@ -385,24 +380,20 @@ def write_ec_files(base_file_name: str, ctx: ECContext | None = None) -> None:
 def rebuild_ec_files(base_file_name: str, additional_dirs: list[str] | None = None,
                      ctx: ECContext | None = None, device: int = 0) -> list[int]:
     """RebuildEcFiles (ctx None ⇒ ratio from .vif or 10+4) / RebuildEcFilesWithContext."""
-    dirs = [d.encode() for d in (additional_dirs or [])]
-    arr = (C.c_char_p * max(1, len(dirs)))(*dirs) if dirs else None
+    arr, nd = _dirs(additional_dirs)
     ids = (C.c_uint32 * MaxShardCount)()
     n = C.c_int(0)
-    k, m, dev = (ctx.DataShards, ctx.ParityShards, ctx.device) if ctx else (0, 0, device)
-    check(lib().swec_rebuild_ec_files(base_file_name.encode(), arr, len(dirs), k, m, dev, ids, C.byref(n)))
+    check(lib().swec_rebuild_ec_files(base_file_name.encode(), arr, nd, *_code(ctx, device), ids, C.byref(n)))
     return list(ids[: n.value])
 
 
 def verify_ec_files(base_file_name: str, additional_dirs: list[str] | None = None, ctx: ECContext | None = None,
                     device: int = 0):
     """Parity scrub of a shard set: returns (ok, mismatching 16-byte vectors per parity shard)."""
-    dirs = [d.encode() for d in (additional_dirs or [])]
-    arr = (C.c_char_p * max(1, len(dirs)))(*dirs) if dirs else None
-    k, m, dev = (ctx.DataShards, ctx.ParityShards, ctx.device) if ctx else (0, 0, device)
+    arr, nd = _dirs(additional_dirs)
     bad = (C.c_uint64 * MaxShardCount)()
     ok = C.c_int(0)
-    check(lib().swec_verify_ec_files(base_file_name.encode(), arr, len(dirs), k, m, dev, bad, C.byref(ok)))
+    check(lib().swec_verify_ec_files(base_file_name.encode(), arr, nd, *_code(ctx, device), bad, C.byref(ok)))
     nm = ctx.ParityShards if ctx else ParityShardsCount
     return bool(ok.value), list(bad[:nm])
 
@@ -428,14 +419,25 @@ def _sketch_result(ok, n, pages, per_shard) -> dict:
             "shard_pages": {i: int(per_shard[i]) for i in range(MaxShardCount) if per_shard[i]}}
 
 
-def _damage_result(report, ranges, n_ranges: int, max_ranges: int) -> dict:
-    shards = {i: (int(report.shard_bytes[i]), int(report.shard_first[i]), int(report.shard_last[i]))
-              for i in range(MaxShardCount) if report.shard_bytes[i]}
-    return {"columns": int(report.columns), "damaged_columns": int(report.damaged_columns),
-            "uncorrectable_columns": int(report.uncorrectable_columns),
-            "first_uncorrectable": int(report.first_uncorrectable), "last_uncorrectable": int(report.last_uncorrectable),
-            "shards": shards, "ranges": [(r.shard_id, r.offset, r.length) for r in ranges[:min(n_ranges, max_ranges)]],
-            "n_ranges": n_ranges}
+class _DamageOut:
+    """The report out-parameters of a damage call: `args` are its four ctypes arguments (report, ranges, ranges_cap,
+    n_ranges), result() the report, the first max_ranges ranges and their total as a dict."""
+
+    def __init__(self, max_ranges: int):
+        self.report, self.ranges, self.n = DamageReport(), (DamageRange * max(1, max_ranges))(), C.c_int(0)
+        self.max_ranges = max_ranges
+        self.args = (C.byref(self.report), self.ranges, max_ranges, C.byref(self.n))
+
+    def result(self) -> dict:
+        report, n_ranges = self.report, self.n.value
+        shards = {i: (int(report.shard_bytes[i]), int(report.shard_first[i]), int(report.shard_last[i]))
+                  for i in range(MaxShardCount) if report.shard_bytes[i]}
+        return {"columns": int(report.columns), "damaged_columns": int(report.damaged_columns),
+                "uncorrectable_columns": int(report.uncorrectable_columns),
+                "first_uncorrectable": int(report.first_uncorrectable),
+                "last_uncorrectable": int(report.last_uncorrectable), "shards": shards,
+                "ranges": [(r.shard_id, r.offset, r.length) for r in self.ranges[:min(n_ranges, self.max_ranges)]],
+                "n_ranges": n_ranges}
 
 
 def _needle_damage(recs) -> list[dict]:
@@ -449,11 +451,9 @@ def locate_ec_damage(base_file_name: str, additional_dirs: list[str] | None = No
     counts, "shards" = {shard id: (bytes blamed, first offset, last offset)} for the shards with damage, the
     uncorrectable summary, "ranges" = [(shard id or -1, offset, length)] (the first max_ranges) and "n_ranges"."""
     arr, nd = _dirs(additional_dirs)
-    k, m, dev = (ctx.DataShards, ctx.ParityShards, ctx.device) if ctx else (0, 0, device)
-    report, ranges, n, ok = DamageReport(), (DamageRange * max(1, max_ranges))(), C.c_int(0), C.c_int(0)
-    check(lib().swec_locate_ec_damage(base_file_name.encode(), arr, nd, k, m, dev, radius, C.byref(report), ranges,
-                                      max_ranges, C.byref(n), C.byref(ok)))
-    return {"ok": bool(ok.value), **_damage_result(report, ranges, n.value, max_ranges)}
+    out, ok = _DamageOut(max_ranges), C.c_int(0)
+    check(lib().swec_locate_ec_damage(base_file_name.encode(), arr, nd, *_code(ctx, device), radius, *out.args, C.byref(ok)))
+    return {"ok": bool(ok.value), **out.result()}
 
 
 def repair_ec_damage(base_file_name: str, additional_dirs: list[str] | None = None, ctx: ECContext | None = None,
@@ -462,11 +462,9 @@ def repair_ec_damage(base_file_name: str, additional_dirs: list[str] | None = No
     blamed shards' damaged pages are rewritten.  Returns the report of the files as they were; "ok" is True iff no
     uncorrectable column remains.  Radius 2 can miscorrect a column with 3 or more wrong shards (include/swec.h)."""
     arr, nd = _dirs(additional_dirs)
-    k, m, dev = (ctx.DataShards, ctx.ParityShards, ctx.device) if ctx else (0, 0, device)
-    report, ranges, n, ok = DamageReport(), (DamageRange * max(1, max_ranges))(), C.c_int(0), C.c_int(0)
-    check(lib().swec_repair_ec_damage(base_file_name.encode(), arr, nd, k, m, dev, radius, C.byref(report), ranges,
-                                      max_ranges, C.byref(n), C.byref(ok)))
-    return {"ok": bool(ok.value), **_damage_result(report, ranges, n.value, max_ranges)}
+    out, ok = _DamageOut(max_ranges), C.c_int(0)
+    check(lib().swec_repair_ec_damage(base_file_name.encode(), arr, nd, *_code(ctx, device), radius, *out.args, C.byref(ok)))
+    return {"ok": bool(ok.value), **out.result()}
 
 
 def rebuild_ec_files_checked(base_file_name: str, additional_dirs: list[str] | None = None,
@@ -477,19 +475,18 @@ def rebuild_ec_files_checked(base_file_name: str, additional_dirs: list[str] | N
     no column is uncorrectable) and the report of locate_ec_damage over the present shards.  Radius 0 only detects;
     run repair_ec_damage afterwards to fix the present shards (include/swec.h)."""
     arr, nd = _dirs(additional_dirs)
-    k, m, dev = (ctx.DataShards, ctx.ParityShards, ctx.device) if ctx else (0, 0, device)
     ids, n_ids = (C.c_uint32 * MaxShardCount)(), C.c_int(0)
-    report, ranges, n, ok = DamageReport(), (DamageRange * max(1, max_ranges))(), C.c_int(0), C.c_int(0)
-    check(lib().swec_rebuild_ec_files_checked(base_file_name.encode(), arr, nd, k, m, dev, radius, ids, C.byref(n_ids),
-                                              C.byref(report), ranges, max_ranges, C.byref(n), C.byref(ok)))
-    return {"rebuilt": list(ids[: n_ids.value]), "ok": bool(ok.value), **_damage_result(report, ranges, n.value, max_ranges)}
+    out, ok = _DamageOut(max_ranges), C.c_int(0)
+    check(lib().swec_rebuild_ec_files_checked(base_file_name.encode(), arr, nd, *_code(ctx, device), radius, ids,
+                                              C.byref(n_ids), *out.args, C.byref(ok)))
+    return {"rebuilt": list(ids[: n_ids.value]), "ok": bool(ok.value), **out.result()}
 
 
-def _check_decoded(status: int, report, ranges, n_ranges: int, max_ranges: int) -> None:
+def _check_decoded(status: int, out: _DamageOut) -> None:
     """check(), but a SWEC_ERR_UNCORRECTABLE error carries the report as .report"""
     if STATUS.get(status) == "SWEC_ERR_UNCORRECTABLE":
         err = SwecError(status, lib().swec_last_error().decode(errors="replace"))
-        err.report = _damage_result(report, ranges, n_ranges, max_ranges)
+        err.report = out.result()
         raise err
     check(status)
 
@@ -504,11 +501,10 @@ def write_dat_file_checked(base_file_name: str, dat_file_size: int, shard_file_n
     report of rebuild_ec_files_checked.  Uncorrectable columns raise SwecError(SWEC_ERR_UNCORRECTABLE), with the report
     in its .report, and leave no .dat (include/swec.h)."""
     names = (C.c_char_p * len(shard_file_names))(*[s.encode() if s else None for s in shard_file_names])
-    report, ranges, n, ok = DamageReport(), (DamageRange * max(1, max_ranges))(), C.c_int(0), C.c_int(0)
+    out, ok = _DamageOut(max_ranges), C.c_int(0)
     _check_decoded(lib().swec_write_dat_file_checked(base_file_name.encode(), dat_file_size, names, data_shards, parity_shards,
-                                                     large_block, small_block, device, radius, C.byref(report), ranges,
-                                                     max_ranges, C.byref(n), C.byref(ok)), report, ranges, n.value, max_ranges)
-    return {"dat_file_size": dat_file_size, "ok": bool(ok.value), **_damage_result(report, ranges, n.value, max_ranges)}
+                                                     large_block, small_block, device, radius, *out.args, C.byref(ok)), out)
+    return {"dat_file_size": dat_file_size, "ok": bool(ok.value), **out.result()}
 
 
 def write_dat_file(base_file_name: str, dat_file_size: int, shard_file_names: list[str],
@@ -523,6 +519,11 @@ def write_dat_file(base_file_name: str, dat_file_size: int, shard_file_names: li
 def _dirs(additional_dirs):
     dirs = [d.encode() for d in (additional_dirs or [])]
     return ((C.c_char_p * max(1, len(dirs)))(*dirs) if dirs else None), len(dirs)
+
+
+def _code(ctx: ECContext | None, device: int):
+    """(k, m, device) of a file call: the context's, or 0, 0 (the ratio from .vif, else 10+4) and `device`."""
+    return (ctx.DataShards, ctx.ParityShards, ctx.device) if ctx else (0, 0, device)
 
 
 def volume_ec_shards_generate(data_base_file_name: str, index_base_file_name: str | None = None,
@@ -562,13 +563,11 @@ def ec_shards_to_volume_checked(data_base_file_name: str, index_base_file_name: 
     write_dat_file_checked does; uncorrectable columns raise SwecError(SWEC_ERR_UNCORRECTABLE) with .report and leave
     neither .dat nor .idx, so the EC shards should be kept."""
     arr, nd = _dirs(additional_dirs)
-    size = C.c_int64(0)
-    report, ranges, n, ok = DamageReport(), (DamageRange * max(1, max_ranges))(), C.c_int(0), C.c_int(0)
+    size, out, ok = C.c_int64(0), _DamageOut(max_ranges), C.c_int(0)
     _check_decoded(lib().swec_ec_shards_to_volume_checked(data_base_file_name.encode(), (index_base_file_name or "").encode(),
-                                                          arr, nd, device, radius, C.byref(size), C.byref(report), ranges,
-                                                          max_ranges, C.byref(n), C.byref(ok)), report, ranges, n.value,
-                   max_ranges)
-    return {"dat_file_size": int(size.value), "ok": bool(ok.value), **_damage_result(report, ranges, n.value, max_ranges)}
+                                                          arr, nd, device, radius, C.byref(size), *out.args, C.byref(ok)),
+                   out)
+    return {"dat_file_size": int(size.value), "ok": bool(ok.value), **out.result()}
 
 
 def _needle_reads(needle_ids, capacity, sizes=None):
@@ -664,11 +663,11 @@ class EcVolume:
         max_needles of those with a non-zero count: needle_id, offset, size, shard_mask, damaged_bytes — a repair
         restores them — and uncorrectable_bytes — it cannot), "n_needles" and "unowned" = [damaged, uncorrectable] bytes
         that no live needle owns.  The shard files are only read."""
-        report, ranges, n, ok = DamageReport(), (DamageRange * max(1, max_ranges))(), C.c_int(0), C.c_int(0)
+        out, ok = _DamageOut(max_ranges), C.c_int(0)
         needles, n_needles, unowned = (NeedleDamage * max(1, max_needles))(), C.c_int(0), (C.c_uint64 * 2)()
-        check(lib().swec_ec_volume_locate_needle_damage(self._h, radius, C.byref(report), ranges, max_ranges, C.byref(n),
-                                                        needles, max_needles, C.byref(n_needles), unowned, C.byref(ok)))
-        return {"ok": bool(ok.value), **_damage_result(report, ranges, n.value, max_ranges),
+        check(lib().swec_ec_volume_locate_needle_damage(self._h, radius, *out.args, needles, max_needles,
+                                                        C.byref(n_needles), unowned, C.byref(ok)))
+        return {"ok": bool(ok.value), **out.result(),
                 "needles": _needle_damage(needles[:min(n_needles.value, max_needles)]), "n_needles": n_needles.value,
                 "unowned": [int(unowned[0]), int(unowned[1])]}
 
@@ -683,17 +682,16 @@ class EcVolume:
         every named needle (not only the first max_needles) checks ok: a column miscorrected beyond the guarantee of
         the code shows as a needle that does not."""
         from ._native import NeedleCheck
-        report, ranges, n, ok = DamageReport(), (DamageRange * max(1, max_ranges))(), C.c_int(0), C.c_int(0)
+        out, ok = _DamageOut(max_ranges), C.c_int(0)
         needles, n_needles, unowned = (NeedleDamage * max(1, max_needles))(), C.c_int(0), (C.c_uint64 * 2)()
         checks = (NeedleCheck * max(1, max_needles))()
-        check(lib().swec_ec_volume_repair_needle_damage(self._h, radius, C.byref(report), ranges, max_ranges, C.byref(n),
-                                                        needles, checks, max_needles, C.byref(n_needles), unowned,
-                                                        C.byref(ok)))
+        check(lib().swec_ec_volume_repair_needle_damage(self._h, radius, *out.args, needles, checks, max_needles,
+                                                        C.byref(n_needles), unowned, C.byref(ok)))
         shown = min(n_needles.value, max_needles)
         named = [{**d, "status": int(c.status), "range_index": int(c.range_index), "data_size": int(c.data_size),
                   "crc_got": int(c.crc_got), "crc_want": int(c.crc_want), "legacy_crc": int(c.legacy_crc)}
                  for d, c in zip(_needle_damage(needles[:shown]), checks[:shown])]
-        return {"ok": bool(ok.value), **_damage_result(report, ranges, n.value, max_ranges), "needles": named,
+        return {"ok": bool(ok.value), **out.result(), "needles": named,
                 "n_needles": n_needles.value, "unowned": [int(unowned[0]), int(unowned[1])]}
 
     RepairNeedleDamage = repair_needle_damage
