@@ -28,7 +28,10 @@
  *   swec_locate_sketch_damage_checked  ec.rebuild of a balanced volume (weed/shell/command_ec_rebuild.go) copies every
  *                               present shard to one rebuilder; this locates their damage from sketches first, with
  *                               the lost shards as erasures, and predicts the sketch of every rebuilt shard
- *   swec_reconstruct_batch      batched ReconstructData   weed/storage/store_ec.go:482-560 (one call per interval today)
+ *   swec_sketch_needle_damage,  ScrubEcVolume reports per needle (store_ec_scrub.go); these name the needles the
+ *   swec_ec_volume_sketch_needle_damage  sketch-located pages hit, from the .ecx alone; swec_ec_volume_page_sketch is
+ *                               the holder's sketch of its local shards under the mounted volume's lock
+ *   swec_reconstruct_batch     batched ReconstructData   weed/storage/store_ec.go:482-560 (one call per interval today)
  *   swec_write_dat_file         WriteDatFile              weed/storage/erasure_coding/ec_decoder.go:176-223
  *   swec_ec_shards_generate     VolumeEcShardsGenerate (file work)   weed/server/volume_grpc_erasure_coding.go:43-146
  *   swec_ec_shards_rebuild      VolumeEcShardsRebuild  (file work)   weed/server/volume_grpc_erasure_coding.go:149-225
@@ -498,6 +501,31 @@ int swec_locate_sketch_damage(swec_encoder *enc, const uint64_t *const *sketches
 int swec_locate_sketch_damage_checked(swec_encoder *enc, const uint64_t *const *sketches, int64_t shard_len,
                                       int radius, swec_sketch_page *pages, int64_t pages_cap, int64_t *n_flagged,
                                       uint64_t *shard_pages, uint64_t *const *rebuilt_sketches, int *ok);
+/* Which needles the pages flagged by either sketch locate call hit: the sketch-page twin of
+ * swec_locate_needle_damage_device, with its records (in/out, sized as needle version 3, a negative size owns no
+ * bytes), its encode geometry and its ownership rule.  pages[n_pages]: what the locate call returned for this
+ * shard_len (host arrays; synchronous).  Per flagged page g, columns [4096 g, min(4096 (g+1), shard_len)):
+ *   - a blamed page: every byte of every DATA shard in blamed_mask is damaged; an uncorrectable page: every byte of
+ *     all k data shards is uncorrectable.  Parity blame is never attributed.
+ *   - each such byte goes through the inverse striping to its .dat offset and is counted to the record that owns it,
+ *     whose shard_mask gets bit i; a byte no record owns (superblock, deleted records, gaps, padding) goes to
+ *     unowned[0] (damaged) or unowned[1] (uncorrectable).  So sum(damaged_bytes) + unowned[0] = the sum over blamed
+ *     pages of popcount(mask & data bits) x page length, and sum(uncorrectable_bytes) + unowned[1] = k x the sum over
+ *     uncorrectable pages of page length.
+ *   - The counts are PAGE-GRANULAR UPPER BOUNDS: a page is blamed as a whole, so every record with a byte on it is
+ *     named.  damaged: bytes on a page blamed within the radius, which fetching the page from its k+m holders and
+ *     correcting it restores (INTEGRATION.md, "Scrubbing a balanced volume", step 3).  uncorrectable: bytes the
+ *     sketches could not decide; fetching the page from all k+m shards and swec_correct_damage_device (step 4) may
+ *     still resolve them column by column.
+ * Argument rules, all before any device work (SWEC_ERR_INVALID_ARG), in this order: data_shards > 0, parity_shards > 0,
+ * total <= 32; dat_size >= 0, positive block sizes and shard_len = swec_expected_shard_size(dat_size, k, large, small);
+ * n_pages >= 0 and pages non-NULL when it is > 0; unowned not NULL and records NULL only when n_records is 0; pages
+ * strictly ascending and below ceil(shard_len/4096), uncorrectable 0 or 1, an uncorrectable page with mask 0 and a
+ * blamed page with a non-zero mask below 2^(k+m).  With n_pages = 0 the counts are zeroed and the call returns
+ * without GPU work, even for device < 0; otherwise device < 0 is SWEC_ERR_NO_DEVICE.                              */
+int swec_sketch_needle_damage(int device, int data_shards, int parity_shards, int64_t shard_len, int64_t dat_size,
+                              int64_t large_block, int64_t small_block, const swec_sketch_page *pages, int64_t n_pages,
+                              swec_needle_damage *records, int n_records, uint64_t unowned[2]);
 /* ---- checked decode: errors and erasures before the parity is dropped -----------------------------------------------
  * ec.decode deletes every shard, parity included, once the .dat is written (weed/shell/command_ec_decode.go:156-181),
  * so it is the last point at which damage in the data shards can be corrected.  swec_write_dat_file copies the data
@@ -621,6 +649,30 @@ int swec_ec_volume_scrub_needles(swec_ec_volume *vol, uint32_t volume_id, int64_
 /* What mounting derived (NewEcVolume, ec_volume.go:114-154,399-417): EC ratio and needle version from .vif (defaults
  * 10+4, version 3), the shard size LocateData works with, and a bit per shard file found locally.  Any out pointer
  * may be NULL.                                                                                                 */
+/* The holder side of a balanced scrub through the mounted volume: the page sketches (SWEC_PAGE_SKETCH_VERSION) of
+ * some of its local shards.  sketches[k+m]: a non-NULL entry asks for that shard and receives its first sketches_cap
+ * words, bit for bit what swec_page_sketch_file gives for the file; *shard_len = the shards' length, *n_pages = their
+ * pages.  The files are read through the handle's own descriptors, under its lock, so the sketches never mix pages
+ * from before and after a swec_ec_volume_repair_needle_damage on the same handle; the requested shards go through one
+ * file pipeline pass together (O_DIRECT when "file_direct_io" bit 0 is set).  Errors, before any device work:
+ * SWEC_ERR_INVALID_ARG (NULL vol, sketches, shard_len or n_pages, negative sketches_cap, no shard requested), then
+ * SWEC_ERR_TOO_FEW_SHARDS (a requested shard is not local), SWEC_ERR_SHARD_SIZE (requested shards of unequal length),
+ * then SWEC_ERR_NO_DEVICE for a handle opened with device < 0, unless the shards are empty.                      */
+int swec_ec_volume_page_sketch(swec_ec_volume *vol, uint64_t seed, uint64_t *const *sketches, int64_t sketches_cap,
+                               int64_t *shard_len, int64_t *n_pages);
+/* swec_sketch_needle_damage through the mounted volume: the coordinator, or the ScrubEcVolume handler of any holder
+ * (every holder has the .ecx), names the needles that sketch-located pages hit before a single page is fetched.  No
+ * local shard bytes are read.  Records: the live records of swec_ec_volume_locate_needle_damage (.ecx minus deleted
+ * minus .ecj, re-read when it moved), striped by the LocateData geometry (shard_dat_size, 1 GiB / 1 MiB); the counts
+ * are those of swec_sketch_needle_damage, page-granular upper bounds.  needles[] receives the records with a non-zero
+ * count in ascending needle id, the first needles_cap of them; *n_needles is how many there are.  Errors, in this
+ * order: the arguments (SWEC_ERR_INVALID_ARG: the needle rules of swec_ec_volume_locate_needle_damage, NULL vol or
+ * n_needles, negative shard_len, the page rules of swec_sketch_needle_damage); a local shard file whose length is not
+ * shard_len SWEC_ERR_SHARD_SIZE (pages of another volume); n_pages = 0 returns zero counts without GPU work; a handle
+ * opened with device < 0 SWEC_ERR_NO_DEVICE.  Nothing is written.  Calls on one handle serialise.                 */
+int swec_ec_volume_sketch_needle_damage(swec_ec_volume *vol, int64_t shard_len, const swec_sketch_page *pages,
+                                        int64_t n_pages, swec_needle_damage *needles, int needles_cap, int *n_needles,
+                                        uint64_t unowned[2]);
 int swec_ec_volume_info(swec_ec_volume *vol, int *data_shards, int *parity_shards, int *needle_version,
                         int64_t *shard_dat_size, uint32_t *local_shard_bits);
 /* EcVolume.FileAndDeleteCount (ec_volume.go:330-349): .ecx entries, distinct journalled deletions.      */

@@ -497,6 +497,83 @@ func (v *swecEcVolume) LocateNeedleDamage(radius int, maxNeedles int) (needles [
 	return needles, total, unowned, nil
 }
 
+// PageSketch answers the shard holder's side of a distributed parity scrub (a VolumeEcShardSketch RPC) for shards this
+// volume has mounted: the page sketches of the shards in shardIds, 8 bytes per 4 KiB page under the coordinator's
+// seed, all read in one pass through the volume's own descriptors and under its lock, so that a sketch never mixes
+// pages from before and after a RepairNeedleDamage.  The caller must check that the coordinator asked for
+// SWEC_PAGE_SKETCH_VERSION.  A shard that is not mounted here is an error (SWEC_ERR_TOO_FEW_SHARDS).
+func (v *swecEcVolume) PageSketch(seed uint64, shardIds []int) (sketches map[int][]uint64, shardSize int64, err error) {
+	var k, m C.int
+	var shardDatSize C.int64_t
+	if err := swecCall(func() C.int { return C.swec_ec_volume_info(v.h, &k, &m, nil, &shardDatSize, nil) }); err != nil {
+		return nil, 0, fmt.Errorf("page sketch: %w", err)
+	}
+	for _, id := range shardIds {
+		if id < 0 || id >= int(k+m) {
+			return nil, 0, fmt.Errorf("page sketch: no ec shard %d in a %d+%d volume", id, k, m)
+		}
+	}
+	ptrs := (*[C.SWEC_MAX_SHARDS]*C.uint64_t)(C.calloc(C.SWEC_MAX_SHARDS, C.size_t(unsafe.Sizeof(uintptr(0)))))
+	defer C.free(unsafe.Pointer(ptrs))
+	// a shard holds shard_dat_size bytes plus at most one small block of padding; a longer one is asked again
+	for capPages := (int64(shardDatSize) + 1<<20 + 4096) / 4096; ; {
+		var p runtime.Pinner
+		bufs := make(map[int][]uint64, len(shardIds))
+		for _, id := range shardIds {
+			bufs[id] = make([]uint64, capPages+1) // +1: never a zero-length slice to take the address of
+			p.Pin(&bufs[id][0])
+			ptrs[id] = (*C.uint64_t)(unsafe.Pointer(&bufs[id][0]))
+		}
+		var length, nPages C.int64_t
+		err := swecCall(func() C.int {
+			return C.swec_ec_volume_page_sketch(v.h, C.uint64_t(seed), &ptrs[0], C.int64_t(capPages), &length, &nPages)
+		})
+		p.Unpin()
+		if err != nil {
+			return nil, 0, fmt.Errorf("page sketch: %w", err)
+		}
+		if int64(nPages) <= capPages {
+			for id, b := range bufs {
+				bufs[id] = b[:nPages]
+			}
+			return bufs, int64(length), nil
+		}
+		capPages = int64(nPages)
+	}
+}
+
+// SketchNeedleDamage names the live needles that the pages swecLocateSketchDamage (or its checked twin) flagged hit, from
+// this volume's .ecx alone: any holder's ScrubEcVolume handler can report per needle before a single page is fetched.
+// needles are in ascending id, at most maxNeedles of them (total is how many there are); unowned are the damaged /
+// uncorrectable bytes no live needle owns.  The counts are page-granular upper bounds: every needle with a byte on a
+// flagged page is named.  shardSize is the holders' shard size; a mounted shard of another size is an error.
+func (v *swecEcVolume) SketchNeedleDamage(pages []swecSketchPage, shardSize int64, maxNeedles int) (needles []swecNeedleDamage, total int, unowned [2]uint64, err error) {
+	in := make([]C.swec_sketch_page, len(pages)+1)
+	for i, q := range pages {
+		in[i].page, in[i].blamed_mask = C.int64_t(q.Page), C.uint32_t(q.Blamed)
+		if q.Uncorrectable {
+			in[i].uncorrectable = 1
+		}
+	}
+	var nNeedles C.int
+	var cUnowned [2]C.uint64_t
+	buf := make([]C.swec_needle_damage, maxNeedles+1)
+	if err := swecCall(func() C.int {
+		return C.swec_ec_volume_sketch_needle_damage(v.h, C.int64_t(shardSize), &in[0], C.int64_t(len(pages)), &buf[0],
+			C.int(maxNeedles), &nNeedles, &cUnowned[0])
+	}); err != nil {
+		return nil, 0, unowned, fmt.Errorf("sketch needle damage: %w", err)
+	}
+	total = int(nNeedles)
+	for i := 0; i < total && i < maxNeedles; i++ {
+		d := buf[i]
+		needles = append(needles, swecNeedleDamage{uint64(d.needle_id), int64(d.offset), int32(d.size), uint32(d.shard_mask),
+			uint64(d.damaged_bytes), uint64(d.uncorrectable_bytes)})
+	}
+	unowned = [2]uint64{uint64(cUnowned[0]), uint64(cUnowned[1])}
+	return needles, total, unowned, nil
+}
+
 // swecNeedleRepair is a needle RepairNeedleDamage touched, and how it reads back from the repaired files: Status 0 means
 // Needle.ReadBytes accepts it (size, layout and CRC32-C); any other status (1 size mismatch, 2 out of range, 3 bad CRC,
 // 4 past the end of its shard) means the needle has to come from a replica or a backup.

@@ -151,6 +151,14 @@ PROTOTYPES = {
     "swec_locate_sketch_damage_checked": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.POINTER(SketchPage),
                                                     C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_uint64), C.c_void_p,
                                                     C.POINTER(C.c_int)]),
+    "swec_sketch_needle_damage": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
+                                            C.POINTER(SketchPage), C.c_int64, C.POINTER(NeedleDamage), C.c_int,
+                                            C.POINTER(C.c_uint64)]),
+    "swec_ec_volume_page_sketch": (C.c_int, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_int64, C.POINTER(C.c_int64),
+                                             C.POINTER(C.c_int64)]),
+    "swec_ec_volume_sketch_needle_damage": (C.c_int, [C.c_void_p, C.c_int64, C.POINTER(SketchPage), C.c_int64,
+                                                      C.POINTER(NeedleDamage), C.c_int, C.POINTER(C.c_int),
+                                                      C.POINTER(C.c_uint64)]),
     "swec_write_dat_file": (C.c_int, [C.c_char_p, C.c_int64, C.c_void_p, C.c_int, C.c_int64, C.c_int64]),
     "swec_write_dat_file_checked": (C.c_int, [C.c_char_p, C.c_int64, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_int64,
                                               C.c_int, C.c_int, C.POINTER(DamageReport), C.POINTER(DamageRange), C.c_int,

@@ -961,6 +961,46 @@ int needle_damage_files(swec_encoder* enc, const std::vector<int>& in, int64_t s
     return nd.collect(recs->data(), unowned);
 }
 
+// One pipeline pass over every file: one stored stream per file read per slot and no matrix, and the step sketches
+// every stream of the slot.  Items start on page boundaries, so their sketches concatenate.  The O_DIRECT twins
+// ("file_direct_io" bit 0) are the same inodes opened again through /proc/self/fd.
+int page_sketch_files(swec_encoder* enc, const std::vector<int>& fds, int64_t size, uint64_t seed,
+                      uint64_t* const* out, int64_t cap) {
+    const int n = int(fds.size());
+    const size_t pages = size_t((size + 4095) / 4096);
+    FdSet twins;
+    std::vector<int> dfds;
+    for (int fd : fds)
+        dfds.push_back(twins.keep(open_direct("/proc/self/fd/" + std::to_string(fd), O_RDONLY,
+                                              g_opt_file_direct_io.load() & 1)));
+    int rc = enc->ensure_device();
+    if (rc) return rc;
+    DeviceBuffer dev;  // declared before the pipeline: freed after its shutdown has drained every slot
+    SWEC_CUDA(dev.alloc(size_t(n) * pages * 8));
+    const size_t chunk = (file_chunk(size) + 4095) & ~size_t(4095);
+    FilePipeline pipe(enc, Matrix(0, 0), chunk, n, [&](uint8_t* const*, uint8_t* const* shards, size_t len,
+                                                       int64_t base, int, cudaStream_t s) -> int {
+        for (int j = 0; j < n; j++)
+            SWEC_CUDA(launch_page_sketch(shards[j], len, u64(base), seed,
+                                         dev.as<u64>() + size_t(j) * pages + size_t(base) / 4096, s));
+        return SWEC_OK;
+    });
+    if ((rc = pipe.start())) return rc;
+    for (int64_t o = 0; o < size; o += int64_t(chunk)) {
+        Item it;
+        it.len = size_t(std::min<int64_t>(int64_t(chunk), size - o));
+        it.shard_off = o;
+        for (int j = 0; j < n; j++) it.reads.push_back({j, fds[size_t(j)], o, 0, it.len, dfds[size_t(j)]});
+        if (pipe.submit(std::move(it))) break;
+    }
+    if ((rc = pipe.finish())) return rc;
+    pipe.report("page_sketch");
+    const size_t words = size_t(std::min<int64_t>(cap, int64_t(pages)));
+    for (int j = 0; j < n && words; j++)
+        if (out[j]) SWEC_CUDA(cudaMemcpy(out[j], dev.as<u64>() + size_t(j) * pages, words * 8, cudaMemcpyDeviceToHost));
+    return SWEC_OK;
+}
+
 }  // namespace swec
 
 extern "C" {
@@ -1113,37 +1153,14 @@ int swec_page_sketch_file(const char* path, int device, uint64_t seed, uint64_t*
     if (fd < 0) return io_fail(std::string("open ") + path);
     struct stat st;
     if (fstat(fd, &st) != 0) return io_fail(std::string("stat ") + path);
-    const int64_t size = int64_t(st.st_size), pages = (size + 4095) / 4096;
+    const int64_t size = int64_t(st.st_size);
     if (size > 0) {
-        // one stream read per slot and no matrix: the step sketches it; items start on page boundaries
         CallEncoder enc;
         int rc = new_call_encoder(1, 1, device, &enc);
-        if (rc) return rc;
-        const int dfd = fds.keep(open_direct(path, O_RDONLY, g_opt_file_direct_io.load() & 1));
-        if ((rc = enc->ensure_device())) return rc;
-        DeviceBuffer dev;  // declared before the pipeline: freed after its shutdown has drained every slot
-        SWEC_CUDA(dev.alloc(size_t(pages) * 8));
-        const size_t chunk = (file_chunk(size) + 4095) & ~size_t(4095);
-        FilePipeline pipe(enc.get(), Matrix(0, 0), chunk, 1, [&](uint8_t* const*, uint8_t* const* shards, size_t len,
-                                                                 int64_t base, int, cudaStream_t s) -> int {
-            SWEC_CUDA(launch_page_sketch(shards[0], len, u64(base), seed, dev.as<u64>() + base / 4096, s));
-            return SWEC_OK;
-        });
-        if ((rc = pipe.start())) return rc;
-        for (int64_t o = 0; o < size; o += int64_t(chunk)) {
-            Item it;
-            it.len = size_t(std::min<int64_t>(int64_t(chunk), size - o));
-            it.shard_off = o;
-            it.reads.push_back({0, fd, o, 0, it.len, dfd});
-            if (pipe.submit(std::move(it))) break;
-        }
-        if ((rc = pipe.finish())) return rc;
-        pipe.report("page_sketch");
-        if (const int64_t n = std::min(sketches_cap, pages))
-            SWEC_CUDA(cudaMemcpy(sketches, dev.as<u64>(), size_t(n) * 8, cudaMemcpyDeviceToHost));
+        if (rc || (rc = page_sketch_files(enc.get(), {fd}, size, seed, &sketches, sketches_cap))) return rc;
     }
     *shard_len = size;
-    *n_pages = pages;
+    *n_pages = (size + 4095) / 4096;
     return SWEC_OK;
 }
 

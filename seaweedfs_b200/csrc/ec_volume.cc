@@ -33,6 +33,7 @@
 #include "engine.h"
 #include "needle_damage.h"
 #include "needles.h"
+#include "sketch.h"
 #include "volume_format.h"
 
 namespace swec {
@@ -705,6 +706,35 @@ int recheck_needles(swec_ec_volume* v, const std::vector<swec_needle_damage>& na
     return SWEC_OK;
 }
 
+// The live records as the handle's reads see them: .ecx entries that are not deleted, minus the journalled ids
+// (FindNeedleFromEcx, ec_volume.go:419-429), the journal re-read when it moved.  Under v->mu.
+std::vector<swec_needle_damage> live_records(swec_ec_volume* v) {
+    v->refresh_journal();
+    std::vector<swec_needle_damage> recs;
+    for (int64_t e = 0; e < v->entries(); e++) {
+        const IndexEntry x = v->entry(e);
+        if (size_deleted(x.size) || v->journalled(x.key)) continue;
+        swec_needle_damage r{};
+        r.needle_id = x.key;
+        r.offset = x.offset;
+        r.size = x.size;
+        recs.push_back(r);
+    }
+    return recs;
+}
+
+// The named needles of the handle calls: the records with a non-zero count, in ascending needle id, left in *recs; the
+// first needles_cap of them to needles[], how many there are to *n_needles.
+void name_needles(std::vector<swec_needle_damage>* recs, swec_needle_damage* needles, int needles_cap, int* n_needles) {
+    std::stable_sort(recs->begin(), recs->end(),
+                     [](const swec_needle_damage& a, const swec_needle_damage& b) { return a.needle_id < b.needle_id; });
+    recs->erase(std::remove_if(recs->begin(), recs->end(),
+                               [](const swec_needle_damage& r) { return !r.damaged_bytes && !r.uncorrectable_bytes; }),
+                recs->end());
+    for (int j = 0; j < needles_cap && j < int(recs->size()); j++) needles[j] = (*recs)[size_t(j)];
+    *n_needles = int(recs->size());
+}
+
 // Both needle damage calls on the handle (include/swec.h): every check before any device work, the live records as the
 // reads see them, then pass 1 and, with damage, pass 2 (needle_damage_files).  With `checks` (the repair), pass 2 also
 // writes the corrections, and every named needle is re-checked from the repaired files.
@@ -729,29 +759,12 @@ int handle_needle_damage(swec_ec_volume* v, int radius, const DamageOut& out, sw
     for (int i = 0; i < total; i++)
         if ((rc = check_length(v->shard_fd[size_t(i)], &size))) return rc;
     if (v->device < 0) return fail(SWEC_ERR_NO_DEVICE, "no CUDA device: the volume was opened with device < 0");
-    // live records: .ecx entries that are not deleted, minus the journalled ids (FindNeedleFromEcx, ec_volume.go:419-429)
-    v->refresh_journal();
-    std::vector<swec_needle_damage> recs;
-    for (int64_t e = 0; e < v->entries(); e++) {
-        const IndexEntry x = v->entry(e);
-        if (size_deleted(x.size) || v->journalled(x.key)) continue;
-        swec_needle_damage r{};
-        r.needle_id = x.key;
-        r.offset = x.offset;
-        r.size = x.size;
-        recs.push_back(r);
-    }
+    std::vector<swec_needle_damage> recs = live_records(v);
     if (!v->enc && (rc = swec_encoder_new(v->k, v->m, v->device, &v->enc))) return rc;
     const StripeMap map = StripeMap::locate(v->shard_dat_size, v->k, kLargeBlockSize, kSmallBlockSize);
     if ((rc = needle_damage_files(v->enc, v->shard_fd, size, radius, map, v->version, repair, &recs, out, unowned)))
         return rc;
-    std::stable_sort(recs.begin(), recs.end(),
-                     [](const swec_needle_damage& a, const swec_needle_damage& b) { return a.needle_id < b.needle_id; });
-    recs.erase(std::remove_if(recs.begin(), recs.end(),
-                              [](const swec_needle_damage& r) { return !r.damaged_bytes && !r.uncorrectable_bytes; }),
-               recs.end());
-    for (int j = 0; j < needles_cap && j < int(recs.size()); j++) needles[j] = recs[size_t(j)];
-    *n_needles = int(recs.size());
+    name_needles(&recs, needles, needles_cap, n_needles);
     if (!repair) {
         *ok = out.report->damaged_columns == 0 ? 1 : 0;
         return SWEC_OK;
@@ -814,6 +827,62 @@ int swec_ec_volume_repair_needle_damage(swec_ec_volume* v, int radius, swec_dama
                                         int* ok) {
     return handle_needle_damage(v, radius, {report, ranges, ranges_cap, n_ranges}, needles, true, checks, needles_cap,
                                 n_needles, unowned, ok);
+}
+
+int swec_ec_volume_sketch_needle_damage(swec_ec_volume* v, int64_t shard_len, const swec_sketch_page* pages,
+                                        int64_t n_pages, swec_needle_damage* needles, int needles_cap, int* n_needles,
+                                        uint64_t unowned[2]) {
+    int rc = check_needle_damage_args(needles_cap, needles, unowned, 0, nullptr);
+    if (rc) return rc;
+    if (!v || !n_needles) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
+    if (shard_len < 0) return fail(SWEC_ERR_INVALID_ARG, "shard_len must be >= 0");
+    if (n_pages < 0 || (n_pages > 0 && !pages))
+        return fail(SWEC_ERR_INVALID_ARG, "n_pages must be >= 0, and pages non-NULL when it is > 0");
+    std::lock_guard<std::mutex> lock(v->mu);
+    if ((rc = check_sketch_pages(v->k, v->m, shard_len, pages, n_pages))) return rc;
+    *n_needles = 0;
+    unowned[0] = unowned[1] = 0;
+    for (int fd : v->shard_fd) {  // a local shard of another length: the pages are not of this volume
+        int64_t size = shard_len;
+        if (fd >= 0 && (rc = check_length(fd, &size))) return rc;
+    }
+    if (n_pages == 0) return SWEC_OK;
+    if (v->device < 0) return fail(SWEC_ERR_NO_DEVICE, "no CUDA device: the volume was opened with device < 0");
+    std::vector<swec_needle_damage> recs = live_records(v);
+    const StripeMap map = StripeMap::locate(v->shard_dat_size, v->k, kLargeBlockSize, kSmallBlockSize);
+    if ((rc = sketch_needle_damage(v->device, map, shard_len, pages, n_pages, recs.data(), int(recs.size()), v->version,
+                                   unowned)))
+        return rc;
+    name_needles(&recs, needles, needles_cap, n_needles);
+    return SWEC_OK;
+}
+
+int swec_ec_volume_page_sketch(swec_ec_volume* v, uint64_t seed, uint64_t* const* sketches, int64_t sketches_cap,
+                               int64_t* shard_len, int64_t* n_pages) {
+    if (!v || !sketches || !shard_len || !n_pages) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
+    if (sketches_cap < 0) return fail(SWEC_ERR_INVALID_ARG, "sketches_cap must be >= 0");
+    std::lock_guard<std::mutex> lock(v->mu);
+    std::vector<int> fds;
+    std::vector<uint64_t*> out;
+    for (int i = 0; i < v->k + v->m; i++) {
+        if (!sketches[i]) continue;
+        if (v->shard_fd[size_t(i)] < 0) return fail(SWEC_ERR_TOO_FEW_SHARDS, "shard " + shard_ext(i) + " is not local");
+        fds.push_back(v->shard_fd[size_t(i)]);
+        out.push_back(sketches[i]);
+    }
+    if (fds.empty()) return fail(SWEC_ERR_INVALID_ARG, "no shard requested: every sketches entry is NULL");
+    int64_t size = -1;
+    int rc;
+    for (int fd : fds)
+        if ((rc = check_length(fd, &size))) return rc;
+    if (size > 0) {
+        if (v->device < 0) return fail(SWEC_ERR_NO_DEVICE, "no CUDA device: the volume was opened with device < 0");
+        if (!v->enc && (rc = swec_encoder_new(v->k, v->m, v->device, &v->enc))) return rc;
+        if ((rc = page_sketch_files(v->enc, fds, size, seed, out.data(), sketches_cap))) return rc;
+    }
+    *shard_len = size;
+    *n_pages = (size + 4095) / 4096;
+    return SWEC_OK;
 }
 
 // FileAndDeleteCount (ec_volume.go:330-349): entries of the sealed .ecx, and distinct journalled ids.

@@ -5,8 +5,9 @@
 //                         zero: every column the correcting locate decoded within the radius is a codeword again.  A
 //                         data byte is damaged when the correcting locate changed it: a blamed byte always changes,
 //                         because its error value is not zero.  Each such byte of data shard i is mapped to its .dat
-//                         offset (stripe_map.h), the live records (sorted by offset) are binary-searched for its owner,
-//                         and the owner's counters and shard mask, or the unowned counters, take it with atomics.
+//                         offset (stripe_map.h), its owner among the live records is found by the ownership rule
+//                         (RecordTally, needle_damage.h), and the owner's counters and shard mask, or the unowned
+//                         counters, take it with atomics.
 // The locate kernel itself (damage.cu) is not changed: pass 2 runs its correcting instantiation on a copy.
 #include <cuda_runtime.h>
 
@@ -31,14 +32,9 @@ struct AttributeParams {
     const u8* stored[SWEC_MAX_SHARDS];  // parity after the correcting locate
     u64 n;
     int64_t base;
-    int k, m, nrec;
+    int k, m;
     StripeMap map;
-    const int64_t* off;  // record offsets, ascending
-    const int64_t* end;
-    unsigned long long* damaged;        // [nrec]
-    unsigned long long* uncorrectable;  // [nrec]
-    unsigned long long* unowned;        // [2]
-    unsigned* mask;                     // [nrec]
+    RecordTally t;
 };
 
 __global__ void __launch_bounds__(256) nd_attribute_kernel(const __grid_constant__ AttributeParams p) {
@@ -49,23 +45,13 @@ __global__ void __launch_bounds__(256) nd_attribute_kernel(const __grid_constant
         for (int i = 0; i < p.k; i++) {
             if (!residual && p.orig[i][x] == p.fixed[i][x]) continue;
             const int kind = residual ? 1 : 0;
-            const int64_t d = p.map.dat_offset(i, p.base + int64_t(x));
-            int owner = -1;
-            if (d >= 0) {  // the last record whose offset is not above d
-                int lo = 0, hi = p.nrec;
-                while (lo < hi) {
-                    const int mid = (lo + hi) >> 1;
-                    if (p.off[mid] <= d) lo = mid + 1;
-                    else hi = mid;
-                }
-                if (lo > 0 && d < p.end[lo - 1]) owner = lo - 1;
-            }
+            const int owner = p.t.owner(p.map.dat_offset(i, p.base + int64_t(x)));
             if (owner < 0) {
-                atomicAdd(p.unowned + kind, 1ull);
+                atomicAdd(p.t.unowned + kind, 1ull);
                 continue;
             }
-            atomicAdd((kind ? p.uncorrectable : p.damaged) + owner, 1ull);
-            atomicOr(p.mask + owner, 1u << i);
+            atomicAdd((kind ? p.t.uncorrectable : p.t.damaged) + owner, 1ull);
+            atomicOr(p.t.mask + owner, 1u << i);
         }
     }
 }
@@ -132,17 +118,23 @@ int NeedleDamage::launch(const uint8_t* const* orig, uint8_t* const* fixed, uint
     p.base = base;
     p.k = k_;
     p.m = m_;
-    p.nrec = n_;
     p.map = map_;
-    p.off = spans_.as<int64_t>();
-    p.end = p.off + n_;
-    p.damaged = counters_.as<unsigned long long>();
-    p.uncorrectable = p.damaged + n_;
-    p.unowned = p.damaged + 2 * n_;
-    p.mask = masks_.as<unsigned>();
+    p.t = tally();
     nd_attribute_kernel<<<grid_for(len, 256, 8), 256, 0, s>>>(p);
     SWEC_CUDA(launched());
     return SWEC_OK;
+}
+
+RecordTally NeedleDamage::tally() const {
+    RecordTally t;
+    t.off = spans_.as<int64_t>();
+    t.end = t.off + n_;
+    t.n = n_;
+    t.damaged = counters_.as<unsigned long long>();
+    t.uncorrectable = t.damaged + n_;
+    t.unowned = t.damaged + 2 * n_;
+    t.mask = masks_.as<unsigned>();
+    return t;
 }
 
 int NeedleDamage::collect(swec_needle_damage* recs, uint64_t unowned[2]) {

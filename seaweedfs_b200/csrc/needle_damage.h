@@ -23,6 +23,44 @@ namespace swec {
 int check_needle_damage_args(int needles_cap, const swec_needle_damage* needles, const uint64_t* unowned,
                              int n_records, const swec_needle_damage* records);
 
+// The live records in device memory, sorted by offset, and their counters: what the attribution kernels add to
+// (needle_damage.cu per byte, sketch.cu per run of a flagged page).  The ownership rule lives here alone: a .dat byte
+// belongs to the record with the greatest offset not above it (the later entry on a tie) when it lies inside it.
+struct RecordTally {
+    const int64_t* off;  // [n], ascending
+    const int64_t* end;  // [n]
+    int n;
+    unsigned long long* damaged;        // [n]
+    unsigned long long* uncorrectable;  // [n]
+    unsigned long long* unowned;        // [2]
+    unsigned* mask;                     // [n]
+
+    // the last record whose offset is not above d, or -1: the only one that can own d
+    SWEC_HD int candidate(int64_t d) const {
+        int lo = 0, hi = n;
+        while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (off[mid] <= d) lo = mid + 1;
+            else hi = mid;
+        }
+        return lo - 1;
+    }
+    // the record that owns .dat offset d (-1 for none, and for padding, d < 0)
+    SWEC_HD int owner(int64_t d) const {
+        if (d < 0) return -1;
+        const int p = candidate(d);
+        return p >= 0 && d < end[p] ? p : -1;
+    }
+    // how many bytes of [lo, hi) record p owns, p = candidate(x) for some x in [lo, hi): the candidate of a byte
+    // stays p up to the next record's offset
+    SWEC_HD int64_t owned(int p, int64_t lo, int64_t hi) const {
+        int64_t stop = end[p] < hi ? end[p] : hi;
+        if (p + 1 < n && off[p + 1] < stop) stop = off[p + 1];
+        const int64_t start = off[p] > lo ? off[p] : lo;
+        return stop > start ? stop - start : 0;
+    }
+};
+
 class NeedleDamage {
   public:
     NeedleDamage() = default;
@@ -43,6 +81,8 @@ class NeedleDamage {
                int slot, cudaStream_t s);
     // after every launch has completed: shard_mask, damaged_bytes and uncorrectable_bytes of recs[n] (init's order)
     int collect(swec_needle_damage* recs, uint64_t unowned[2]);
+    // the sorted records and counters, for a kernel of another translation unit (sketch.cu); after init
+    RecordTally tally() const;
 
   private:
     int k_ = 0, m_ = 0, n_ = 0;

@@ -10,6 +10,12 @@
 //                             shards (damage.h): one thread per page, the 8 bytes of its sketch syndromes decoded as 8
 //                             columns by the locate kernels' decoder (locate_decode.cuh), their blame merged per page,
 //                             and the located errors of information shards taken out of the lost shards' sketches.
+//   swec_sketch_attribute_kernel  the needles that flagged pages hit: one thread per (flagged page, data shard), which
+//                             cuts the page's columns of that shard into runs of consecutive .dat offsets (one run
+//                             when both block sizes are multiples of 4096), binary-searches each run's first candidate
+//                             record and walks the offset-sorted records forward, one atomic per (record, run).  Work
+//                             grows with the records a page overlaps, not with its 4096 bytes: a whole 3 GiB shard
+//                             flagged is 786,432 threads, not 3.2 G byte lookups.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -21,6 +27,7 @@
 #include "device_common.cuh"
 #include "engine.h"
 #include "locate_decode.cuh"
+#include "needle_damage.h"
 #include "sketch.h"
 
 namespace swec {
@@ -266,7 +273,100 @@ int locate_sketches(swec_encoder* e, const CheckedPlan& plan, const uint64_t* co
     return SWEC_OK;
 }
 
+struct SketchAttributeParams {
+    const swec_sketch_page* pages;  // flagged pages, ascending
+    u64 n_pages;
+    int64_t shard_len;
+    StripeMap map;
+    RecordTally t;
+};
+
+// One thread per (flagged page, data shard i), grid-stride.  A blamed page counts the columns of the data shards in its
+// mask as damaged, an uncorrectable one the columns of all k data shards as uncorrectable; parity blame is never
+// attributed.  Each block run of the page goes to its records by the ownership rule (RecordTally::owned), and the
+// bytes no record owns, padding included, to the unowned counter of the kind, once per thread.
+__global__ void __launch_bounds__(256) swec_sketch_attribute_kernel(const __grid_constant__ SketchAttributeParams p) {
+    const u64 k = u64(p.map.k), total = p.n_pages * k;
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 w = (u64)blockIdx.x * blockDim.x + threadIdx.x; w < total; w += stride) {
+        const u64 j = w / k;
+        const int i = int(w - j * k);
+        const swec_sketch_page pg = p.pages[j];
+        const int kind = pg.uncorrectable ? 1 : 0;
+        if (!kind && !((pg.blamed_mask >> i) & 1u)) continue;
+        const int64_t lo = pg.page * int64_t(kPage), hi = min(lo + int64_t(kPage), p.shard_len);
+        unsigned long long lost = 0;
+        for (int64_t x = lo; x < hi;) {
+            const int64_t stop = min(hi, p.map.block_end(x));
+            const int64_t d0 = p.map.dat_offset(i, x);  // -1: the whole run is padding
+            const int64_t len = stop - x;
+            x = stop;
+            if (d0 < 0) {
+                lost += u64(len);
+                continue;
+            }
+            const int64_t d1 = min(d0 + len, p.map.dat_end);
+            int64_t got = 0;
+            for (int q = max(p.t.candidate(d0), 0); q < p.t.n && p.t.off[q] < d1; q++) {
+                const int64_t o = p.t.owned(q, d0, d1);
+                if (!o) continue;
+                atomicAdd((kind ? p.t.uncorrectable : p.t.damaged) + q, (unsigned long long)o);
+                atomicOr(p.t.mask + q, 1u << i);
+                got += o;
+            }
+            lost += u64(len - got);
+        }
+        if (lost) atomicAdd(p.t.unowned + kind, lost);
+    }
+}
+
 }  // namespace
+
+int check_sketch_pages(int k, int m, int64_t shard_len, const swec_sketch_page* pages, int64_t n_pages) {
+    const int64_t limit = (shard_len + int64_t(kPage) - 1) / int64_t(kPage);
+    const uint64_t shards = (uint64_t(1) << (k + m)) - 1;
+    for (int64_t j = 0; j < n_pages; j++) {
+        const swec_sketch_page& pg = pages[j];
+        const std::string at = "pages[" + std::to_string(j) + "]";
+        if (pg.page < 0 || pg.page >= limit || (j > 0 && pg.page <= pages[j - 1].page))
+            return fail(SWEC_ERR_INVALID_ARG, at + ": pages must be strictly ascending and below ceil(shard_len/4096)");
+        if (pg.uncorrectable != 0 && pg.uncorrectable != 1)
+            return fail(SWEC_ERR_INVALID_ARG, at + ": uncorrectable must be 0 or 1");
+        if (pg.uncorrectable ? pg.blamed_mask != 0 : (pg.blamed_mask == 0 || (pg.blamed_mask & ~shards)))
+            return fail(SWEC_ERR_INVALID_ARG, at + ": an uncorrectable page has mask 0, a blamed page a non-zero mask "
+                                                   "of the k+m shards");
+    }
+    return SWEC_OK;
+}
+
+int sketch_needle_damage(int device, const StripeMap& map, int64_t shard_len, const swec_sketch_page* pages,
+                         int64_t n_pages, swec_needle_damage* recs, int n, int version, uint64_t unowned[2]) {
+    SWEC_CUDA(cudaSetDevice(device));
+    cudaStream_t s = cudaStreamPerThread;
+    NeedleDamage nd;
+    if (int rc = nd.init(map.k, 0, map, recs, n, version, 0, 0, s)) return rc;
+    DeviceBuffer flagged;
+    SWEC_CUDA(flagged.upload(pages, size_t(n_pages), s));
+    SketchAttributeParams p;
+    memset(&p, 0, sizeof p);
+    p.pages = flagged.as<swec_sketch_page>();
+    p.n_pages = u64(n_pages);
+    p.shard_len = shard_len;
+    p.map = map;
+    p.t = nd.tally();
+    static const int per_sm = [] {
+        int c = 0;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, swec_sketch_attribute_kernel, 256, 0) != cudaSuccess) {
+            cudaGetLastError();
+            c = 4;
+        }
+        return std::max(1, c);
+    }();
+    swec_sketch_attribute_kernel<<<grid_for(u64(n_pages) * u64(map.k), 256, per_sm), 256, 0, s>>>(p);
+    SWEC_CUDA(launched());
+    SWEC_CUDA(cudaStreamSynchronize(s));
+    return nd.collect(recs, unowned);
+}
 
 cudaError_t launch_page_sketch(const void* shard, u64 n, u64 first_column, u64 seed, u64* sketches, cudaStream_t s) {
     if (n == 0) return cudaSuccess;
@@ -333,6 +433,33 @@ int swec_locate_sketch_damage_checked(swec_encoder* e, const uint64_t* const* sk
         return fail(SWEC_ERR_TOO_FEW_SHARDS, "fewer than data_shards sketches present");
     return locate_sketches(e, plan, sketches, shard_len, radius, pages, pages_cap, n_flagged, shard_pages,
                            rebuilt_sketches, ok);
+}
+
+int swec_sketch_needle_damage(int device, int k, int m, int64_t shard_len, int64_t dat_size, int64_t large,
+                              int64_t small, const swec_sketch_page* pages, int64_t n_pages, swec_needle_damage* records,
+                              int n_records, uint64_t unowned[2]) {
+    if (k <= 0 || m <= 0 || k + m > SWEC_MAX_SHARDS)
+        return fail(SWEC_ERR_INVALID_ARG, "need data_shards > 0, parity_shards > 0, total <= 32");
+    if (dat_size < 0 || large <= 0 || small <= 0) return fail(SWEC_ERR_INVALID_ARG, "bad geometry");
+    if (shard_len != swec_expected_shard_size(dat_size, k, large, small))
+        return fail(SWEC_ERR_INVALID_ARG, "shard_len " + std::to_string(shard_len) + " is not the shard size " +
+                                              std::to_string(swec_expected_shard_size(dat_size, k, large, small)) +
+                                              " of the geometry");
+    if (n_pages < 0 || (n_pages > 0 && !pages))
+        return fail(SWEC_ERR_INVALID_ARG, "n_pages must be >= 0, and pages non-NULL when it is > 0");
+    int rc = check_needle_damage_args(0, nullptr, unowned, n_records, records);
+    if (rc || (rc = check_sketch_pages(k, m, shard_len, pages, n_pages))) return rc;
+    if (n_pages == 0) {
+        for (int j = 0; j < n_records; j++) {
+            records[j].shard_mask = 0;
+            records[j].damaged_bytes = records[j].uncorrectable_bytes = 0;
+        }
+        unowned[0] = unowned[1] = 0;
+        return SWEC_OK;
+    }
+    if (device < 0) return fail(SWEC_ERR_NO_DEVICE, "device < 0; no CPU fallback exists");
+    return sketch_needle_damage(device, StripeMap::encode(dat_size, k, large, small), shard_len, pages, n_pages, records,
+                                n_records, 3, unowned);
 }
 
 }  // extern "C"

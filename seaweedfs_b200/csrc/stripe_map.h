@@ -6,7 +6,8 @@
 //            anything past it, is no .dat byte at all
 //   locate   the striping LocateData reads (ec_locate.go:16-98, swec_locate_data): shard_dat_size / large rows of
 //            large blocks, then small rows without end
-// needle_damage.cu maps located bytes to needles with it; the host only builds the map.
+// needle_damage.cu maps located bytes to needles with it, sketch.cu the runs of flagged pages; the host only builds
+// the map.
 #pragma once
 #include <cstdint>
 
@@ -38,6 +39,14 @@ struct StripeMap {
             d = large_bytes * k + (y / small) * small * k + int64_t(i) * small + y % small;
         }
         return d < dat_end ? d : -1;
+    }
+
+    // the shard offset where the block holding shard offset x ends: in every data shard, the bytes [x, block_end(x))
+    // have consecutive .dat offsets (until those reach dat_end)
+    SWEC_HD int64_t block_end(int64_t x) const {
+        const int64_t large_bytes = large_rows * large;
+        if (x < large_bytes) return (x / large + 1) * large;
+        return large_bytes + ((x - large_bytes) / small + 1) * small;
     }
 };
 

@@ -413,6 +413,34 @@ def page_sketch_file(path: str, seed: int, device: int = 0) -> tuple[np.ndarray,
         cap = n.value
 
 
+def _sketch_pages(pages):
+    """The ctypes array of a "pages" list [(page, blamed mask, uncorrectable)] of the sketch locate calls, and its length."""
+    pages = list(pages)
+    arr = (SketchPage * max(1, len(pages)))()
+    for a, (g, mask, unc) in zip(arr, pages):
+        a.page, a.blamed_mask, a.uncorrectable = g, mask, int(unc)
+    return arr, len(pages)
+
+
+def sketch_needle_damage(pages, shard_len: int, dat_size: int, records, data_shards: int = DataShardsCount,
+                         parity_shards: int = ParityShardsCount, large_block: int = ErasureCodingLargeBlockSize,
+                         small_block: int = ErasureCodingSmallBlockSize, device: int = 0) -> dict:
+    """Which records the pages flagged by Encoder.locate_sketch_damage[_checked] hit (swec_sketch_needle_damage), for
+    shards of the volume image of dat_size bytes striped with large_block / small_block (shard_len must be its shard
+    size).  records: (needle_id, offset, size) of every live record, sized as needle version 3.  Returns "needles" (one
+    dict per record, in order, zero counts included) and "unowned" = [damaged, uncorrectable].  The counts are
+    page-granular upper bounds (include/swec.h)."""
+    arr, n_pages = _sketch_pages(pages)
+    records = list(records)
+    recs = (NeedleDamage * max(1, len(records)))()
+    for r, (nid, off, size) in zip(recs, records):
+        r.needle_id, r.offset, r.size = nid, off, size
+    unowned = (C.c_uint64 * 2)()
+    check(lib().swec_sketch_needle_damage(device, data_shards, parity_shards, shard_len, dat_size, large_block,
+                                          small_block, arr, n_pages, recs, len(records), unowned))
+    return {"needles": _needle_damage(recs[:len(records)]), "unowned": [int(unowned[0]), int(unowned[1])]}
+
+
 def _sketch_result(ok, n, pages, per_shard) -> dict:
     return {"ok": bool(ok.value), "n_flagged": int(n.value),
             "pages": [(int(p.page), int(p.blamed_mask), bool(p.uncorrectable)) for p in pages[:n.value]],
@@ -695,6 +723,37 @@ class EcVolume:
                 "n_needles": n_needles.value, "unowned": [int(unowned[0]), int(unowned[1])]}
 
     RepairNeedleDamage = repair_needle_damage
+
+    def page_sketch(self, seed: int, shards=None) -> tuple[dict, int]:
+        """The page sketches of local shards, read through the handle under its lock so that they never overlap a
+        repair through it (swec_ec_volume_page_sketch): ({shard id: uint64 array of ceil(len / 4096) words}, len).
+        shards: the shard ids to sketch (None: every local shard), all in one file pipeline pass."""
+        info = self.info()
+        ids = info["local_shards"] if shards is None else list(shards)
+        total = info["data_shards"] + info["parity_shards"]
+        cap = (info["shard_dat_size"] + ErasureCodingSmallBlockSize + 4096) // 4096   # the shards' pages, or more
+        while True:
+            out = {i: np.zeros(max(1, cap), dtype=np.uint64) for i in ids}
+            ptrs = (C.c_void_p * total)(*[out[i].ctypes.data if i in out else None for i in range(total)])
+            shard_len, n = C.c_int64(0), C.c_int64(0)
+            check(lib().swec_ec_volume_page_sketch(self._h, seed, ptrs, cap, C.byref(shard_len), C.byref(n)))
+            if n.value <= cap:
+                return {i: a[:n.value] for i, a in out.items()}, int(shard_len.value)
+            cap = n.value
+
+    def sketch_needle_damage(self, pages, shard_len: int, max_needles: int = 1 << 16) -> dict:
+        """Which live needles the pages flagged by Encoder.locate_sketch_damage[_checked] (their "pages" list, for
+        shards of shard_len bytes) hit, from the .ecx alone (swec_ec_volume_sketch_needle_damage): no local shard is
+        needed.  Returns "needles" (ascending id, the first max_needles of those with a non-zero count), "n_needles" and
+        "unowned" = [damaged, uncorrectable].  The counts are page-granular upper bounds (include/swec.h)."""
+        arr, n_pages = _sketch_pages(pages)
+        needles, n_needles, unowned = (NeedleDamage * max(1, max_needles))(), C.c_int(0), (C.c_uint64 * 2)()
+        check(lib().swec_ec_volume_sketch_needle_damage(self._h, shard_len, arr, n_pages, needles, max_needles,
+                                                        C.byref(n_needles), unowned))
+        return {"needles": _needle_damage(needles[:min(n_needles.value, max_needles)]), "n_needles": n_needles.value,
+                "unowned": [int(unowned[0]), int(unowned[1])]}
+
+    PageSketch, SketchNeedleDamage = page_sketch, sketch_needle_damage
 
     def close(self) -> None:
         h, self._h = getattr(self, "_h", None), None
