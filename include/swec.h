@@ -22,6 +22,7 @@
  *   swec_repair_ec_damage       (no counterpart) corrects the located bytes in place instead of rebuilding whole shards
  *   swec_rebuild_ec_files_checked  rebuildEcFiles reading every present shard (ec_encoder.go:342-357), which corrects
  *                               damage in the shards it rebuilds from instead of copying it into the rebuilt ones
+ *   swec_heal_ec_files          (no counterpart) the checked rebuild that also corrects the damaged present shards in place
  *   swec_page_sketch_file,      (no counterpart) ScrubEcVolume FULL checks only needle CRCs over the network
  *   swec_locate_sketch_damage   (weed/storage/store_ec_scrub.go); these check parity of a balanced volume from
  *                               8 bytes per 4 KiB page of every shard
@@ -35,6 +36,7 @@
  *   swec_write_dat_file         WriteDatFile              weed/storage/erasure_coding/ec_decoder.go:176-223
  *   swec_ec_shards_generate     VolumeEcShardsGenerate (file work)   weed/server/volume_grpc_erasure_coding.go:43-146
  *   swec_ec_shards_rebuild      VolumeEcShardsRebuild  (file work)   weed/server/volume_grpc_erasure_coding.go:149-225
+ *   swec_ec_shards_heal         the same through swec_heal_ec_files
  *   swec_ec_shards_to_volume    VolumeEcShardsToVolume (file work)   weed/server/volume_grpc_erasure_coding.go:578-668
  *   swec_ec_shards_to_volume_checked  the same from any k shards, correcting damaged data shards before the .dat is
  *                               written (swec_write_dat_file_checked, swec_decode_data_checked_device)
@@ -395,7 +397,8 @@ int swec_locate_needle_damage_device(swec_encoder *enc, const void *const *shard
  * with 4 lost nothing can be checked.  With nothing lost (c = m) the report is the one of swec_locate_ec_damage.
  * Present shards are never written, neither the files nor the device buffers.  To fix them, run swec_repair_ec_damage
  * (or swec_correct_damage_device) on the completed set afterwards: with every rebuilt column right, a column with one
- * damaged present shard is within radius 1 of the full code.
+ * damaged present shard is within radius 1 of the full code.  The heal calls below do both in one read, and never
+ * rewrite a column the checked rebuild reports as uncorrectable.
  * The report and ranges are those of the locate calls, over the present shards (a missing shard is never blamed);
  * with c = 0 the report has columns = 0 and no ranges.  Argument rules: report not NULL, ranges_cap not negative,
  * ranges not NULL when ranges_cap > 0, radius 0, 1 or 2 (SWEC_ERR_INVALID_ARG otherwise, before anything else).
@@ -414,6 +417,36 @@ int swec_rebuild_ec_files_checked(const char *base_file_name, const char *const 
 int swec_reconstruct_checked_device(swec_encoder *enc, void *const *shards, const uint8_t *present, size_t shard_len,
                                     int radius, swec_damage_report *report, swec_damage_range *ranges, int ranges_cap,
                                     int *n_ranges, void *stream);
+/* ---- heal: the checked rebuild that also corrects the present shards ------------------------------------------------
+ * The checked rebuild above, which also writes the errors it locates back into the present shards, in one decode of the
+ * code punctured to them (distance c+1, t = min(radius, floor(c/2))).  Per column:
+ *   - at most t wrong present shards: the whole column, present and rebuilt shards, becomes the true codeword;
+ *   - t+1 .. c-t wrong present shards: the column is counted as uncorrectable, its present bytes are left as they were,
+ *     and its rebuilt bytes are exactly what swec_rebuild_ec_files writes;
+ *   - more than c-t wrong present shards: the column can be MISCORRECTED, present bytes included, like the repair.
+ *   - radius 0, and c = 0: nothing is corrected; the present shards are left as they were.
+ * The checked rebuild followed by swec_repair_ec_damage reads the set twice and decodes the completed set with the full
+ * code, whose larger radius can rewrite a column the checked rebuild left uncorrectable (rebuilt from wrong present
+ * bytes) into a different codeword.  The heal leaves such a column as found.
+ * The report, the ranges and the rebuilt shards are byte for byte those of the checked rebuild for the same input, so
+ * shard_bytes[i] = the bytes corrected in present shard i; with nothing missing they are those of the repair at the same
+ * radius.  *ok = 1 iff c >= 1 and no column is uncorrectable.
+ * File level: the arguments, rules, errors, texts and order of swec_rebuild_ec_files_checked, whose pipeline is pass 1:
+ * the same reads and the same rebuilt files.  Pass 2 is swec_repair_ec_damage's: it reads again only the 4 KiB pages
+ * pass 1 flagged, from the information and check shards, corrects them on the GPU, and pwrites each blamed present
+ * shard's own flagged pages back to the file where the shard was found (O_DIRECT when "file_direct_io" bit 1 is set);
+ * every modified file is fdatasync'ed before the call returns.  Only blamed shards are opened for writing, so a set
+ * without damage, or with only uncorrectable columns, is never opened for writing.  Each byte is written once, so
+ * running the call again finishes a heal cut short.  On any failure no ids are reported and no rebuilt file is left.
+ * Device level: the argument rules of swec_reconstruct_checked_device; present buffers are written only at the blamed
+ * bytes of columns decoded within t, each 256 MiB piece right after the launch that takes the errors out of its rebuilt
+ * bytes; synchronises `stream`.                                                                                       */
+int swec_heal_ec_files(const char *base_file_name, const char *const *additional_dirs, int n_additional_dirs,
+                       int data_shards, int parity_shards, int device, int radius, uint32_t *rebuilt, int *n_rebuilt,
+                       swec_damage_report *report, swec_damage_range *ranges, int ranges_cap, int *n_ranges, int *ok);
+int swec_heal_device(swec_encoder *enc, void *const *shards, const uint8_t *present, size_t shard_len, int radius,
+                     swec_damage_report *report, swec_damage_range *ranges, int ranges_cap, int *n_ranges,
+                     void *stream);
 int swec_write_dat_file(const char *base_file_name, int64_t dat_file_size,
                         const char *const *shard_file_names, int data_shards,
                         int64_t large_block, int64_t small_block);
@@ -582,6 +615,12 @@ int swec_ec_shards_generate(const char *data_base_file_name, const char *index_b
 int swec_ec_shards_rebuild(const char *data_base_file_name, const char *index_base_file_name,
                            const char *const *additional_dirs, int n_additional_dirs, int device,
                            uint32_t *rebuilt, int *n_rebuilt);
+/* The same with swec_heal_ec_files in place of RebuildEcFiles: the lost shards rebuilt and the damaged present ones
+ * corrected in one read (see the heal above), then RebuildEcxFile.  Returns the heal's report, ranges and ok.       */
+int swec_ec_shards_heal(const char *data_base_file_name, const char *index_base_file_name,
+                        const char *const *additional_dirs, int n_additional_dirs, int device, int radius,
+                        uint32_t *rebuilt, int *n_rebuilt, swec_damage_report *report, swec_damage_range *ranges,
+                        int ranges_cap, int *n_ranges, int *ok);
 /* VolumeEcShardsToVolume (ec.decode): needs all data shards (data_base's directory, then
  * additional_dirs); RebuildEcxFile → HasLiveNeedles (SWEC_ERR_NO_LIVE_NEEDLES when none) →
  * FindDatFileSize → WriteDatFile → WriteIdxFileFromEcIndex.  No GPU work.  *dat_file_size may be NULL. */

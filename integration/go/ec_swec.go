@@ -857,6 +857,75 @@ func swecRebuildEcFilesChecked(baseFileName string, ctx *ECContext, additionalDi
 	return generated, details, nil
 }
 
+// swecHealEcFiles is swecRebuildEcFilesChecked that also corrects the damage it locates in the present shard files, in
+// the same full read plus a re-read of the flagged pages: the lost shards are rebuilt and the damaged present ones
+// repaired in place, where the checked rebuild followed by swecRepairEcDamage reads every shard twice.  Columns with
+// more wrong shards than the radius corrects are left as they were (details say where); the two-call flow could rewrite
+// such a column into a wrong codeword.  Only the blamed shards' flagged pages are rewritten, so nobody else may write
+// the shard files during the call.  generated are the rebuilt ids; details say what was corrected or left.
+func swecHealEcFiles(baseFileName string, ctx *ECContext, additionalDirs []string, radius int) (generated []uint32, details []string, err error) {
+	cs := C.CString(baseFileName)
+	defer C.free(unsafe.Pointer(cs))
+	dirs := make([]*C.char, len(additionalDirs)+1)
+	for i, d := range additionalDirs {
+		dirs[i] = C.CString(d)
+		defer C.free(unsafe.Pointer(dirs[i]))
+	}
+	var ids [C.SWEC_MAX_SHARDS]C.uint32_t
+	var report C.swec_damage_report
+	var nIds, nRanges, ok C.int
+	if err := swecCall(func() C.int {
+		return C.swec_heal_ec_files(cs, (**C.char)(unsafe.Pointer(&dirs[0])), C.int(len(additionalDirs)),
+			C.int(ctx.DataShards), C.int(ctx.ParityShards), swecPickDevice(), C.int(radius), &ids[0], &nIds, &report,
+			nil, 0, &nRanges, &ok)
+	}); err != nil {
+		return nil, nil, fmt.Errorf("heal ec files: %w", err)
+	}
+	generated, details = swecHealResult(ids[:nIds], &report)
+	return generated, details, nil
+}
+
+// ecShardsHealSwec is ecShardsRebuildSwec through swecHealEcFiles: RebuildEcFiles healing the present shards, then
+// RebuildEcxFile, in VolumeEcShardsRebuild (:149-225).  The ratio comes from .vif, else 10+4.
+func ecShardsHealSwec(dataBaseFileName, indexBaseFileName string, additionalDirs []string, radius int) (generated []uint32, details []string, err error) {
+	cd, ci := C.CString(dataBaseFileName), C.CString(indexBaseFileName)
+	defer C.free(unsafe.Pointer(cd))
+	defer C.free(unsafe.Pointer(ci))
+	dirs := make([]*C.char, len(additionalDirs)+1)
+	for i, d := range additionalDirs {
+		dirs[i] = C.CString(d)
+		defer C.free(unsafe.Pointer(dirs[i]))
+	}
+	var ids [C.SWEC_MAX_SHARDS]C.uint32_t
+	var report C.swec_damage_report
+	var nIds, nRanges, ok C.int
+	if err := swecCall(func() C.int {
+		return C.swec_ec_shards_heal(cd, ci, (**C.char)(unsafe.Pointer(&dirs[0])), C.int(len(additionalDirs)),
+			swecPickDevice(), C.int(radius), &ids[0], &nIds, &report, nil, 0, &nRanges, &ok)
+	}); err != nil {
+		return nil, nil, fmt.Errorf("heal ec shards: %w", err)
+	}
+	generated, details = swecHealResult(ids[:nIds], &report)
+	return generated, details, nil
+}
+
+func swecHealResult(ids []C.uint32_t, report *C.swec_damage_report) (generated []uint32, details []string) {
+	for _, id := range ids {
+		generated = append(generated, uint32(id))
+	}
+	for i := 0; i < C.SWEC_MAX_SHARDS; i++ {
+		if n := uint64(report.shard_bytes[i]); n > 0 {
+			details = append(details, fmt.Sprintf("ec shard %d: %d bytes corrected, offsets %d..%d",
+				i, n, int64(report.shard_first[i]), int64(report.shard_last[i])))
+		}
+	}
+	if report.uncorrectable_columns > 0 {
+		details = append(details, fmt.Sprintf("%d byte columns are damaged in more shards than can be corrected, left as they were and rebuilt from the shards as found, offsets %d..%d",
+			uint64(report.uncorrectable_columns), int64(report.first_uncorrectable), int64(report.last_uncorrectable)))
+	}
+	return generated, details
+}
+
 // ---- pinned batch buffers ---------------------------------------------------------------------------------
 // runtime.Pinner only stops the Go GC from moving a slice; to CUDA such memory is PAGEABLE, so every Encode /
 // Reconstruct on it bounces through the library's pinned ring (a memcpy per shard each way).  The batch buffers of

@@ -142,6 +142,11 @@ PROTOTYPES = {
     "swec_decode_data_checked_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int,
                                                   C.POINTER(DamageReport), C.POINTER(DamageRange), C.c_int,
                                                   C.POINTER(C.c_int), C.c_void_p]),
+    "swec_heal_ec_files": (C.c_int, [C.c_char_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                     C.POINTER(C.c_int), C.POINTER(DamageReport), C.POINTER(DamageRange), C.c_int,
+                                     C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "swec_heal_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.POINTER(DamageReport),
+                                   C.POINTER(DamageRange), C.c_int, C.POINTER(C.c_int), C.c_void_p]),
     "swec_page_sketch_device": (C.c_int, [C.c_int, C.c_void_p, C.c_size_t, C.c_uint64, C.c_uint64, C.c_void_p,
                                           C.c_void_p]),
     "swec_page_sketch_file": (C.c_int, [C.c_char_p, C.c_int, C.c_uint64, C.c_void_p, C.c_int64, C.POINTER(C.c_int64),
@@ -166,6 +171,9 @@ PROTOTYPES = {
     "swec_ec_shards_generate": (C.c_int, [C.c_char_p, C.c_char_p, C.c_uint32, C.c_uint64, C.c_int]),
     "swec_ec_shards_rebuild": (C.c_int, [C.c_char_p, C.c_char_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
                                          C.POINTER(C.c_int)]),
+    "swec_ec_shards_heal": (C.c_int, [C.c_char_p, C.c_char_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                      C.POINTER(C.c_int), C.POINTER(DamageReport), C.POINTER(DamageRange), C.c_int,
+                                      C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "swec_ec_shards_to_volume": (C.c_int, [C.c_char_p, C.c_char_p, C.c_void_p, C.c_int, C.POINTER(C.c_int64)]),
     "swec_ec_shards_to_volume_checked": (C.c_int, [C.c_char_p, C.c_char_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
                                                    C.POINTER(C.c_int64), C.POINTER(DamageReport), C.POINTER(DamageRange),

@@ -578,20 +578,30 @@ int submit_flagged(FilePipeline& pipe, const std::vector<swec_damage_range>& run
     return pipe.finish();
 }
 
+// 0, 1, .. n-1: the streams of a pipeline over every shard of the set, in shard order
+std::vector<int> all_shard_ids(size_t n) {
+    std::vector<int> ids(n);
+    for (size_t i = 0; i < n; i++) ids[i] = int(i);
+    return ids;
+}
+
 // The writes of the repairs' pass 2: each blamed shard gets back only its own pages of pass 1's `runs`, through out[i]
-// (out_d[i]: its O_DIRECT twin, -1 = none), which the caller opens for the blamed shards alone.
+// (out_d[i]: its O_DIRECT twin, -1 = none), which the caller opens for the blamed shards alone.  Stream i of the
+// pipeline holds shard ids[i]; `runs` name shard ids.
 class PageWrites {
   public:
     std::vector<int> out, out_d;
 
-    PageWrites(const std::vector<swec_damage_range>& runs, int total)
-        : out(size_t(total), -1), out_d(size_t(total), -1), runs_(runs), next_(size_t(total), 0), stop_(size_t(total), 0) {
+    PageWrites(const std::vector<swec_damage_range>& runs, const std::vector<int>& ids)
+        : out(ids.size(), -1), out_d(ids.size(), -1), runs_(runs), ids_(ids), next_(ids.size(), 0), stop_(ids.size(), 0) {
+        std::vector<int> stream(SWEC_MAX_SHARDS, -1);
+        for (size_t i = 0; i < ids.size(); i++) stream[size_t(ids[i])] = int(i);
         // each shard's slice of `runs`, which lists them shard by shard in ascending offset; an empty one: not blamed
         for (size_t r = runs.size(); r-- > 0;)
             if (runs[r].shard_id >= 0) {
-                const size_t id = size_t(runs[r].shard_id);
-                if (!stop_[id]) stop_[id] = r + 1;
-                next_[id] = r;
+                const size_t i = size_t(stream[size_t(runs[r].shard_id)]);
+                if (!stop_[i]) stop_[i] = r + 1;
+                next_[i] = r;
             }
     }
     bool blamed(int i) const { return stop_[size_t(i)] > 0; }
@@ -611,29 +621,32 @@ class PageWrites {
     // every modified file made durable; `base` + the shard's extension names a failing one
     int sync(const std::string& base) const {
         for (size_t i = 0; i < out.size(); i++)
-            if (out[i] >= 0 && fdatasync(out[i]) != 0) return io_fail("fdatasync " + base + shard_ext(int(i)));
+            if (out[i] >= 0 && fdatasync(out[i]) != 0) return io_fail("fdatasync " + base + shard_ext(ids_[i]));
         return SWEC_OK;
     }
 
   private:
     const std::vector<swec_damage_range>& runs_;
+    const std::vector<int>& ids_;
     std::vector<size_t> next_, stop_;
 };
 
-// Pass 2 of swec_repair_ec_damage.  `runs` are every page run pass 1 found, of the blamed shards and of the
-// uncorrectable columns.  Only the columns of those pages go through the pipeline again, with a correcting locator, and
-// the report and ranges are collected from that.  Each blamed shard gets back only its own pages, in the file where it
-// was found, made durable before the call returns.
+// Pass 2 of swec_repair_ec_damage and swec_heal_ec_files.  `runs` are every page run pass 1 found, of the blamed shards
+// and of the uncorrectable columns.  Only the columns of those pages go through the pipeline again, with a correcting
+// locator over the code whose check rows are `rows`: stream i is shard ids[i], read through in[i].  `out` (may be NULL:
+// the caller keeps pass 1's report) receives the report and ranges of that locator.  Each blamed shard gets back only
+// its own pages, in the file where it was found, made durable before the call returns; `name` names the pipeline's
+// SWEC_PIPE_STATS line.
 int repair_pages(swec_encoder* enc, const Matrix& rows, const std::string& b, const char* const* dirs, int ndirs,
-                 const std::vector<int>& in, int64_t size, int radius, const std::vector<swec_damage_range>& runs,
-                 const DamageOut& out) {
+                 const std::vector<int>& in, const std::vector<int>& ids, int64_t size, int radius,
+                 const std::vector<swec_damage_range>& runs, const char* name, const DamageOut* out) {
     const int total = int(in.size());
-    PageWrites writes(runs, total);
+    PageWrites writes(runs, ids);
     FdSet fds;
     const long direct = g_opt_file_direct_io.load();
     std::vector<int> in_d(static_cast<size_t>(total), -1);
     for (int i = 0; i < total; i++) {
-        const std::string path = find_shard_file(b, dirs, ndirs, i);
+        const std::string path = find_shard_file(b, dirs, ndirs, ids[size_t(i)]);
         in_d[size_t(i)] = fds.keep(open_direct(path, O_RDONLY, direct & 1));
         if (!writes.blamed(i)) continue;
         if ((writes.out[size_t(i)] = fds.keep(open(path.c_str(), O_RDWR))) < 0) return io_fail("open " + path);
@@ -646,9 +659,9 @@ int repair_pages(swec_encoder* enc, const Matrix& rows, const std::string& b, co
     if (rc) return rc;
     if ((rc = locator.init(rows, size, radius, enc->stream, /*correct=*/true))) return rc;
     if ((rc = submit_flagged(pipe, runs, chunk, in, in_d, [&](Item& it) { writes.add(it); }))) return rc;
-    pipe.report("repair_ec_damage");
+    pipe.report(name);
     if ((rc = writes.sync(b))) return rc;
-    return locator.collect(out);
+    return out ? locator.collect(*out) : SWEC_OK;
 }
 
 // Pass 1 of the damage calls, swec_locate_ec_damage itself: every column of the k+m shard files `in`, all `size` bytes,
@@ -687,7 +700,8 @@ int damage_files(const char* base, const char* const* dirs, int ndirs, int k, in
     std::vector<swec_damage_range> runs;
     if ((rc = locate_pass(enc.get(), rows, in, size, radius, out, repair ? &runs : nullptr))) return rc;
     if (repair && out.report->damaged_columns &&
-        (rc = repair_pages(enc.get(), rows, b, dirs, ndirs, in, size, radius, runs, out)))
+        (rc = repair_pages(enc.get(), rows, b, dirs, ndirs, in, all_shard_ids(in.size()), size, radius, runs,
+                           "repair_ec_damage", &out)))
         return rc;
     *ok = (repair ? out.report->uncorrectable_columns : out.report->damaged_columns) == 0 ? 1 : 0;
     return SWEC_OK;
@@ -742,10 +756,12 @@ int walk_items(const StripeGeometry& g, size_t chunk, int64_t tail_width, const 
 // and c check streams at their plan positions.  Per slot: one apply of plan.fused (the check shards re-encoded, the
 // missing shards rebuilt), then, with c >= 1, the rebuilding or decoding locator, which compares the c check rows with
 // the stored ones and corrects the errors it locates in the information set.  With c = 0 (exactly k shards present)
-// the set is rebuilt and the report says nothing was checked.
+// the set is rebuilt and the report says nothing was checked.  `runs` (may be NULL) receives every page run; `name`
+// (may be NULL) names the pipeline's SWEC_PIPE_STATS line.
 int checked_pipeline(swec_encoder* enc, const CheckedPlan& plan, const std::vector<int>& in, const std::vector<int>& in_d,
                      int64_t cols, const std::vector<int>& reserve, int64_t reserve_size, int radius, DamageOut* chk,
-                     const std::function<int(size_t chunk, const SubmitFn& submit)>& walk) {
+                     const std::function<int(size_t chunk, const SubmitFn& submit)>& walk,
+                     std::vector<swec_damage_range>* runs = nullptr, const char* name = nullptr) {
     const int k = enc->k, c = plan.c();
     const size_t chunk = file_chunk(cols);
     DamageLocator locator;
@@ -763,20 +779,22 @@ int checked_pipeline(swec_encoder* enc, const CheckedPlan& plan, const std::vect
         return pipe.submit(std::move(it));
     });  // a failed submit ends the walk, and finish() returns its error
     if ((rc = pipe.finish())) return rc;
+    if (name) pipe.report(name);
     if (c == 0) {
         chk->unchecked();
         return SWEC_OK;
     }
-    if ((rc = locator.collect(*chk))) return rc;
+    if ((rc = locator.collect(*chk, runs))) return rc;
     chk->checked = true;
     return SWEC_OK;
 }
 
 // The checked rebuild: every present shard is read, as the check shards of the punctured code beyond the first k, and
-// the rebuilt shards are written to `out` (in ascending id of the missing shards).
+// the rebuilt shards are written to `out` (in ascending id of the missing shards).  `runs` and `name`: checked_pipeline's.
 int rebuild_checked(swec_encoder* enc, const std::vector<int>& in, const std::vector<int>& in_d,
                     const std::vector<uint8_t>& present, const std::vector<int>& out, const std::vector<int>& out_d,
-                    int64_t todo, int radius, DamageOut* chk) {
+                    int64_t todo, int radius, DamageOut* chk, std::vector<swec_damage_range>* runs = nullptr,
+                    const char* name = nullptr) {
     CheckedPlan plan;
     if (!plan.build(enc->gen, enc->k, present.data(), /*decode=*/false)) return fail(SWEC_ERR_TOO_FEW_SHARDS, "not enough shards");
     return checked_pipeline(enc, plan, in, in_d, todo, out, todo, radius, chk, [&](size_t chunk, const SubmitFn& submit) {
@@ -789,14 +807,31 @@ int rebuild_checked(swec_encoder* enc, const std::vector<int>& in, const std::ve
             rc = submit(std::move(it), o);
         }
         return rc;
-    });
+    }, runs, name);
+}
+
+// Pass 2 of swec_heal_ec_files.  Pass 1, the checked rebuild, located the damage of the present shards over the code
+// punctured to them, and its `runs` flagged the pages.  Those pages are read again from the information and check
+// shards and corrected by the correcting locator over P': the punctured code is systematic, so that is the heal of a set
+// with nothing to rebuild, and it blames what pass 1 blamed.  Nothing to write (no damage, or only uncorrectable
+// columns): nothing is read or opened for writing.
+int heal_pages(swec_encoder* enc, const std::string& b, const char* const* dirs, int ndirs, const std::vector<int>& in,
+               const std::vector<uint8_t>& present, int64_t size, int radius, const std::vector<swec_damage_range>& runs,
+               const DamageOut& chk) {
+    if (!chk.checked || chk.report->damaged_columns == chk.report->uncorrectable_columns) return SWEC_OK;
+    CheckedPlan plan;
+    if (!plan.build(enc->gen, enc->k, present.data(), /*decode=*/false)) return fail(SWEC_ERR_TOO_FEW_SHARDS, "not enough shards");
+    std::vector<int> ids = plan.info, fds;
+    for (int i = 0; i < plan.c(); i++) ids.push_back(plan.check(i));
+    for (int id : ids) fds.push_back(in[size_t(id)]);
+    return repair_pages(enc, plan.checks(), b, dirs, ndirs, fds, ids, size, plan.radius(radius), runs, "heal_pages", nullptr);
 }
 
 // swec_rebuild_ec_files, and with `chk` swec_rebuild_ec_files_checked at `radius`: the same files, checks, errors and order.  The
 // checked rebuild reads every present shard, not only the first k, and corrects the damage it locates in the first k
-// before it reaches the rebuilt shards.
+// before it reaches the rebuilt shards.  With `heal` too, swec_heal_ec_files: the checked rebuild, then heal_pages.
 int rebuild_files(const char* base, const char* const* dirs, int ndirs, int k, int m, int device, uint32_t* rebuilt,
-                  int* n_rebuilt, int radius, DamageOut* chk) {
+                  int* n_rebuilt, int radius, DamageOut* chk, bool heal = false) {
     if (!base || !rebuilt || !n_rebuilt || (ndirs > 0 && !dirs)) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
     *n_rebuilt = 0;
     const std::string b(base);
@@ -859,8 +894,11 @@ int rebuild_files(const char* base, const char* const* dirs, int ndirs, int k, i
     const bool ragged = !missing.empty() && size > mib && size % mib != 0;
     const int64_t todo = ragged ? size / mib * mib : size;
 
+    std::vector<swec_damage_range> runs;
     if (chk) {
-        if ((rc = rebuild_checked(enc.get(), in, in_d, present, out, out_d, todo, radius, chk))) return rc;
+        if ((rc = rebuild_checked(enc.get(), in, in_d, present, out, out_d, todo, radius, chk, heal ? &runs : nullptr,
+                                  heal ? "heal_ec_files" : nullptr)))
+            return rc;
     } else {
         std::vector<int> ins, outs_idx;  // outs_idx == missing: fused row r rebuilds the shard of out[r]
         Matrix fused;
@@ -880,8 +918,23 @@ int rebuild_files(const char* base, const char* const* dirs, int ndirs, int k, i
         if ((rc = pipe.finish())) return rc;
     }
     if (ragged) return shard_size_error(mib, size % mib);
+    if (heal && (rc = heal_pages(enc.get(), b, dirs, ndirs, in, present, todo, radius, runs, *chk))) return rc;
     undo.armed = false;
     return SWEC_OK;
+}
+
+// swec_rebuild_ec_files_checked, and with `heal` swec_heal_ec_files: the same arguments, rules and pass 1
+int checked_files(const char* base, const char* const* dirs, int ndirs, int k, int m, int device, int radius,
+                  uint32_t* rebuilt, int* n_rebuilt, const DamageOut& out, int* ok, bool heal) {
+    if (!base || !rebuilt || !n_rebuilt || !ok || (ndirs > 0 && !dirs)) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
+    *ok = 0;
+    *n_rebuilt = 0;
+    DamageOut chk = out;
+    int rc;
+    if ((rc = chk.check()) || (rc = check_radius(radius, 0))) return rc;
+    rc = rebuild_files(base, dirs, ndirs, k, m, device, rebuilt, n_rebuilt, radius, &chk, heal);
+    *ok = rc == SWEC_OK && chk.checked && chk.report->uncorrectable_columns == 0 ? 1 : 0;
+    return rc;
 }
 
 // The checked decode over columns [0, cols) of the shards, in the items of walk_items() with the tail row as wide as
@@ -924,7 +977,8 @@ int needle_damage_files(swec_encoder* enc, const std::vector<int>& in, int64_t s
     int rc = locate_pass(enc, rows, in, size, radius, out, &runs);
     if (rc || out.report->damaged_columns == 0) return rc;
     const int k = enc->k;
-    PageWrites writes(runs, int(in.size()));
+    const std::vector<int> ids = all_shard_ids(in.size());
+    PageWrites writes(runs, ids);
     FdSet fds;
     const long direct = g_opt_file_direct_io.load();
     for (int i = 0; repair && i < int(in.size()); i++) {
@@ -1092,15 +1146,15 @@ int swec_rebuild_ec_files(const char* base, const char* const* dirs, int ndirs, 
 int swec_rebuild_ec_files_checked(const char* base, const char* const* dirs, int ndirs, int k, int m, int device,
                                   int radius, uint32_t* rebuilt, int* n_rebuilt, swec_damage_report* report,
                                   swec_damage_range* ranges, int ranges_cap, int* n_ranges, int* ok) {
-    if (!base || !rebuilt || !n_rebuilt || !ok || (ndirs > 0 && !dirs)) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
-    *ok = 0;
-    *n_rebuilt = 0;
-    DamageOut chk{report, ranges, ranges_cap, n_ranges};
-    int rc;
-    if ((rc = chk.check()) || (rc = check_radius(radius, 0))) return rc;
-    rc = rebuild_files(base, dirs, ndirs, k, m, device, rebuilt, n_rebuilt, radius, &chk);
-    *ok = rc == SWEC_OK && chk.checked && report->uncorrectable_columns == 0 ? 1 : 0;
-    return rc;
+    return checked_files(base, dirs, ndirs, k, m, device, radius, rebuilt, n_rebuilt, {report, ranges, ranges_cap, n_ranges},
+                         ok, false);
+}
+
+int swec_heal_ec_files(const char* base, const char* const* dirs, int ndirs, int k, int m, int device, int radius,
+                       uint32_t* rebuilt, int* n_rebuilt, swec_damage_report* report, swec_damage_range* ranges,
+                       int ranges_cap, int* n_ranges, int* ok) {
+    return checked_files(base, dirs, ndirs, k, m, device, radius, rebuilt, n_rebuilt, {report, ranges, ranges_cap, n_ranges},
+                         ok, true);
 }
 
 int swec_verify_ec_files(const char* base, const char* const* dirs, int ndirs, int k, int m, int device,

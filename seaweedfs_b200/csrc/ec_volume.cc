@@ -2,6 +2,7 @@
 // drive the RS path (SURVEY §8f row 1), as single C-ABI calls:
 //   swec_ec_shards_generate    VolumeEcShardsGenerate   weed/server/volume_grpc_erasure_coding.go:43-146
 //   swec_ec_shards_rebuild     VolumeEcShardsRebuild    weed/server/volume_grpc_erasure_coding.go:149-225
+//   swec_ec_shards_heal        the same, rebuilding through swec_heal_ec_files: the damaged present shards corrected too
 //   swec_ec_shards_to_volume   VolumeEcShardsToVolume   weed/server/volume_grpc_erasure_coding.go:578-668
 //   swec_ec_shards_to_volume_checked   the same from any k shards, damaged data shards corrected on the GPU first
 //   swec_read_ec_needles       Store.ReadEcShardNeedle + readEcShardIntervals + readOneEcShardInterval +
@@ -113,6 +114,16 @@ int swec_ec_shards_rebuild(const char* data_base, const char* index_base, const 
     int rc = swec_rebuild_ec_files(data_base, additional_dirs, n_additional_dirs, 0, 0, device, rebuilt, n_rebuilt);
     if (rc) return rc;
     // RebuildEcxFile on the index base, falling back to the data directory (:211-217)
+    return swec_rebuild_ecx_file(index_base_of(data_base, index_base, true).c_str());
+}
+
+int swec_ec_shards_heal(const char* data_base, const char* index_base, const char* const* additional_dirs,
+                        int n_additional_dirs, int device, int radius, uint32_t* rebuilt, int* n_rebuilt,
+                        swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges, int* ok) {
+    if (!data_base || !rebuilt || !n_rebuilt) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
+    int rc = swec_heal_ec_files(data_base, additional_dirs, n_additional_dirs, 0, 0, device, radius, rebuilt, n_rebuilt,
+                                report, ranges, ranges_cap, n_ranges, ok);
+    if (rc) return rc;
     return swec_rebuild_ecx_file(index_base_of(data_base, index_base, true).c_str());
 }
 

@@ -772,9 +772,11 @@ namespace {
 // The device-level damage and checked calls: per piece, one apply of plan.fused from the information shards, the check
 // rows into scratch and the rebuilt rows into the caller's buffers, then (c >= 1) the initialised locator; returns once
 // the stream is done.  The computed check rows go to scratch a piece at a time: a 3 GiB shard set needs 1 GiB of it,
-// not 12 GiB.  A data byte corrected in a piece has already been encoded, and no later piece reads it.
+// not 12 GiB.  A data byte corrected in a piece has already been encoded, and no later piece reads it.  `fixer` (may be
+// NULL): a correcting locator over plan.checks() that runs on each piece after `locator`, correcting the information and
+// check shards in place.
 int locate_pieces(swec_encoder* e, const CheckedPlan& plan, uint8_t* const* sh, size_t n, DamageLocator& locator,
-                  cudaStream_t s) {
+                  cudaStream_t s, DamageLocator* fixer = nullptr) {
     const int k = e->k, c = plan.c();
     const size_t piece = std::min(n, size_t(256) << 20);
     StreamScratch scratch(s);
@@ -792,6 +794,11 @@ int locate_pieces(swec_encoder* e, const CheckedPlan& plan, uint8_t* const* sh, 
         for (int o : plan.rebuilt_rows) comp[o] = sh[plan.outs[size_t(o)]] + off;
         int rc = e->apply(plan.fused, in, comp, len, Layout{}, s);
         if (rc == SWEC_OK && c > 0) rc = locator.launch(comp, at, len, int64_t(off), s);
+        if (rc == SWEC_OK && fixer) {
+            uint8_t* checks[SWEC_MAX_SHARDS];  // the computed check rows, in check order
+            for (int i = 0; i < c; i++) checks[i] = comp[plan.check_rows[size_t(i)]];
+            rc = fixer->launch(checks, at, len, int64_t(off), s);
+        }
         if (rc) return rc;
     }
     SWEC_CUDA(cudaStreamSynchronize(s));
@@ -840,9 +847,11 @@ namespace {
 // shards are rebuilt into the caller's buffers by the same apply, then cleared of the errors the locator finds in the
 // information set.  The rebuild reads every present shard and rebuilds every missing one.  The decode rebuilds only the
 // missing data shards and also corrects the present data shards in place; parity shards are only read, and a missing
-// one needs no buffer.
+// one needs no buffer.  The heal (swec_heal_device, `heal`) is the rebuild that also corrects every present shard in
+// place: after the rebuilding locator, each piece goes through a correcting locator over P', which decodes the same
+// syndromes at the same radius and so writes back exactly the errors the report blames.  Its own report is dropped.
 int checked_device(swec_encoder* e, void* const* shards, const uint8_t* present, size_t n, int radius, bool decode,
-                   const DamageOut& out, void* stream) {
+                   const DamageOut& out, void* stream, bool heal = false) {
     if (!e || !shards || !present) return fail(SWEC_ERR_INVALID_ARG, "NULL argument");
     int rc;
     if ((rc = out.check()) || (rc = check_radius(radius, 0))) return rc;
@@ -857,7 +866,11 @@ int checked_device(swec_encoder* e, void* const* shards, const uint8_t* present,
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     DamageLocator locator;
     if (plan.c() > 0 && (rc = locator.init_rebuild(plan, int64_t(n), radius, s))) return rc;
-    if ((rc = locate_pieces(e, plan, reinterpret_cast<uint8_t* const*>(shards), n, locator, s))) return rc;
+    DamageLocator fixer;  // radius 0 decodes nothing, so it corrects nothing
+    const bool fix = heal && plan.radius(radius) > 0;
+    if (fix && (rc = fixer.init(plan.checks(), int64_t(n), plan.radius(radius), s, /*correct=*/true))) return rc;
+    if ((rc = locate_pieces(e, plan, reinterpret_cast<uint8_t* const*>(shards), n, locator, s, fix ? &fixer : nullptr)))
+        return rc;
     if (plan.c() == 0) {  // every present shard is an information shard: nothing to check
         out.unchecked();
         return SWEC_OK;
@@ -879,6 +892,11 @@ int swec_decode_data_checked_device(swec_encoder* e, void* const* shards, const 
                                     swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges,
                                     void* stream) {
     return checked_device(e, shards, present, n, radius, true, {report, ranges, ranges_cap, n_ranges}, stream);
+}
+
+int swec_heal_device(swec_encoder* e, void* const* shards, const uint8_t* present, size_t n, int radius,
+                     swec_damage_report* report, swec_damage_range* ranges, int ranges_cap, int* n_ranges, void* stream) {
+    return checked_device(e, shards, present, n, radius, false, {report, ranges, ranges_cap, n_ranges}, stream, true);
 }
 
 int swec_stream_synchronize(swec_encoder* e, void* stream) {

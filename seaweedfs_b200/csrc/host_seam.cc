@@ -177,6 +177,20 @@ bool constant_pitch(const uint8_t* const* p, int n, size_t min_pitch, size_t* pi
     return true;
 }
 
+// `rows` rows of `len` bytes, `spitch` apart at src, to `dpitch` apart at dst: one strided DMA.  Equally spaced caller
+// buffers are usually slices of one allocation (constant_pitch), but separate pinned allocations can land equally spaced
+// too, and the runtime refuses a strided copy whose span is not one pinned range with cudaErrorInvalidValue, before
+// anything is queued: then each row goes as a copy of its own.
+cudaError_t copy_rows(uint8_t* dst, size_t dpitch, const uint8_t* src, size_t spitch, size_t len, size_t rows,
+                      cudaStream_t s) {
+    cudaError_t e = cudaMemcpy2DAsync(dst, dpitch, src, spitch, len, rows, cudaMemcpyDefault, s);
+    if (e != cudaErrorInvalidValue) return e;
+    cudaGetLastError();
+    e = cudaSuccess;
+    for (size_t r = 0; r < rows && e == cudaSuccess; r++) e = cudaMemcpyAsync(dst + r * dpitch, src + r * spitch, len, cudaMemcpyDefault, s);
+    return e;
+}
+
 }  // namespace
 
 int apply_host(swec_encoder_impl* e, const Matrix& rows, const uint8_t* const* in, uint8_t* const* out, size_t n,
@@ -249,7 +263,7 @@ int apply_host(swec_encoder_impl* e, const Matrix& rows, const uint8_t* const* i
             for (int i = 0; i < K; i++) din[i] = s.dev + size_t(i) * pitch;
             for (int r = 0; r < R; r++) dout[r] = s.dev + size_t(K + r) * pitch;
             if (in_2d) {
-                SWEC_CUDA(cudaMemcpy2DAsync(s.dev, pitch, in[0] + off, in_pitch, len, size_t(K), cudaMemcpyDefault, s.stream));
+                SWEC_CUDA(copy_rows(s.dev, pitch, in[0] + off, in_pitch, len, size_t(K), s.stream));
             } else {
                 for (int i = 0; i < K; i++) {
                     const uint8_t* src = b.direct[i] ? in[i] + off : s.host + size_t(i) * pitch;
@@ -258,7 +272,7 @@ int apply_host(swec_encoder_impl* e, const Matrix& rows, const uint8_t* const* i
             }
             if (const int rc2 = e->apply(rows, din, dout, len, Layout{}, s.stream)) return rc2;
             if (out_2d) {
-                SWEC_CUDA(cudaMemcpy2DAsync(out[0] + off, out_pitch, dout[0], pitch, len, size_t(R), cudaMemcpyDefault, s.stream));
+                SWEC_CUDA(copy_rows(out[0] + off, out_pitch, dout[0], pitch, len, size_t(R), s.stream));
             } else {
                 if (check) {  // bring the caller's copy of every row next to the computed one and compare in HBM
                     bounce.clear();

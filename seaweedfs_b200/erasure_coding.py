@@ -233,6 +233,15 @@ class Encoder:
                                                     *out.args, stream))
         return out.result()
 
+    def heal_device(self, shard_ptrs, present, shard_len: int, radius: int = 1, max_ranges: int = 4096,
+                    stream: int = 0) -> dict:
+        """reconstruct_checked_device that also corrects the damage it locates in the present shards, in place
+        (swec_heal_device): columns within the radius become the true codeword, uncorrectable ones keep their present
+        bytes.  Returns the report of reconstruct_checked_device for the same shards (include/swec.h)."""
+        pres, out = np.ascontiguousarray(np.asarray(present, dtype=np.uint8)), _DamageOut(max_ranges)
+        check(lib().swec_heal_device(self._h, _ptrs(shard_ptrs), pres.ctypes.data, shard_len, radius, *out.args, stream))
+        return out.result()
+
     def page_sketch_device(self, shard_ptr: int, shard_len: int, sketches_ptr: int, seed: int, first_column: int = 0,
                            stream: int = 0) -> None:
         """The page sketches (include/swec.h, SWEC_PAGE_SKETCH_VERSION) of shard_len bytes of one shard in device
@@ -510,6 +519,19 @@ def rebuild_ec_files_checked(base_file_name: str, additional_dirs: list[str] | N
     return {"rebuilt": list(ids[: n_ids.value]), "ok": bool(ok.value), **out.result()}
 
 
+def heal_ec_files(base_file_name: str, additional_dirs: list[str] | None = None, ctx: ECContext | None = None,
+                  device: int = 0, radius: int = 1, max_ranges: int = 4096) -> dict:
+    """rebuild_ec_files_checked that also corrects the damage it locates in the present shard files, in one full read
+    (swec_heal_ec_files): only the blamed shards' flagged pages are rewritten, and uncorrectable columns are left as
+    found.  Returns what rebuild_ec_files_checked returns for the same files (include/swec.h)."""
+    arr, nd = _dirs(additional_dirs)
+    ids, n_ids = (C.c_uint32 * MaxShardCount)(), C.c_int(0)
+    out, ok = _DamageOut(max_ranges), C.c_int(0)
+    check(lib().swec_heal_ec_files(base_file_name.encode(), arr, nd, *_code(ctx, device), radius, ids, C.byref(n_ids),
+                                   *out.args, C.byref(ok)))
+    return {"rebuilt": list(ids[: n_ids.value]), "ok": bool(ok.value), **out.result()}
+
+
 def _check_decoded(status: int, out: _DamageOut) -> None:
     """check(), but a SWEC_ERR_UNCORRECTABLE error carries the report as .report"""
     if STATUS.get(status) == "SWEC_ERR_UNCORRECTABLE":
@@ -570,6 +592,19 @@ def volume_ec_shards_rebuild(data_base_file_name: str, index_base_file_name: str
     check(lib().swec_ec_shards_rebuild(data_base_file_name.encode(), (index_base_file_name or "").encode(),
                                        arr, n, device, ids, C.byref(cnt)))
     return list(ids[: cnt.value])
+
+
+def volume_ec_shards_heal(data_base_file_name: str, index_base_file_name: str | None = None,
+                          additional_dirs: list[str] | None = None, device: int = 0, radius: int = 1,
+                          max_ranges: int = 4096) -> dict:
+    """volume_ec_shards_rebuild through heal_ec_files (swec_ec_shards_heal): the lost shards rebuilt and the damaged
+    present ones corrected, then RebuildEcxFile.  Returns what heal_ec_files returns."""
+    arr, nd = _dirs(additional_dirs)
+    ids, n_ids = (C.c_uint32 * MaxShardCount)(), C.c_int(0)
+    out, ok = _DamageOut(max_ranges), C.c_int(0)
+    check(lib().swec_ec_shards_heal(data_base_file_name.encode(), (index_base_file_name or "").encode(), arr, nd, device,
+                                    radius, ids, C.byref(n_ids), *out.args, C.byref(ok)))
+    return {"rebuilt": list(ids[: n_ids.value]), "ok": bool(ok.value), **out.result()}
 
 
 def volume_ec_shards_to_volume(data_base_file_name: str, index_base_file_name: str | None = None,
